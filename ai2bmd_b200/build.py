@@ -1,4 +1,4 @@
-"""In-tree build of the CUDA extension (nvcc, sm_100a only).  No JIT cache, no torch extension loader:
+"""In-tree build of the CUDA extension (nvcc, sm_90a only).  No JIT cache, no torch extension loader:
 the product is a plain C-ABI shared library, ``ai2bmd_b200/_lib/libvisnet_b200.so``."""
 from __future__ import annotations
 
@@ -9,7 +9,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, "csrc")
 LIB_DIR = os.path.join(_HERE, "_lib")
 LIB_PATH = os.path.join(LIB_DIR, "libvisnet_b200.so")
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
 
 

@@ -1,4 +1,4 @@
-"""The reference's Calculator surface over the B200 engine.
+"""The reference's Calculator surface over the H100 engine.
 
 Mirrors, name for name, the classes of ``/root/reference/src/Calculators`` that sit on the hot path:
 
@@ -27,14 +27,14 @@ from .weights import load_state_dict
 
 def _device_index(device: str) -> int:
     if device == "cpu":
-        raise RuntimeError("the B200 engine has no CPU path (device='cpu' requested)")
+        raise RuntimeError("the engine has no CPU path (device='cpu' requested)")
     if not device.startswith("cuda"):
         raise ValueError(f"Unrecognized device {device!r}")   # device_strategy.py:24-35
     return int(device.split(":")[1]) if ":" in device else 0
 
 
 class ViSNetModel:
-    """Energy and forces of a packed fragment batch with the ViSNet potential on one B200."""
+    """Energy and forces of a packed fragment batch with the ViSNet potential on one H100."""
 
     implemented_properties = ["energy", "forces"]
 

@@ -1,4 +1,4 @@
-// Shared device helpers for the ViSNet sm_100a engine.
+// Shared device helpers for the ViSNet sm_90a engine.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -13,8 +13,7 @@ constexpr int KNB = 32;       // neighbour slots per atom (incl. self)
 constexpr int LDS_PAD = 4;    // smem row padding (floats) keeps rows 16 B aligned
 
 // Activations use the hardware exp2 / reciprocal (MUFU.EX2, MUFU.RCP): ~1e-6 relative error, far inside the stated
-// force tolerance; the IEEE expf + division they replace were a third of the edge-stage stall samples
-// (profiles/r01b_edge_bwd_tc_c4_full.txt).
+// force tolerance, and cheaper than the IEEE expf + division in the latency-bound edge stages.
 __device__ __forceinline__ float sigmoidf_(float x) { return __fdividef(1.0f, 1.0f + __expf(-x)); }
 __device__ __forceinline__ float silu_(float x) { return __fdividef(x, 1.0f + __expf(-x)); }
 // d/dx [x*sigmoid(x)] = s*(1 + x*(1-s))

@@ -1,4 +1,4 @@
-// Host side of the ViSNet sm_100a engine: workspace, launch sequence, CUDA-graph replay, C ABI.
+// Host side of the ViSNet sm_90a engine: workspace, launch sequence, CUDA-graph replay, C ABI.
 // See include/visnet_b200.h for the boundary each entry point replaces in the reference.
 #include <cuda_runtime.h>
 
@@ -122,7 +122,7 @@ struct StepIO {
 
 struct vb_handle {
     int device = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     std::string err;
     std::mutex mu;
     // weights
@@ -160,7 +160,7 @@ struct vb_handle {
     int use_graph = 1, npw = 0, te_fwd = 0, te_bwd = 32;
     int use_pdl = 0;   // programmatic dependent launch between the stages: measured neutral to slower (DESIGN.md section 5)
     int npw_opt = 0, te_fwd_opt = 0, edge_tc_opt = -1;   // user choices (0 / -1 = choose by problem size)
-    int tc_rows_opt = 0, tc_rows = 128;                  // kernel variant: capacity of a tcgen05 tile (32 / 64 / 96 / 128; MMA M stays 128)
+    int tc_rows_opt = 0, tc_rows = 128;                  // kernel variant: capacity of a tensor-core tile (32 / 64 / 96 / 128; the product has 128 rows)
     int tile_rows = 128;                                 // edges per tile actually used (<= tc_rows): whole waves of CTAs
     long long edges_plan = 0;                            // edge count the tile length was planned for (estimate or calibrated)
     int krot = 1;      // rotate the K loops of the SIMT node GEMM units per CTA (L2 slice hot-spotting: all CTAs walk the same weights)
@@ -169,7 +169,7 @@ struct vb_handle {
     int fused = 0, fused_opt = -1;   // 1: one launch per layer and direction (k_fused.cuh); -1 = choose by problem size
     int node_tc = 0, node_tc_opt = -1;   // 1: node stage on tensor cores (k_node_tc.cuh); -1 = choose by problem size
     int embed_batch_opt = -1;            // embedding kernels: several nodes per CTA (1), one (0), by size (-1)
-    int edge_tc = -1;  // bit 0: forward edge stage on tcgen05, bit 1: adjoint edge stage on tcgen05; -1 = by size
+    int edge_tc = -1;  // bit 0: forward edge stage on tensor cores, bit 1: adjoint edge stage on tensor cores; -1 = by size
     // graph cache: one instantiated graph per (kind, I/O pointer set); pointers are baked into the captured launches
     struct GraphEntry { int kind; StepIO io; cudaGraphExec_t exec; };
     std::vector<GraphEntry> graphs;
@@ -488,11 +488,11 @@ void launch_edge_fwd_tc(Launcher& Lc, int l) {
     const LayerW& lw = h->mw.layer[l];
     const size_t chunk = 4 * 8192;
     int n = 0;
-    a.jobs[n++] = TcJob{lw.tcW1, (int)TC_COL_D0, 0};                       // dk
-    a.jobs[n++] = TcJob{lw.tcW1 + chunk, (int)TC_COL_D1, 0};               // dv
-    if (l < L - 1) a.jobs[n++] = TcJob{lw.tcW1 + 2 * chunk, (int)TC_COL_D0, 0};   // f
-    a.jobs[n++] = TcJob{lw.tcWs, (int)TC_COL_D1, 0};                       // s1
-    a.jobs[n++] = TcJob{lw.tcWs + chunk, (int)TC_COL_D0, 0};               // s2
+    a.jobs[n++] = TcJob{lw.tcW1, 0};                       // dk
+    a.jobs[n++] = TcJob{lw.tcW1 + chunk, 0};               // dv
+    if (l < L - 1) a.jobs[n++] = TcJob{lw.tcW1 + 2 * chunk, 0};   // f
+    a.jobs[n++] = TcJob{lw.tcWs, 0};                       // s1
+    a.jobs[n++] = TcJob{lw.tcWs + chunk, 0};               // s2
     a.njobs = n;
     a.tl = h->timeline ? h->d_tl + (size_t)l * TC_TL_SLOTS : nullptr;
     a.tile_rows = h->tile_rows;
@@ -519,11 +519,11 @@ void launch_edge_bwd_tc(Launcher& Lc, int l) {
     const size_t chunk = 4 * 8192;
     const bool upd = l < L - 1;
     int n = 0;
-    a.jobs[n++] = TcJob{lw.tcWsN, (int)TC_COL_D1, 0};                        // g_m  = g_s1' Ws[0:128]
-    a.jobs[n++] = TcJob{lw.tcWsN + chunk, (int)TC_COL_D1, 1};                //      + g_s2' Ws[128:256]
-    a.jobs[n++] = TcJob{lw.tcW1N + chunk, (int)TC_COL_D0, 0};                // g_f  = g_Pdv Wdv
-    a.jobs[n++] = TcJob{lw.tcW1N, (int)TC_COL_D0, 1};                        //      + g_Pdk Wdk
-    if (upd) a.jobs[n++] = TcJob{lw.tcW1N + 2 * chunk, (int)TC_COL_D0, 1};   //      + g_Pf  Wf
+    a.jobs[n++] = TcJob{lw.tcWsN, 0};                        // g_m  = g_s1' Ws[0:128]
+    a.jobs[n++] = TcJob{lw.tcWsN + chunk, 1};                //      + g_s2' Ws[128:256]
+    a.jobs[n++] = TcJob{lw.tcW1N + chunk, 0};                // g_f  = g_Pdv Wdv
+    a.jobs[n++] = TcJob{lw.tcW1N, 1};                        //      + g_Pdk Wdk
+    if (upd) a.jobs[n++] = TcJob{lw.tcW1N + 2 * chunk, 1};   //      + g_Pf  Wf
     a.njobs = n;
     a.tl = h->timeline ? h->d_tl + (size_t)(L + l) * TC_TL_SLOTS : nullptr;
     a.tile_rows = h->tile_rows;
@@ -546,20 +546,20 @@ void edge_bwd(Launcher& Lc, int l) {
 void fill_fwd_jobs(const LayerW& lw, int l, TcJob* jobs, int& n) {
     const size_t chunk = 4 * 8192;
     n = 0;
-    jobs[n++] = TcJob{lw.tcW1, (int)TC_COL_D0, 0};                       // dk
-    jobs[n++] = TcJob{lw.tcW1 + chunk, (int)TC_COL_D1, 0};               // dv
-    if (l < L - 1) jobs[n++] = TcJob{lw.tcW1 + 2 * chunk, (int)TC_COL_D0, 0};   // f
-    jobs[n++] = TcJob{lw.tcWs, (int)TC_COL_D1, 0};                       // s1
-    jobs[n++] = TcJob{lw.tcWs + chunk, (int)TC_COL_D0, 0};               // s2
+    jobs[n++] = TcJob{lw.tcW1, 0};                       // dk
+    jobs[n++] = TcJob{lw.tcW1 + chunk, 0};               // dv
+    if (l < L - 1) jobs[n++] = TcJob{lw.tcW1 + 2 * chunk, 0};   // f
+    jobs[n++] = TcJob{lw.tcWs, 0};                       // s1
+    jobs[n++] = TcJob{lw.tcWs + chunk, 0};               // s2
 }
 void fill_bwd_jobs(const LayerW& lw, int l, TcJob* jobs, int& n) {
     const size_t chunk = 4 * 8192;
     n = 0;
-    jobs[n++] = TcJob{lw.tcWsN, (int)TC_COL_D1, 0};                        // g_m  = g_s1' Ws[0:128]
-    jobs[n++] = TcJob{lw.tcWsN + chunk, (int)TC_COL_D1, 1};                //      + g_s2' Ws[128:256]
-    jobs[n++] = TcJob{lw.tcW1N + chunk, (int)TC_COL_D0, 0};                // g_f  = g_Pdv Wdv
-    jobs[n++] = TcJob{lw.tcW1N, (int)TC_COL_D0, 1};                        //      + g_Pdk Wdk
-    if (l < L - 1) jobs[n++] = TcJob{lw.tcW1N + 2 * chunk, (int)TC_COL_D0, 1};   //      + g_Pf  Wf
+    jobs[n++] = TcJob{lw.tcWsN, 0};                        // g_m  = g_s1' Ws[0:128]
+    jobs[n++] = TcJob{lw.tcWsN + chunk, 1};                //      + g_s2' Ws[128:256]
+    jobs[n++] = TcJob{lw.tcW1N + chunk, 0};                // g_f  = g_Pdv Wdv
+    jobs[n++] = TcJob{lw.tcW1N, 1};                        //      + g_Pdk Wdk
+    if (l < L - 1) jobs[n++] = TcJob{lw.tcW1N + 2 * chunk, 1};   //      + g_Pf  Wf
 }
 int fused_grid(const vb_handle* h) {
     const int nblocks = (h->ws.N + FU_NB - 1) / FU_NB;
@@ -596,7 +596,7 @@ void node_tc_common(const vb_handle* h, NodeTcArgs& a, int k) {
     a.njx = 3; a.njv = 5; a.jx = 1; a.jv = 1;
 }
 void node_tc_jobs(TcJob* jobs, const float* img, int n) {
-    for (int c = 0; c < n; c++) jobs[c] = TcJob{img + (size_t)c * 4 * 8192, 0, 0};
+    for (int c = 0; c < n; c++) jobs[c] = TcJob{img + (size_t)c * 4 * 8192, 0};
 }
 int node_tc_grid(const NodeTcArgs& a) { return a.tx * (a.njx / a.jx) + a.tv * (a.njv / a.jv); }
 // one job per CTA while that still fits ~2 waves (each CTA then streams a single weight image); otherwise a CTA runs all
@@ -638,7 +638,7 @@ void launch_node_bwdA_tc(Launcher& Lc, int k) {            // K-chunk partials o
     node_tc_jobs(a.jobs_v, h->mw.layer[k].tcWvtN, 5);
     if (k == L - 1) a.njv = 3;
     a.acc_qkv = h->ws.GQKV; a.acc_tu = h->ws.GTU;
-    if (!node_tc_split(h, a)) { a.jx = a.njx; a.jv = a.njv; }   // all K chunks in one CTA, accumulated in TMEM
+    if (!node_tc_split(h, a)) { a.jx = a.njx; a.jv = a.njv; }   // all K chunks in one CTA, accumulated in registers
     Lc.launch(node_tc_kernel<NT_BWDA>, dim3(node_tc_grid(a)), dim3(TC2_THREADS), TC_SMEM_BYTES, a);
     Lc.check();
 }
@@ -657,7 +657,7 @@ void launch_node_bwdB_tc(Launcher& Lc, int k) {            // dE/dxa partials = 
     node_tc_common(h, a, k);
     a.tv = 0;
     node_tc_jobs(a.jobs_x, h->mw.layer[k - 1].tcWoN, 3);
-    if (h->ws.gxa_parts == 1) a.jx = 3;                        // accumulate the three K chunks in TMEM: one complete dE/dxa
+    if (h->ws.gxa_parts == 1) a.jx = 3;                        // accumulate the three K chunks in one CTA: one complete dE/dxa
     Lc.launch(node_tc_kernel<NT_BWDB>, dim3(node_tc_grid(a)), dim3(TC2_THREADS), TC_SMEM_BYTES, a);
     Lc.check();
 }
@@ -910,13 +910,11 @@ void record_stages(vb_handle* h) {
     h->launches = (int)h->stage_names.size();
 }
 
-// Tile length of the tcgen05 edge kernels.  A tile's latency is a fixed part (every CTA streams the layer's weights
-// L2 -> shared memory, barriers, TMEM round trips) plus per-row SIMT phases in which each of the 16 compute warps owns
+// Tile length of the tensor-core edge kernels.  A tile's latency is a fixed part (every CTA streams the layer's weights
+// L2 -> shared memory, barriers, accumulator round trips) plus per-row SIMT phases in which each of the 16 compute warps owns
 // ceil(rows / 16) rows.  So the edges are cut into the fewest whole waves of tiles <= 128 edges, and the tile length is
-// the smallest MULTIPLE OF 16 that still fits those waves: Chignolin (6.7k edges) 141 tiles of 48 instead of 105 of 64,
-// WW (19.7k) 247 tiles of 80 in two even waves instead of 154 of 128 (one full wave + 6 tiles).  Lengths between
-// multiples of 16 were measured slower (more CTAs, same rows per warp: Trp-cage 88 vs 96 +3 %), and so was 112 instead
-// of 128 (ABD +2 %, 512 fragments +2.5 %): from 7 rows per warp on the full tile is kept.  `edges` is an estimate (17 per
+// the smallest MULTIPLE OF 16 that still fits those waves (lengths between multiples of 16 add CTAs without
+// shortening any warp's run of rows); from 7 rows per warp on the full tile is kept.  `edges` is an estimate (17 per
 // atom, +3 % margin) until vb_set_option("calibrate") replaces it by the count of the last evaluation.
 void plan_tiles(vb_handle* h, long long edges) {
     const long long sm = h->sm_count;
@@ -938,21 +936,21 @@ void plan_tiles(vb_handle* h, long long edges) {
 void choose_defaults(vb_handle* h) {
     const int N = h->ws.N;
     h->npw = h->npw_opt; h->te_fwd = h->te_fwd_opt; h->edge_tc = h->edge_tc_opt;
-    // fused per-layer launches (k_fused.cuh) are opt-in: inside a graph a launch boundary costs ~1-2 us, less than what the
-    // fused kernels lose to the 96-register budget of a 576-thread CTA running the node GEMMs (profiles/README.md)
+    // fused per-layer launches (k_fused.cuh) are opt-in: inside a graph a launch boundary costs little, and the fused kernels
+    // run the node stage under the 96-register budget of the tensor-core CTA
     h->fused = h->fused_opt >= 0 ? h->fused_opt : 0;
-    // node stage on tensor cores from ~600 atoms on (measured, graph replay: Chignolin 391 atoms 0.78 -> 0.82 ms slower,
-    // Trp-cage 737 atoms 1.08 -> 0.97 ms, WW 2.07 -> 1.81, ABD 2.22 -> 1.98, 512 fragments 13.8 -> 12.3: the three-launch
-    // stage has a higher fixed latency than the single SIMT kernel, profiles/README.md)
+    // node stage on tensor cores from ~600 atoms on: the three-launch stage has a higher fixed latency than the single SIMT
+    // kernel, which wins on small systems (threshold not yet re-measured on H100)
     h->node_tc = h->node_tc_opt >= 0 ? h->node_tc_opt : (N >= 600 ? 1 : 0);
     if (h->fused) h->node_tc = 0;
     set_gxa_parts(h);
     if (h->npw == 0) h->npw = (N > 4096) ? 2 : 1;
     if (h->te_fwd == 0) h->te_fwd = ((long long)N * 17 / 64 >= 2LL * h->sm_count) ? 64 : 32;
-    // tcgen05 edge kernels (one tile per CTA, 16 compute warps): with the tile length chosen below both stages beat
-    // the fp32 SIMT kernels at every size measured, down to a single 26-atom fragment (tools/tc_crossover.py,
-    // profiles/README.md); the SIMT kernels stay selectable ("edge_tc" 0..2) as the independent implementation
-    if (h->edge_tc < 0) h->edge_tc = 3;
+    // forward edge stage on tensor cores, adjoint edge stage on the fp32 SIMT kernel.  Measured per launch on an H100
+    // (tools/stage_times.py, 700 W): forward wgmma 60 us vs SIMT 80 us on Chignolin, 1.32 vs 1.57 ms on the 512-fragment
+    // batch; adjoint wgmma 103 us vs SIMT 72 us, 2.55 vs 2.00 ms -- the wgmma adjoint keeps its accumulator live across
+    // SIMT phases under the 96-register budget of its 17-warp CTA and spills.  "edge_tc" 0..3 selects any combination.
+    if (h->edge_tc < 0) h->edge_tc = 1;
     plan_tiles(h, h->edges_plan > 0 ? h->edges_plan : (long long)N * 17);
 }
 
@@ -993,8 +991,8 @@ int vb_create(const float* weights_host, size_t n_floats, const vb_hparams* hp, 
     }
     cudaDeviceProp prop;
     cudaGetDeviceProperties(&prop, device);
-    if (prop.major < 10) {
-        g_create_error = "vb_create: device is not sm_100 class; the kernels are built for sm_100a only";
+    if (prop.major != 9 || prop.minor != 0) {
+        g_create_error = "vb_create: device is not sm_90 (Hopper); the kernels are built for sm_90a only";
         return VB_ERR_CUDA;
     }
     vb_handle* h = new vb_handle();
@@ -1795,7 +1793,7 @@ int vb_profile_stages(vb_handle* h, const float* pos_dev, int n_iter, float* ms_
 }
 
 int vb_tc_selftest(int device, const float* a_host, const float* img_host, float* d_host, int reps, float* ms_out) {
-    // D[128][128] = A[128][128] * W^T through the tcgen05/TMEM/TMA pipeline of the tensor-core edge kernels.
+    // D[128][128] = A[128][128] * W^T through the wgmma / TMA pipeline of the tensor-core edge kernels.
     if (!a_host || !img_host || !d_host || reps <= 0) return VB_ERR_ARG;
     if (cudaSetDevice(device) != cudaSuccess) { g_create_error = "vb_tc_selftest: cudaSetDevice failed"; return VB_ERR_CUDA; }
     float *dA = nullptr, *dI = nullptr, *dD = nullptr;
@@ -1808,7 +1806,7 @@ int vb_tc_selftest(int device, const float* a_host, const float* img_host, float
     cudaEvent_t e0, e1;
     cudaEventCreate(&e0); cudaEventCreate(&e1);
     cudaEventRecord(e0);
-    tc_selftest_kernel<<<1, TC_THREADS, TC_SMEM_BYTES>>>(dA, dI, dD, reps);
+    tc_selftest_kernel<<<1, TC2_THREADS, TC_SMEM_BYTES>>>(dA, dI, dD, reps);
     cudaEventRecord(e1);
     cudaError_t err = cudaDeviceSynchronize();
     float ms = 0.f;

@@ -212,7 +212,7 @@ __global__ void __launch_bounds__(NW * 32) edge_fwd_kernel(EdgeArgs a) {
 // attention pre-activation ATT in HBM/L2, so the reverse sweep only runs the two adjoint contractions
 //   g_m = g_xa_i + g_Spre Ws            (K = 256)
 //   g_f = g_f_next + [g_Pdk|g_Pdv|g_Pf] W1   (K = 384, 256 in the last layer)
-// (measured: the stage is contraction bound, not HBM bound, so 2.5 KB/edge of stored state beats recomputing
+// (the stage is contraction bound, not HBM bound, so 2.5 KB/edge of stored state is cheaper than recomputing
 // five 128x128 contractions per edge tile).
 // ---------------------------------------------------------------------------------------------
 constexpr int LEQ = 2 * D + 2 * LDS_PAD;   // 264: g_Spre row (256) / later the two per-edge tiles g_q (0..127) and g_wdot (132..259)

@@ -1,13 +1,4 @@
-// Tensor-core (tcgen05 / TMEM / TMA) version of the per-edge stage.
-//
-// CTA = 6 warps.  Warps 0-3 ("row threads", thread t <-> tile row t <-> TMEM lane t) own one edge each of a
-// 128-edge tile: they produce the A operands (tcgen05.st into TMEM, 3xTF32 hi/lo planes), consume the
-// accumulators (tcgen05.ld) and do all per-edge math thread-locally (a head = 16 consecutive columns of one
-// row, so the attention reduction needs no shuffles).  Warp 4 lane 0 streams the pre-swizzled weight images
-// through a 4-stage shared-memory ring with 1-D TMA bulk copies; warp 5 lane 0 issues the MMAs
-// (D[128x128] += A[128xK] * W^T, three tf32 MMAs per K-step: hi*hi + lo*hi + hi*lo ~ fp32 accuracy).
-// Per-target segmented sums go through a padded shared tile and are finished by the same 128 threads in
-// thread-per-channel mapping.
+// Tensor-core (wgmma / TMA) version of the per-edge stage.
 //
 // Weight images: for every 128-column GEMM chunk and every K-slab of 32: a 16 KB "hi" plane then a 16 KB "lo"
 // plane, each already in the K-major SWIZZLE_128B shared-memory layout (see tc_common.cuh), so one
@@ -18,33 +9,26 @@
 
 namespace vb {
 
-constexpr int TC_TE = 128;           // edges per tile (= MMA M)
-constexpr int TC_STAGES = 4;
+constexpr int TC_TE = 128;           // rows per tile (two wgmma M = 64 halves)
+constexpr int TC_STAGES = 2;         // weight ring depth: with the fp32 A operand in shared memory, two 32 KB stages fit
 constexpr int TC_MAXJOBS = 12;
-constexpr int TC_THREADS = 192;
-constexpr int TC_LT = D + LDS_PAD;   // padded row length of the staging tile (132 floats)
+constexpr int TC_LT = D + LDS_PAD;   // padded row length of the staging tile and of the A operand (132 floats)
 constexpr int TC_TILE_EXT = 1792;    // floats appended to the staging tile for the fused kernels' node stage (7 KB)
-
-// TMEM column map (512 columns): A hi plane, A lo plane, two accumulators
-constexpr uint32_t TC_COL_AHI = 0, TC_COL_ALO = 128, TC_COL_D0 = 256, TC_COL_D1 = 384;
 
 struct TcJob {
     const float* img;   // weight image of this 128x128 chunk (4 slabs x 32 KB)
-    int d_col;          // accumulator column base (TC_COL_D0 / TC_COL_D1)
-    int accumulate;     // 0: overwrite the accumulator with the first MMA, 1: add to what is there
+    int accumulate;     // 0: the product overwrites the accumulator, 1: adds to it
 };
 
 struct TcShared {
     alignas(1024) uint8_t ring[TC_STAGES][tc::STAGE_BYTES];
     alignas(16) float tile[TC_TE][TC_LT];
     float tile_ext[TC_TILE_EXT];        // fused kernels (k_fused.cuh): the node stage's shared rows start at `tile` and may run on into here
+    alignas(16) float abuf[TC_TE][TC_LT];   // A operand of the products in flight (fp32; split into tf32 hi / lo as it is loaded)
     EdgeMeta<TC_TE> meta;
     alignas(8) uint64_t b_full[TC_STAGES];
     uint64_t b_empty[TC_STAGES];
-    uint64_t go[TC_MAXJOBS];
-    uint64_t done[TC_MAXJOBS];
     uint64_t b_tile;                    // per-edge feature rows landed in `tile` (one arrival + byte count per compute warp)
-    uint32_t tmem_base;
     alignas(16) float eacc[TC_TE][4];   // per-edge adjoint scalars of the current tile: dE/dC, dE/dd[3]
     float gattn[TC_TE][H];              // adjoint kernel: dE/da_h per edge
 };
@@ -55,26 +39,7 @@ __device__ __forceinline__ TcShared* tc_shared_base(uint8_t* raw) {
     return reinterpret_cast<TcShared*>(raw + (((s + 1023u) & ~1023u) - s));
 }
 constexpr size_t TC_SMEM_BYTES = sizeof(TcShared) + 1024;
-
-// one-time CTA setup: barriers + TMEM; returns the TMEM base address
-__device__ __forceinline__ uint32_t tc_setup(TcShared& sh, int njobs, int go_count = TC_TE) {
-    const int warp = threadIdx.x >> 5;
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < TC_STAGES; s++) { tc::mbar_init(&sh.b_full[s], 1); tc::mbar_init(&sh.b_empty[s], 1); }
-        for (int j = 0; j < njobs; j++) { tc::mbar_init(&sh.go[j], go_count); tc::mbar_init(&sh.done[j], 1); }
-        tc::fence_barrier_init();
-    }
-    if (warp == 4) tc::tmem_alloc(&sh.tmem_base, 512);
-    tc::fence_before_sync();
-    __syncthreads();
-    tc::fence_after_sync();
-    return sh.tmem_base;
-}
-__device__ __forceinline__ void tc_teardown(uint32_t tmem_base) {
-    tc::fence_before_sync();
-    __syncthreads();
-    if ((threadIdx.x >> 5) == 4) tc::tmem_dealloc(tmem_base, 512);
-}
+static_assert(TC_SMEM_BYTES <= 227 * 1024, "tensor-core kernels must fit the 227 KB of shared memory of an H100 block");
 
 // weight producer: one thread; streams the slabs of `njobs` jobs for `ntiles` tiles through the ring
 __device__ __forceinline__ void tc_producer(TcShared& sh, const TcJob* jobs, int njobs, int ntiles) {
@@ -94,103 +59,6 @@ __device__ __forceinline__ void tc_producer(TcShared& sh, const TcJob* jobs, int
     }
 }
 
-// MMA issuer: one thread
-__device__ __forceinline__ void tc_mma_issuer(TcShared& sh, const TcJob* jobs, int njobs, int ntiles, uint32_t tmem_base,
-                                              unsigned long long* tl = nullptr) {
-    constexpr uint32_t idesc = tc::idesc_tf32(128, 128);
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int t = 0; t < ntiles; t++) {
-        const uint32_t tpar = (uint32_t)(t & 1);
-        for (int j = 0; j < njobs; j++) {
-            tc::mbar_wait(&sh.go[j], tpar);
-            tc::fence_after_sync();
-            if (tl != nullptr && t == 0) tl[32 + 2 * j] = (unsigned long long)clock64();
-            const uint32_t d_addr = tmem_base + (uint32_t)jobs[j].d_col;
-            uint32_t acc = (uint32_t)jobs[j].accumulate;
-#pragma unroll 1
-            for (int s = 0; s < D / tc::SLAB_K; s++) {
-                tc::mbar_wait(&sh.b_full[stage], phase);
-                tc::fence_after_sync();
-                const uint32_t bhi = tc::smem_u32(sh.ring[stage]);
-                const uint32_t blo = bhi + tc::SLAB_BYTES;
-#pragma unroll
-                for (int kk = 0; kk < tc::SLAB_K / 8; kk++) {
-                    const uint32_t a_off = (uint32_t)(s * tc::SLAB_K + kk * 8);
-                    const uint64_t dhi = tc::smem_desc_sw128(bhi + kk * 32);
-                    const uint64_t dlo = tc::smem_desc_sw128(blo + kk * 32);
-                    tc::mma_tf32_ts(d_addr, tmem_base + TC_COL_ALO + a_off, dhi, idesc, acc);   // lo * hi
-                    tc::mma_tf32_ts(d_addr, tmem_base + TC_COL_AHI + a_off, dlo, idesc, 1u);    // hi * lo
-                    tc::mma_tf32_ts(d_addr, tmem_base + TC_COL_AHI + a_off, dhi, idesc, 1u);    // hi * hi
-                    acc = 1u;
-                }
-                tc::mma_commit(&sh.b_empty[stage]);
-                if (++stage == TC_STAGES) { stage = 0; phase ^= 1; }
-            }
-            tc::mma_commit(&sh.done[j]);
-            if (tl != nullptr && t == 0) tl[33 + 2 * j] = (unsigned long long)clock64();
-        }
-    }
-}
-
-// row thread: publish "the A operand / accumulator for job j is ready"
-__device__ __forceinline__ void tc_signal_go(TcShared& sh, int j) {
-    tc::wait_st();
-    tc::fence_before_sync();
-    tc::mbar_arrive(&sh.go[j]);
-}
-__device__ __forceinline__ void tc_wait_done(TcShared& sh, int j, uint32_t tpar) {
-    tc::mbar_wait(&sh.done[j], tpar);
-    tc::fence_after_sync();
-}
-// barrier among the 128 row threads only (named barrier 1)
-__device__ __forceinline__ void rows_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
-
-// ---------------------------------------------------------------------------------------------
-// Self-test: Dout[128][128] = A[128][128] * W^T with W given as a tc image (validates descriptors,
-// swizzle, TMEM lane/column conventions, the ring and every barrier before the edge kernels use them).
-// ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(TC_THREADS, 1) tc_selftest_kernel(const float* __restrict__ A, const float* __restrict__ img,
-                                                                    float* __restrict__ Dout, int reps) {
-    extern __shared__ __align__(1024) uint8_t dyn_raw[];
-    TcShared& sh = *tc_shared_base(dyn_raw);
-    __shared__ TcJob jobs[1];
-    if (threadIdx.x == 0) jobs[0] = TcJob{img, (int)TC_COL_D0, 0};
-    const uint32_t tmem = tc_setup(sh, 1);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (warp == 4) {
-        if (lane == 0) tc_producer(sh, jobs, 1, reps);
-    } else if (warp == 5) {
-        if (lane == 0) tc_mma_issuer(sh, jobs, 1, reps, tmem);
-    } else {
-        const int row = threadIdx.x;
-        const uint32_t lane_base = (uint32_t)(warp * 32) << 16;
-        for (int t = 0; t < reps; t++) {
-            for (int c0 = 0; c0 < D; c0 += 16) {
-                float v[16];
-#pragma unroll
-                for (int q = 0; q < 16; q += 4) {
-                    const float4 x = ld4(A + (size_t)row * D + c0 + q);
-                    v[q] = x.x; v[q + 1] = x.y; v[q + 2] = x.z; v[q + 3] = x.w;
-                }
-                tc::store_a16(tmem + lane_base + TC_COL_AHI, tmem + lane_base + TC_COL_ALO, c0, v);
-            }
-            tc_signal_go(sh, 0);
-            tc_wait_done(sh, 0, (uint32_t)(t & 1));
-            for (int c0 = 0; c0 < D; c0 += 16) {
-                float v[16];
-                tc::tmem_ld16(tmem + lane_base + TC_COL_D0 + c0, v);
-#pragma unroll
-                for (int q = 0; q < 16; q += 4) st4(Dout + (size_t)row * D + c0 + q, f4(v[q], v[q + 1], v[q + 2], v[q + 3]));
-            }
-            tc::fence_before_sync();
-            rows_sync();          // every row thread finished reading D before the next repetition overwrites it
-            tc::fence_after_sync();
-        }
-    }
-    tc_teardown(tmem);
-}
-
 }  // namespace vb
 
 
@@ -198,19 +66,21 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_selftest_kernel(const float*
 // Tensor-core edge stage, hybrid layout.
 //   * 16 compute warps keep the coalesced "lane owns 4 channels" layout of k_edge.cuh for every global
 //     gather / scatter / elementwise step (one 512 B request per node row per warp);
-//   * the five 128x128x128 contractions per tile run on tcgen05: the A operand is moved from the padded
-//     shared staging tile into TMEM (thread-per-row, 3xTF32 planes), the accumulator comes back the same way;
-//   * warp 16 lane 0 = TMA weight producer, warp 17 lane 0 = MMA issuer (tc_producer / tc_mma_issuer);
-//   * a tile holds ROWS = 32 / 64 / 96 / 128 edges (template parameter): MMA M stays 128, TMEM lanes >= ROWS are never
-//     written or read, compute warp w owns rows [w*ROWS/16, (w+1)*ROWS/16) in the coalesced phases.
+//   * the five 128x128x128 contractions per tile run on wgmma: the A operand is copied from the padded shared
+//     staging tile into a second padded buffer, every compute warpgroup multiplies one 64 x 64 quarter of the
+//     product (A fragments split into 3xTF32 hi / lo in registers, B = the weight ring) and the accumulator comes
+//     back into the staging tile;
+//   * warp 16 lane 0 = TMA weight producer (tc_producer); the compute warps consume the ring in job order;
+//   * a tile holds ROWS = 32 / 64 / 96 / 128 edges (template parameter): compute warp w owns rows
+//     [w*ROWS/16, (w+1)*ROWS/16) in the coalesced phases; a warpgroup whose 64 product rows are all past the
+//     tile's edges skips its MMAs.
 // =====================================================================================================
 namespace vb {
 
 constexpr int TC2_CWARPS = 16;                      // compute warps
 constexpr int TC2_CTHREADS = TC2_CWARPS * 32;       // 512
-constexpr int TC2_THREADS = TC2_CTHREADS + 64;      // + producer warp + MMA warp
-constexpr int TC2_CBLK = D / (TC2_CWARPS / 4);         // columns each warp moves between the staging tile and TMEM
-constexpr int TC2_NGRP = TC2_CTHREADS / D;             // channel groups in the per-target aggregation phases
+constexpr int TC2_THREADS = TC2_CTHREADS + 32;      // + producer warp
+constexpr int TC2_NGRP = TC2_CTHREADS / D;          // channel groups in the per-target aggregation phases
 
 struct EdgeTcArgs {
     int layer;
@@ -221,76 +91,137 @@ struct EdgeTcArgs {
     int tile_rows;              // edges per tile, <= the kernel's ROWS
     unsigned long long* tl;     // optional timeline (SM clock stamps of CTA 0, first tile); nullptr = off
 };
-constexpr int TC_TL_SLOTS = 64;  // [0,32): compute thread 0 phase stamps ; [32,48): MMA issuer (go seen / MMAs issued per job)
+constexpr int TC_TL_SLOTS = 64;  // [0,32): compute thread 0 phase stamps
 #define TC_TL(k) do { if (a.tl != nullptr && blockIdx.x == 0 && it == 0 && threadIdx.x == 0) a.tl[k] = (unsigned long long)clock64(); } while (0)
 
 __device__ __forceinline__ void csync() { asm volatile("bar.sync 1, %0;" ::"n"(TC2_CTHREADS) : "memory"); }
 
-__device__ __forceinline__ uint32_t tc2_setup(TcShared& sh, int njobs) {
-    const int warp = threadIdx.x >> 5;
+__device__ __forceinline__ void tc2_setup(TcShared& sh) {
     if (threadIdx.x == 0) {
-        for (int s = 0; s < TC_STAGES; s++) { tc::mbar_init(&sh.b_full[s], 1); tc::mbar_init(&sh.b_empty[s], 1); }
-        for (int j = 0; j < njobs; j++) { tc::mbar_init(&sh.go[j], TC2_CTHREADS); tc::mbar_init(&sh.done[j], 1); }
+        for (int s = 0; s < TC_STAGES; s++) { tc::mbar_init(&sh.b_full[s], 1); tc::mbar_init(&sh.b_empty[s], TC2_CWARPS); }
         tc::mbar_init(&sh.b_tile, TC2_CWARPS);
         tc::fence_barrier_init();
     }
-    if (warp == TC2_CWARPS) tc::tmem_alloc(&sh.tmem_base, 512);
-    tc::fence_before_sync();
     __syncthreads();
-    tc::fence_after_sync();
-    return sh.tmem_base;
-}
-__device__ __forceinline__ void tc2_teardown(uint32_t tmem_base) {
-    tc::fence_before_sync();
-    __syncthreads();
-    if ((threadIdx.x >> 5) == TC2_CWARPS) tc::tmem_dealloc(tmem_base, 512);
 }
 
-// staging tile (fp32, row-major, padded) -> A operand planes in TMEM.  Compute warp w serves TMEM lane quarter
-// w&3 (rows 32*(w&3)..+31) and column half w>>2.
-template <int ROWS>
-__device__ __forceinline__ void tc2_tile_to_a(TcShared& sh, uint32_t tmem, int warp, int lane) {
-    if ((warp & 3) * 32 >= ROWS) return;          // short tiles: TMEM lanes >= ROWS stay stale (their D rows are never read)
-    const int row = (warp & 3) * 32 + lane, ch = (warp >> 2) * TC2_CBLK;
-    const uint32_t tl = tmem + ((uint32_t)((warp & 3) * 32) << 16);
-#pragma unroll
-    for (int c0 = 0; c0 < TC2_CBLK; c0 += 16) {
-        float v[16];
-#pragma unroll
-        for (int q = 0; q < 16; q += 4) {
-            const float4 x = ld4(&sh.tile[row][ch + c0 + q]);
-            v[q] = x.x; v[q + 1] = x.y; v[q + 2] = x.z; v[q + 3] = x.w;
-        }
-        tc::store_a16(tl + TC_COL_AHI, tl + TC_COL_ALO, ch + c0, v);
+// position of a compute thread in the weight ring (every compute thread walks the same sequence)
+struct TcRing {
+    int stage = 0;
+    uint32_t phase = 0;
+};
+
+// staging tile -> A operand (rows below `rows`), after every compute warp is done with the previous A operand and
+// has finished writing the tile
+__device__ __forceinline__ void tc2_tile_to_a(TcShared& sh, int rows) {
+    csync();
+    for (int idx = threadIdx.x; idx < rows * (D / 4); idx += TC2_CTHREADS) {
+        const int r = idx >> 5, c = (idx & 31) * 4;
+        st4(&sh.abuf[r][c], ld4(&sh.tile[r][c]));
     }
 }
-// accumulator (TMEM) -> staging tile
-template <int ROWS>
-__device__ __forceinline__ void tc2_d_to_tile(TcShared& sh, uint32_t tmem, uint32_t d_col, int warp, int lane) {
-    if ((warp & 3) * 32 >= ROWS) return;
-    const int row = (warp & 3) * 32 + lane, ch = (warp >> 2) * TC2_CBLK;
-    const uint32_t tl = tmem + ((uint32_t)((warp & 3) * 32) << 16) + d_col;
-    constexpr int NB16 = TC2_CBLK / 16;
-    uint32_t r[NB16][16];
+
+// acc (+)= A * W^T for the next job of the ring (all compute warps).  Warpgroup q = warp / 4 computes rows
+// 64 * (q & 1) .. +63 and columns 64 * (q >> 1) .. +63 of the 128 x 128 product; each K-step is three tf32 MMAs,
+// lo * hi + hi * lo + hi * hi (~ fp32 accuracy).  A warpgroup whose rows all lie at or past `nvalid` only releases
+// the ring stages.  On return `acc` holds this thread's part of the product (layout: tc_common.cuh).
+__device__ __forceinline__ void tc2_mma(TcShared& sh, TcRing& ring, float (&acc)[32], int accumulate, int warp, int lane,
+                                        int nvalid) {
+    csync();                                                   // the A operand is complete
+    const int q = warp >> 2, m0 = (q & 1) * 64 + (warp & 3) * 16, g = lane >> 2, t = lane & 3;
+    const bool active = (q & 1) * 64 < nvalid;                 // warpgroup-uniform
+    if (!accumulate) {
 #pragma unroll
-    for (int b = 0; b < NB16; b++) tc::tmem_ld16_nowait(tl + ch + b * 16, r[b]);
-    tc::wait_ld();
+        for (int i = 0; i < 32; i++) acc[i] = 0.f;
+    }
+#pragma unroll 1
+    for (int s = 0; s < D / tc::SLAB_K; s++) {
+        tc::mbar_wait(&sh.b_full[ring.stage], ring.phase);
+        if (active) {
+            const uint32_t bhi = tc::smem_u32(sh.ring[ring.stage]) + (uint32_t)(q >> 1) * (64 * 128);
+            const uint32_t blo = bhi + tc::SLAB_BYTES;
+            uint32_t ahi[4][4], alo[4][4];
 #pragma unroll
-    for (int b = 0; b < NB16; b++)
+            for (int kk = 0; kk < 4; kk++) {
+                const int k = s * tc::SLAB_K + kk * 8 + t;
+                tc::split_tf32(sh.abuf[m0 + g][k], ahi[kk][0], alo[kk][0]);
+                tc::split_tf32(sh.abuf[m0 + g + 8][k], ahi[kk][1], alo[kk][1]);
+                tc::split_tf32(sh.abuf[m0 + g][k + 4], ahi[kk][2], alo[kk][2]);
+                tc::split_tf32(sh.abuf[m0 + g + 8][k + 4], ahi[kk][3], alo[kk][3]);
+            }
+            tc::wgmma_fence();
 #pragma unroll
-        for (int q = 0; q < 16; q += 4)
-            st4(&sh.tile[row][ch + b * 16 + q], f4(__uint_as_float(r[b][q]), __uint_as_float(r[b][q + 1]),
-                                                    __uint_as_float(r[b][q + 2]), __uint_as_float(r[b][q + 3])));
+            for (int kk = 0; kk < 4; kk++) {
+                const uint64_t dhi = tc::smem_desc_sw128(bhi + kk * 32);
+                const uint64_t dlo = tc::smem_desc_sw128(blo + kk * 32);
+                tc::mma_m64n64k8_tf32(acc, alo[kk], dhi);
+                tc::mma_m64n64k8_tf32(acc, ahi[kk], dlo);
+                tc::mma_m64n64k8_tf32(acc, ahi[kk], dhi);
+            }
+            tc::wgmma_commit();
+            tc::wgmma_wait_all();
+#pragma unroll
+            for (int kk = 0; kk < 4; kk++)
+#pragma unroll
+                for (int i = 0; i < 4; i++) { tc::reg_fence(ahi[kk][i]); tc::reg_fence(alo[kk][i]); }
+#pragma unroll
+            for (int i = 0; i < 32; i++) tc::reg_fence(acc[i]);
+        }
+        __syncwarp();
+        if (lane == 0) tc::mbar_arrive(&sh.b_empty[ring.stage]);
+        if (++ring.stage == TC_STAGES) { ring.stage = 0; ring.phase ^= 1; }
+    }
 }
-__device__ __forceinline__ void tc2_go(TcShared& sh, int j) {      // every compute thread
-    tc::wait_st();
-    tc::fence_before_sync();
-    tc::mbar_arrive(&sh.go[j]);
+
+// accumulator -> staging tile (rows below `nvalid`)
+__device__ __forceinline__ void tc2_acc_to_tile(TcShared& sh, const float (&acc)[32], int warp, int lane, int nvalid) {
+    const int q = warp >> 2, r = (q & 1) * 64 + (warp & 3) * 16 + (lane >> 2), c = (q >> 1) * 64 + 2 * (lane & 3);
+#pragma unroll
+    for (int i = 0; i < 8; i++) {
+        if (r < nvalid) *reinterpret_cast<float2*>(&sh.tile[r][c + 8 * i]) = make_float2(acc[4 * i], acc[4 * i + 1]);
+        if (r + 8 < nvalid) *reinterpret_cast<float2*>(&sh.tile[r + 8][c + 8 * i]) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
+    }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Self-test: Dout[128][128] = A[128][128] * W^T with W given as a tc image (validates descriptors,
+// swizzle, fragment layouts, the ring and its barriers before the edge kernels use them).
+// ---------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(TC2_THREADS, 1) tc_selftest_kernel(const float* __restrict__ A, const float* __restrict__ img,
+                                                                     float* __restrict__ Dout, int reps) {
+    extern __shared__ __align__(1024) uint8_t dyn_raw[];
+    TcShared& sh = *tc_shared_base(dyn_raw);
+    __shared__ TcJob jobs[1];
+    if (threadIdx.x == 0) jobs[0] = TcJob{img, 0};
+    tc2_setup(sh);
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (warp == TC2_CWARPS) {
+        if (lane == 0) tc_producer(sh, jobs, 1, reps);
+        return;
+    }
+    TcRing ring;
+    float acc[32];
+    for (int t = 0; t < reps; t++) {
+        for (int idx = threadIdx.x; idx < TC_TE * (D / 4); idx += TC2_CTHREADS) {
+            const int r = idx >> 5, c = (idx & 31) * 4;
+            st4(&sh.tile[r][c], ld4(A + (size_t)r * D + c));
+        }
+        tc2_tile_to_a(sh, TC_TE);
+        tc2_mma(sh, ring, acc, 0, warp, lane, TC_TE);
+        csync();
+        tc2_acc_to_tile(sh, acc, warp, lane, TC_TE);
+        csync();
+        for (int idx = threadIdx.x; idx < TC_TE * (D / 4); idx += TC2_CTHREADS) {
+            const int r = idx >> 5, c = (idx & 31) * 4;
+            st4(Dout + (size_t)r * D + c, ld4(&sh.tile[r][c]));
+        }
+        csync();
+    }
 }
 
 // ---------------------------------------------------------------------------------------------
 // forward (math and reference lines: see edge_fwd_kernel in k_edge.cuh)
-// job order: dk -> D0, dv -> D1, [f -> D0], s1 -> D1, s2 -> D0
+// job order: dk, dv, [f], s1, s2
 // ---------------------------------------------------------------------------------------------
 template <int ROWS>
 __global__ void __launch_bounds__(TC2_THREADS, 1) edge_fwd_tc_kernel(const __grid_constant__ EdgeTcArgs a) {
@@ -309,14 +240,14 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_fwd_tc_kernel(const __gri
     const int ntiles_total = (E + trows - 1) / trows;
     const int my_tiles = ((int)blockIdx.x < ntiles_total) ? (ntiles_total - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x : 0;
     if (a.tl != nullptr && blockIdx.x == 0 && threadIdx.x == 0) a.tl[0] = (unsigned long long)clock64();
-    const uint32_t tmem = tc2_setup(sh, a.njobs);
+    tc2_setup(sh);
     if (a.tl != nullptr && blockIdx.x == 0 && threadIdx.x == 0) a.tl[1] = (unsigned long long)clock64();
 
     if (warp == TC2_CWARPS) {
         if (lane == 0) tc_producer(sh, a.jobs, a.njobs, my_tiles);
-    } else if (warp == TC2_CWARPS + 1) {
-        if (lane == 0) tc_mma_issuer(sh, a.jobs, a.njobs, my_tiles, tmem, blockIdx.x == 0 ? a.tl : nullptr);
     } else {
+        TcRing ring;
+        float acc[32];
         const float* __restrict__ Fin = ws.F[l];
         float* __restrict__ Fout = upd ? ws.F[l + 1] : nullptr;
         const float* __restrict__ QKV = ws.QKV[l];
@@ -349,18 +280,14 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_fwd_tc_kernel(const __gri
             tc::mbar_wait(&sh.b_tile, tpar);
             csync();
             TC_TL(2);
-            tc2_tile_to_a<ROWS>(sh, tmem, warp, lane);
-            tc2_go(sh, J_DK);
-            tc2_go(sh, J_DV);
+            tc2_tile_to_a(sh, nvalid);
             TC_TL(3);
             // ---- dk -> attention weights ----
             float Areg[RPW];
-            tc::mbar_wait(&sh.done[J_DK], tpar);
-            tc::fence_after_sync();
+            tc2_mma(sh, ring, acc, a.jobs[J_DK].accumulate, warp, lane, nvalid);
             TC_TL(4);
             csync();                                              // everyone finished reading f from the tile
-            tc2_d_to_tile<ROWS>(sh, tmem, TC_COL_D0, warp, lane);
-            tc::fence_before_sync();
+            tc2_acc_to_tile(sh, acc, warp, lane, nvalid);
             csync();
             {
                 TC_TL(5);
@@ -381,13 +308,11 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_fwd_tc_kernel(const __gri
                 }
             }
             TC_TL(6);
-            if (upd) { tc::fence_before_sync(); tc::mbar_arrive(&sh.go[J_F]); }     // D0 is free
             // ---- dv -> message m (in place in the tile) ----
-            tc::mbar_wait(&sh.done[J_DV], tpar);
-            tc::fence_after_sync();
+            tc2_mma(sh, ring, acc, a.jobs[J_DV].accumulate, warp, lane, nvalid);
             TC_TL(7);
             csync();
-            tc2_d_to_tile<ROWS>(sh, tmem, TC_COL_D1, warp, lane);
+            tc2_acc_to_tile(sh, acc, warp, lane, nvalid);
             csync();
             {
                 TC_TL(8);
@@ -418,15 +343,13 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_fwd_tc_kernel(const __gri
             }
             TC_TL(10);
             // ---- A = m, start s1 (-> D1) ----
-            if (upd) { tc::mbar_wait(&sh.done[J_F], tpar); tc::fence_after_sync(); }   // A planes no longer read
-            tc2_tile_to_a<ROWS>(sh, tmem, warp, lane);
-            tc2_go(sh, J_S1);
+            if (upd) tc2_mma(sh, ring, acc, a.jobs[J_F].accumulate, warp, lane, nvalid);
+            tc2_tile_to_a(sh, nvalid);
             TC_TL(11);
             // ---- edge update from the f chunk (D0) ----
             if (upd) {
                 csync();                                          // m tile fully consumed (xa + A copy)
-                tc2_d_to_tile<ROWS>(sh, tmem, TC_COL_D0, warp, lane);
-                tc::fence_before_sync();
+                tc2_acc_to_tile(sh, acc, warp, lane, nvalid);
                 csync();
                 const float4 bb = ldg4(lw.b1 + 2 * D + col);
 #pragma unroll 1
@@ -462,15 +385,12 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_fwd_tc_kernel(const __gri
                 }
             }
             TC_TL(12);
-            tc::fence_before_sync();
-            tc::mbar_arrive(&sh.go[J_S2]);                        // D0 is free (A = m already published by go[J_S1])
             // ---- s1 (D1): va_i += sum_e vn_j * s1 ----
             float bnd[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
-            tc::mbar_wait(&sh.done[J_S1], tpar);
-            tc::fence_after_sync();
+            tc2_mma(sh, ring, acc, a.jobs[J_S1].accumulate, warp, lane, nvalid);
             TC_TL(13);
             csync();
-            tc2_d_to_tile<ROWS>(sh, tmem, TC_COL_D1, warp, lane);
+            tc2_acc_to_tile(sh, acc, warp, lane, nvalid);
             csync();
             {
                 TC_TL(14);
@@ -520,12 +440,10 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_fwd_tc_kernel(const __gri
                 tc::tma_prefetch_l2(Fin + (size_t)en * D, (uint32_t)min(trows, E - en) * D * 4);
             }
             // ---- s2 (D0): va_i += sum_e s2 * d ----
-            tc::mbar_wait(&sh.done[J_S2], tpar);
-            tc::fence_after_sync();
+            tc2_mma(sh, ring, acc, a.jobs[J_S2].accumulate, warp, lane, nvalid);
             TC_TL(16);
             csync();
-            tc2_d_to_tile<ROWS>(sh, tmem, TC_COL_D0, warp, lane);
-            tc::fence_before_sync();
+            tc2_acc_to_tile(sh, acc, warp, lane, nvalid);
             csync();
             {
                 TC_TL(17);
@@ -559,7 +477,6 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_fwd_tc_kernel(const __gri
             csync();                                              // tile / meta free for the next tile
         }
     }
-    tc2_teardown(tmem);
     if (a.tl != nullptr && blockIdx.x == 0 && threadIdx.x == 0) a.tl[31] = (unsigned long long)clock64();
 }
 
@@ -570,7 +487,7 @@ namespace vb {
 // ---------------------------------------------------------------------------------------------
 // adjoint on tensor cores (math and reference lines: see edge_bwd_kernel in k_edge.cuh).  Pre-activations come
 // from the forward stage (P1, SP, ATT), so the tile runs only the two adjoint contractions:
-// jobs (upd):  0 g3a -> D1   1 g3b -> D1(+)   2 g4dv -> D0   3 g4dk -> D0(+)   4 g4f -> D0(+)
+// jobs (upd):  0 g3a   1 g3b (+)   2 g4dv   3 g4dk (+)   4 g4f (+)
 // ---------------------------------------------------------------------------------------------
 template <int ROWS>
 __global__ void __launch_bounds__(TC2_THREADS, 1) edge_bwd_tc_kernel(const __grid_constant__ EdgeTcArgs a) {
@@ -590,14 +507,14 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_bwd_tc_kernel(const __gri
     const int ntiles_total = (E + trows - 1) / trows;
     const int my_tiles = ((int)blockIdx.x < ntiles_total) ? (ntiles_total - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x : 0;
     if (a.tl != nullptr && blockIdx.x == 0 && threadIdx.x == 0) a.tl[0] = (unsigned long long)clock64();
-    const uint32_t tmem = tc2_setup(sh, a.njobs);
+    tc2_setup(sh);
     if (a.tl != nullptr && blockIdx.x == 0 && threadIdx.x == 0) a.tl[1] = (unsigned long long)clock64();
 
     if (warp == TC2_CWARPS) {
         if (lane == 0) tc_producer(sh, a.jobs, a.njobs, my_tiles);
-    } else if (warp == TC2_CWARPS + 1) {
-        if (lane == 0) tc_mma_issuer(sh, a.jobs, a.njobs, my_tiles, tmem, blockIdx.x == 0 ? a.tl : nullptr);
     } else {
+        TcRing ring;
+        float acc[32];
         const float* __restrict__ QKV = ws.QKV[l];
         const float* __restrict__ VN = ws.VN[l];
         const float* __restrict__ TU = ws.TU[l];
@@ -605,9 +522,7 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_bwd_tc_kernel(const __gri
         const float* __restrict__ SP = ws.SP[l];
         const float* __restrict__ ATT = ws.ATT[l];
         const int cch = threadIdx.x & (D - 1), grp = threadIdx.x >> 7;
-        auto wait_done = [&](int j, uint32_t tpar) { tc::mbar_wait(&sh.done[j], tpar); tc::fence_after_sync(); };
         for (int it = 0; it < my_tiles; it++) {
-            const uint32_t tpar = (uint32_t)(it & 1);
             const int e0 = ((int)blockIdx.x + it * (int)gridDim.x) * trows;
             const int nvalid = min(trows, E - e0);
             // rows are dealt to the compute warps in contiguous runs of rpw = ceil(nvalid / 16): a tile shorter than ROWS
@@ -648,8 +563,7 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_bwd_tc_kernel(const __gri
             }
             TC_TL(3);
             csync();
-            tc2_tile_to_a<ROWS>(sh, tmem, warp, lane);
-            tc2_go(sh, J_G3A);
+            tc2_tile_to_a(sh, nvalid);
             TC_TL(4);
             csync();
             // ---- s2 half ----
@@ -671,17 +585,15 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_bwd_tc_kernel(const __gri
             }
             TC_TL(5);
             csync();
-            wait_done(J_G3A, tpar);
+            tc2_mma(sh, ring, acc, a.jobs[J_G3A].accumulate, warp, lane, nvalid);
             TC_TL(6);
-            tc2_tile_to_a<ROWS>(sh, tmem, warp, lane);
-            tc2_go(sh, J_G3B);
+            tc2_tile_to_a(sh, nvalid);
             TC_TL(7);
             // ---- g_m = g_xa_i + g_Spre Ws ; adjoint of m = v_j dv A ----
-            wait_done(J_G3B, tpar);
+            tc2_mma(sh, ring, acc, a.jobs[J_G3B].accumulate, warp, lane, nvalid);
             TC_TL(8);
             csync();
-            tc2_d_to_tile<ROWS>(sh, tmem, TC_COL_D1, warp, lane);
-            tc::fence_before_sync();
+            tc2_acc_to_tile(sh, acc, warp, lane, nvalid);
             csync();
             TC_TL(9);
 #pragma unroll 1
@@ -718,8 +630,7 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_bwd_tc_kernel(const __gri
             }
             TC_TL(10);
             csync();
-            tc2_tile_to_a<ROWS>(sh, tmem, warp, lane);               // A = g_Pdv (A planes free: g3b done)
-            tc2_go(sh, J_G4DV);
+            tc2_tile_to_a(sh, nvalid);               // A = g_Pdv (A planes free: g3b done)
             TC_TL(11);
             csync();
             // ---- adjoint of a_h = sum q_i k_j dk : first g_Pdk (next A operand), then the g_q tile ----
@@ -748,10 +659,9 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_bwd_tc_kernel(const __gri
             }
             TC_TL(12);
             csync();
-            wait_done(J_G4DV, tpar);
+            tc2_mma(sh, ring, acc, a.jobs[J_G4DV].accumulate, warp, lane, nvalid);
             TC_TL(13);
-            tc2_tile_to_a<ROWS>(sh, tmem, warp, lane);               // A = g_Pdk
-            tc2_go(sh, J_G4DK);
+            tc2_tile_to_a(sh, nvalid);               // A = g_Pdk
             TC_TL(14);
             csync();
 #pragma unroll 4
@@ -836,10 +746,9 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_bwd_tc_kernel(const __gri
                 }
                 TC_TL(16);
                 csync();
-                wait_done(J_G4DK, tpar);
+                tc2_mma(sh, ring, acc, a.jobs[J_G4DK].accumulate, warp, lane, nvalid);
                 TC_TL(17);
-                tc2_tile_to_a<ROWS>(sh, tmem, warp, lane);           // A = g_Pf
-                tc2_go(sh, J_G4F);
+                tc2_tile_to_a(sh, nvalid);           // A = g_Pf
                 TC_TL(18);
                 csync();
 #pragma unroll 4
@@ -909,11 +818,10 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_bwd_tc_kernel(const __gri
                 else tc::tma_prefetch_l2(ATT + (size_t)en * H, nn * H * 4);
             }
             // ---- g_f = g_f_next + [g_Pdk|g_Pdv|g_Pf] W1 ----
-            wait_done(J_LAST, tpar);
+            tc2_mma(sh, ring, acc, a.jobs[J_LAST].accumulate, warp, lane, nvalid);
             TC_TL(20);
             csync();
-            tc2_d_to_tile<ROWS>(sh, tmem, TC_COL_D0, warp, lane);
-            tc::fence_before_sync();
+            tc2_acc_to_tile(sh, acc, warp, lane, nvalid);
             csync();
             TC_TL(21);
 #pragma unroll 4
@@ -935,7 +843,6 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_bwd_tc_kernel(const __gri
             csync();
         }
     }
-    tc2_teardown(tmem);
     if (a.tl != nullptr && blockIdx.x == 0 && threadIdx.x == 0) a.tl[31] = (unsigned long long)clock64();
 }
 

@@ -2,7 +2,7 @@
 //
 // A CTA owns a block of NB consecutive nodes.  Edges are target-major, so the edges whose TARGET is one of those nodes
 // are one contiguous range [rowptr[n0], rowptr[n0 + NB)); the CTA walks that range in sub-tiles of <= 128 edges through
-// the tcgen05 edge stage of k_edge_tc.cuh (same phases, same weight ring / MMA issuer / TMEM plan) and then runs the
+// the tensor-core edge stage of k_edge_tc.cuh (same phases, same weight ring and MMA helpers) and then runs the
 // node stage for its own nodes without leaving the kernel:
 //   forward  layer l : edge stage l  (messages, per-target sums, edge update)  ->  node stage l+1 of the block
 //                      (o_proj + residual + LayerNorm + VecLayerNorm + q/k/v + vec_proj + w_trg/w_src, k_node2.cuh)
@@ -46,7 +46,7 @@ struct FuRows {
     __device__ __forceinline__ bool ok(int r) const { return r < rpw && base + r < nvalid; }
 };
 
-// number of sub-tiles this CTA will run (identical in the producer, the MMA issuer and the compute warps)
+// number of sub-tiles this CTA will run (identical in the producer and the compute warps)
 __device__ __forceinline__ int fu_count_tiles(const Workspace& ws) {
     const int nblocks = (ws.N + FU_NB - 1) / FU_NB;
     int tiles = 0;
@@ -57,43 +57,9 @@ __device__ __forceinline__ int fu_count_tiles(const Workspace& ws) {
     return tiles;
 }
 
-// staging tile <-> TMEM for a sub-tile with `nvalid` rows (TMEM lanes of untouched row quarters stay stale; their
-// accumulator rows are never read)
-__device__ __forceinline__ void fu_tile_to_a(TcShared& sh, uint32_t tmem, int warp, int lane, int nvalid) {
-    if ((warp & 3) * 32 >= nvalid) return;
-    const int row = (warp & 3) * 32 + lane, ch = (warp >> 2) * TC2_CBLK;
-    const uint32_t tl = tmem + ((uint32_t)((warp & 3) * 32) << 16);
-#pragma unroll
-    for (int c0 = 0; c0 < TC2_CBLK; c0 += 16) {
-        float v[16];
-#pragma unroll
-        for (int q = 0; q < 16; q += 4) {
-            const float4 x = ld4(&sh.tile[row][ch + c0 + q]);
-            v[q] = x.x; v[q + 1] = x.y; v[q + 2] = x.z; v[q + 3] = x.w;
-        }
-        tc::store_a16(tl + TC_COL_AHI, tl + TC_COL_ALO, ch + c0, v);
-    }
-}
-__device__ __forceinline__ void fu_d_to_tile(TcShared& sh, uint32_t tmem, uint32_t d_col, int warp, int lane, int nvalid) {
-    if ((warp & 3) * 32 >= nvalid) return;
-    const int row = (warp & 3) * 32 + lane, ch = (warp >> 2) * TC2_CBLK;
-    const uint32_t tl = tmem + ((uint32_t)((warp & 3) * 32) << 16) + d_col;
-    constexpr int NB16 = TC2_CBLK / 16;
-    uint32_t r[NB16][16];
-#pragma unroll
-    for (int b = 0; b < NB16; b++) tc::tmem_ld16_nowait(tl + ch + b * 16, r[b]);
-    tc::wait_ld();
-#pragma unroll
-    for (int b = 0; b < NB16; b++)
-#pragma unroll
-        for (int q = 0; q < 16; q += 4)
-            st4(&sh.tile[row][ch + b * 16 + q], f4(__uint_as_float(r[b][q]), __uint_as_float(r[b][q + 1]),
-                                                    __uint_as_float(r[b][q + 2]), __uint_as_float(r[b][q + 3])));
-}
-
 // =====================================================================================================
 // forward: edge stage l of the block's edges, then node stage l + 1 of the block
-// job order: dk -> D0, dv -> D1, [f -> D0], s1 -> D1, s2 -> D0        (as edge_fwd_tc_kernel)
+// job order: dk, dv, [f], s1, s2        (as edge_fwd_tc_kernel)
 // =====================================================================================================
 __global__ void __launch_bounds__(TC2_THREADS, 1) fused_fwd_kernel(const __grid_constant__ FusedArgs a) {
     pdl_entry();
@@ -106,13 +72,13 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) fused_fwd_kernel(const __grid_
     const int J_DK = 0, J_DV = 1, J_F = 2, J_S1 = upd ? 3 : 2, J_S2 = upd ? 4 : 3;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, col = lane * 4;
     const int my_tiles = fu_count_tiles(ws);
-    const uint32_t tmem = tc2_setup(sh, a.njobs);
+    tc2_setup(sh);
 
     if (warp == TC2_CWARPS) {
         if (lane == 0) tc_producer(sh, a.jobs, a.njobs, my_tiles);
-    } else if (warp == TC2_CWARPS + 1) {
-        if (lane == 0) tc_mma_issuer(sh, a.jobs, a.njobs, my_tiles, tmem, nullptr);
     } else {
+        TcRing ring;
+        float acc[32];
         const float* __restrict__ Fin = ws.F[l];
         float* __restrict__ Fout = upd ? ws.F[l + 1] : nullptr;
         const float* __restrict__ QKV = ws.QKV[l];
@@ -128,7 +94,6 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) fused_fwd_kernel(const __grid_
             const int n0 = b * FU_NB, n1 = min(n0 + FU_NB, ws.N);
             const int eb = ws.rowptr[n0], ee = ws.rowptr[n1];
             for (int e0 = eb; e0 < ee; e0 += TC_TE, t++) {
-                const uint32_t tpar = (uint32_t)(t & 1);
                 const int nvalid = min(TC_TE, ee - e0);
                 const FuRows R(nvalid, warp);
                 // ---- load f tile + meta (coalesced) ----
@@ -138,16 +103,12 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) fused_fwd_kernel(const __grid_
                 }
                 load_edge_meta<TC_TE, TC2_CTHREADS>(sh.meta, ws, e0, nvalid);
                 csync();
-                fu_tile_to_a(sh, tmem, warp, lane, nvalid);
-                tc2_go(sh, J_DK);
-                tc2_go(sh, J_DV);
+                tc2_tile_to_a(sh, nvalid);
                 // ---- dk -> attention weights ----
                 float Areg[FU_RPW];
-                tc::mbar_wait(&sh.done[J_DK], tpar);
-                tc::fence_after_sync();
+                tc2_mma(sh, ring, acc, a.jobs[J_DK].accumulate, warp, lane, nvalid);
                 csync();                                              // everyone finished reading f from the tile
-                fu_d_to_tile(sh, tmem, TC_COL_D0, warp, lane, nvalid);
-                tc::fence_before_sync();
+                tc2_acc_to_tile(sh, acc, warp, lane, nvalid);
                 csync();
                 {
                     const float4 bb = ldg4(lw.b1 + col);
@@ -166,12 +127,10 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) fused_fwd_kernel(const __grid_
                         }
                     }
                 }
-                if (upd) { tc::fence_before_sync(); tc::mbar_arrive(&sh.go[J_F]); }     // D0 is free
                 // ---- dv -> message m (in place in the tile) ----
-                tc::mbar_wait(&sh.done[J_DV], tpar);
-                tc::fence_after_sync();
+                tc2_mma(sh, ring, acc, a.jobs[J_DV].accumulate, warp, lane, nvalid);
                 csync();
-                fu_d_to_tile(sh, tmem, TC_COL_D1, warp, lane, nvalid);
+                tc2_acc_to_tile(sh, acc, warp, lane, nvalid);
                 csync();
                 {
                     const float4 bb = ldg4(lw.b1 + D + col);
@@ -197,14 +156,12 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) fused_fwd_kernel(const __grid_
                     ws.XA[(size_t)i * D + cch] += xa;
                 }
                 // ---- A = m, start s1 (-> D1) ----
-                if (upd) { tc::mbar_wait(&sh.done[J_F], tpar); tc::fence_after_sync(); }   // A planes no longer read
-                fu_tile_to_a(sh, tmem, warp, lane, nvalid);
-                tc2_go(sh, J_S1);
+                if (upd) tc2_mma(sh, ring, acc, a.jobs[J_F].accumulate, warp, lane, nvalid);
+                tc2_tile_to_a(sh, nvalid);
                 // ---- edge update from the f chunk (D0) ----
                 if (upd) {
                     csync();                                          // m tile fully consumed (xa + A copy)
-                    fu_d_to_tile(sh, tmem, TC_COL_D0, warp, lane, nvalid);
-                    tc::fence_before_sync();
+                    tc2_acc_to_tile(sh, acc, warp, lane, nvalid);
                     csync();
                     const float4 bb = ldg4(lw.b1 + 2 * D + col);
 #pragma unroll 1
@@ -240,13 +197,10 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) fused_fwd_kernel(const __grid_
                         }
                     }
                 }
-                tc::fence_before_sync();
-                tc::mbar_arrive(&sh.go[J_S2]);                        // D0 is free (A = m already published by go[J_S1])
                 // ---- s1 (D1): va_i += sum_e vn_j * s1 ----
-                tc::mbar_wait(&sh.done[J_S1], tpar);
-                tc::fence_after_sync();
+                tc2_mma(sh, ring, acc, a.jobs[J_S1].accumulate, warp, lane, nvalid);
                 csync();
-                fu_d_to_tile(sh, tmem, TC_COL_D1, warp, lane, nvalid);
+                tc2_acc_to_tile(sh, acc, warp, lane, nvalid);
                 csync();
                 {
                     const float bsv = __ldg(lw.bs + cch);
@@ -283,11 +237,9 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) fused_fwd_kernel(const __grid_
                     }
                 }
                 // ---- s2 (D0): va_i += sum_e s2 * d ----
-                tc::mbar_wait(&sh.done[J_S2], tpar);
-                tc::fence_after_sync();
+                tc2_mma(sh, ring, acc, a.jobs[J_S2].accumulate, warp, lane, nvalid);
                 csync();
-                fu_d_to_tile(sh, tmem, TC_COL_D0, warp, lane, nvalid);
-                tc::fence_before_sync();
+                tc2_acc_to_tile(sh, acc, warp, lane, nvalid);
                 csync();
                 {
                     const float bsv = __ldg(lw.bs + D + cch);
@@ -314,12 +266,11 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) fused_fwd_kernel(const __grid_
             csync();                                                  // node-stage shared rows (aliasing the tile) are free
         }
     }
-    tc2_teardown(tmem);
 }
 
 // =====================================================================================================
 // backward: node adjoint l + 1 of the block, then edge adjoint l of the block's edges
-// jobs (upd):  0 g3a -> D1   1 g3b -> D1(+)   2 g4dv -> D0   3 g4dk -> D0(+)   4 g4f -> D0(+)     (as edge_bwd_tc_kernel)
+// jobs (upd):  0 g3a   1 g3b (+)   2 g4dv   3 g4dk (+)   4 g4f (+)     (as edge_bwd_tc_kernel)
 // =====================================================================================================
 __global__ void __launch_bounds__(TC2_THREADS, 1) fused_bwd_kernel(const __grid_constant__ FusedArgs a) {
     pdl_entry();
@@ -333,13 +284,13 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) fused_bwd_kernel(const __grid_
     constexpr int RB4 = 4;                          // rows whose loads are issued together
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, col = lane * 4, hd = lane >> 2;
     const int my_tiles = fu_count_tiles(ws);
-    const uint32_t tmem = tc2_setup(sh, a.njobs);
+    tc2_setup(sh);
 
     if (warp == TC2_CWARPS) {
         if (lane == 0) tc_producer(sh, a.jobs, a.njobs, my_tiles);
-    } else if (warp == TC2_CWARPS + 1) {
-        if (lane == 0) tc_mma_issuer(sh, a.jobs, a.njobs, my_tiles, tmem, nullptr);
     } else {
+        TcRing ring;
+        float acc[32];
         const float* __restrict__ QKV = ws.QKV[l];
         const float* __restrict__ VN = ws.VN[l];
         const float* __restrict__ TU = ws.TU[l];
@@ -352,7 +303,6 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) fused_bwd_kernel(const __grid_
         const float* GVEC = ws.GVEC;            // written by this CTA's node adjoint below: coherent loads only (no ld.global.nc)
         const float* GXA = ws.GXA;
         const int cch = threadIdx.x & (D - 1), grp = threadIdx.x >> 7;
-        auto wait_done = [&](int j, uint32_t tpar) { tc::mbar_wait(&sh.done[j], tpar); tc::fence_after_sync(); };
         const int nblocks = (ws.N + FU_NB - 1) / FU_NB;
         int t = 0;
         for (int b = blockIdx.x; b < nblocks; b += gridDim.x) {
@@ -363,7 +313,6 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) fused_bwd_kernel(const __grid_
             csync();                                                  // GVEC / GXA of the block visible; node rows (aliasing the tile) free
             const int eb = ws.rowptr[n0], ee = ws.rowptr[n1];
             for (int e0 = eb; e0 < ee; e0 += TC_TE, t++) {
-                const uint32_t tpar = (uint32_t)(t & 1);
                 const int nvalid = min(TC_TE, ee - e0);
                 const FuRows R(nvalid, warp);
                 load_edge_meta<TC_TE, TC2_CTHREADS>(sh.meta, ws, e0, nvalid);
@@ -398,8 +347,7 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) fused_bwd_kernel(const __grid_
                     }
                 }
                 csync();
-                fu_tile_to_a(sh, tmem, warp, lane, nvalid);
-                tc2_go(sh, J_G3A);
+                tc2_tile_to_a(sh, nvalid);
                 csync();
                 // ---- s2 half ----
 #pragma unroll 4
@@ -419,14 +367,12 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) fused_bwd_kernel(const __grid_
                     }
                 }
                 csync();
-                wait_done(J_G3A, tpar);
-                fu_tile_to_a(sh, tmem, warp, lane, nvalid);
-                tc2_go(sh, J_G3B);
+                tc2_mma(sh, ring, acc, a.jobs[J_G3A].accumulate, warp, lane, nvalid);
+                tc2_tile_to_a(sh, nvalid);
                 // ---- g_m = g_xa_i + g_Spre Ws ; adjoint of m = v_j dv A ----
-                wait_done(J_G3B, tpar);
+                tc2_mma(sh, ring, acc, a.jobs[J_G3B].accumulate, warp, lane, nvalid);
                 csync();
-                fu_d_to_tile(sh, tmem, TC_COL_D1, warp, lane, nvalid);
-                tc::fence_before_sync();
+                tc2_acc_to_tile(sh, acc, warp, lane, nvalid);
                 csync();
 #pragma unroll 1
                 for (int rb = 0; rb < FU_RPW; rb += RB4) {
@@ -462,8 +408,7 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) fused_bwd_kernel(const __grid_
                     }
                 }
                 csync();
-                fu_tile_to_a(sh, tmem, warp, lane, nvalid);               // A = g_Pdv (A planes free: g3b done)
-                tc2_go(sh, J_G4DV);
+                tc2_tile_to_a(sh, nvalid);               // A = g_Pdv (A planes free: g3b done)
                 csync();
                 // ---- adjoint of a_h = sum q_i k_j dk : first g_Pdk (next A operand), then the g_q tile ----
 #pragma unroll 1
@@ -492,9 +437,8 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) fused_bwd_kernel(const __grid_
                     }
                 }
                 csync();
-                wait_done(J_G4DV, tpar);
-                fu_tile_to_a(sh, tmem, warp, lane, nvalid);               // A = g_Pdk
-                tc2_go(sh, J_G4DK);
+                tc2_mma(sh, ring, acc, a.jobs[J_G4DV].accumulate, warp, lane, nvalid);
+                tc2_tile_to_a(sh, nvalid);               // A = g_Pdk
                 csync();
 #pragma unroll 4
                 for (int r = 0; r < FU_RPW; r++) {
@@ -571,9 +515,8 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) fused_bwd_kernel(const __grid_
                         }
                     }
                     csync();
-                    wait_done(J_G4DK, tpar);
-                    fu_tile_to_a(sh, tmem, warp, lane, nvalid);           // A = g_Pf
-                    tc2_go(sh, J_G4F);
+                    tc2_mma(sh, ring, acc, a.jobs[J_G4DK].accumulate, warp, lane, nvalid);
+                    tc2_tile_to_a(sh, nvalid);           // A = g_Pf
                     csync();
 #pragma unroll 4
                     for (int r = 0; r < FU_RPW; r++) {
@@ -623,10 +566,9 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) fused_bwd_kernel(const __grid_
                     }
                 }
                 // ---- g_f = g_f_next + [g_Pdk|g_Pdv|g_Pf] W1 ----
-                wait_done(J_LAST, tpar);
+                tc2_mma(sh, ring, acc, a.jobs[J_LAST].accumulate, warp, lane, nvalid);
                 csync();
-                fu_d_to_tile(sh, tmem, TC_COL_D0, warp, lane, nvalid);
-                tc::fence_before_sync();
+                tc2_acc_to_tile(sh, acc, warp, lane, nvalid);
                 csync();
 #pragma unroll 4
                 for (int r = 0; r < FU_RPW; r++) {
@@ -646,7 +588,6 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) fused_bwd_kernel(const __grid_
             }
         }
     }
-    tc2_teardown(tmem);
 }
 
 }  // namespace vb

@@ -230,7 +230,7 @@ __global__ void __launch_bounds__(EMB_THREADS) embed_node_kernel(ModelW mw, Work
 // its <= 32 edges, rbf rows and edge metadata staged in shared memory by the whole CTA), then multiplies K-slice q of the
 // combine weight for all four nodes, so a CTA reads the 128 KB weight once for four nodes.  With one node per CTA the ~400
 // CTAs of a small protein all pulled the same 128 KB through L2 at the same time and that, not latency, bounded the kernel
-// (23 us for 391 atoms, identical before and after a rewrite that cut its dependent load rounds from ~20 to 5); for the
+// (cutting its dependent load rounds did not change its time); for the
 // same reason every CTA starts its walk over the weight rows at a different row.
 constexpr int EMS_THREADS = 4 * D, EMS_NB = 4;
 __global__ void __launch_bounds__(EMS_THREADS) embed_node_small_kernel(ModelW mw, Workspace ws, unsigned long long* tl) {

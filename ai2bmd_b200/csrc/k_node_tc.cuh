@@ -1,4 +1,4 @@
-// Node stage on tensor cores (tcgen05 / TMEM / TMA weight ring, 3xTF32): the dense node-feature x weight contractions of a
+// Node stage on tensor cores (wgmma / TMA weight ring, 3xTF32): the dense node-feature x weight contractions of a
 // ViS_MP layer -- q/k/v, vec_proj, w_trg/w_src, o_proj and their adjoints -- as 128-row GEMM tiles, one (row tile, column
 // chunk) job per CTA for small systems (every CTA streams ONE 128 KB weight image instead of the layer's whole 720 KB, and
 // the jobs of a stage spread over ~60-70 SMs), all chunks of a row tile in one CTA for large batches (A staged once).
@@ -59,17 +59,16 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) node_tc_kernel(const __grid_co
     constexpr bool KCHUNKS = (MODE == NT_BWDA || MODE == NT_BWDB);     // jobs = K chunks accumulated into one product
     if (threadIdx.x < nj) {
         TcJob j = is_x ? a.jobs_x[j0 + threadIdx.x] : a.jobs_v[j0 + threadIdx.x];
-        j.d_col = (!KCHUNKS && (threadIdx.x & 1)) ? (int)TC_COL_D1 : (int)TC_COL_D0;
         j.accumulate = (KCHUNKS && threadIdx.x > 0) ? 1 : 0;
         jl[threadIdx.x] = j;
     }
-    const uint32_t tmem = tc2_setup(sh, nj);           // (its __syncthreads publishes jl)
+    tc2_setup(sh);                                     // (its __syncthreads publishes jl)
 
     if (warp == TC2_CWARPS) {
         if (lane == 0) tc_producer(sh, jl, nj, 1);
-    } else if (warp == TC2_CWARPS + 1) {
-        if (lane == 0) tc_mma_issuer(sh, jl, nj, 1, tmem, nullptr);
     } else {
+        TcRing ring;
+        float acc[32];
         // A operand rows of job jj -> staging tile (warp per row, lane owns 4 channels: coalesced 512 B rows)
         auto load_a = [&](int jj) {
             for (int r = warp; r < nvalid; r += TC2_CWARPS) {
@@ -101,20 +100,14 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) node_tc_kernel(const __grid_co
             }
         };
         if (!KCHUNKS) {
-            // ---- column chunks of one product: one A operand, accumulators alternate between D0 and D1 ----
+            // ---- column chunks of one product: one A operand ----
             load_a(0);
-            csync();
-            fu_tile_to_a(sh, tmem, warp, lane, nvalid);
-            tc2_go(sh, 0);
-            if (nj > 1) tc2_go(sh, 1);
+            tc2_tile_to_a(sh, nvalid);
             for (int j = 0; j < nj; j++) {
-                tc::mbar_wait(&sh.done[j], 0u);
-                tc::fence_after_sync();
+                tc2_mma(sh, ring, acc, jl[j].accumulate, warp, lane, nvalid);
                 csync();                                          // the tile is free (A copied / previous chunk stored)
-                fu_d_to_tile(sh, tmem, (j & 1) ? TC_COL_D1 : TC_COL_D0, warp, lane, nvalid);
-                tc::fence_before_sync();
+                tc2_acc_to_tile(sh, acc, warp, lane, nvalid);
                 csync();
-                if (j + 2 < nj) tc::mbar_arrive(&sh.go[j + 2]);   // this accumulator is drained: the chunk after next may start
                 const int jj = j0 + j;
                 for (int r = warp; r < nvalid; r += TC2_CWARPS) {
                     const size_t row = (size_t)(row0 + r);
@@ -129,20 +122,15 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) node_tc_kernel(const __grid_co
                 }
             }
         } else {
-            // ---- K chunks of one product: every chunk has its own A operand, all accumulate into D0; with one chunk per
-            //      CTA the result is the partial of chunk j0 (the glue kernel / the edge adjoint sums the partials) ----
+            // ---- K chunks of one product: every chunk has its own A operand, all accumulate into one product; with one
+            //      chunk per CTA the result is the partial of chunk j0 (the glue kernel / the edge adjoint sums the partials) ----
             for (int j = 0; j < nj; j++) {
-                load_a(j0 + j);
-                csync();
-                if (j > 0) { tc::mbar_wait(&sh.done[j - 1], 0u); tc::fence_after_sync(); }   // A planes no longer read
-                fu_tile_to_a(sh, tmem, warp, lane, nvalid);
-                tc2_go(sh, j);
-                csync();                                          // the tile may take the next chunk's rows
+                load_a(j0 + j);                                   // (the previous chunk's MMAs began with a barrier: tile free)
+                tc2_tile_to_a(sh, nvalid);
+                tc2_mma(sh, ring, acc, jl[j].accumulate, warp, lane, nvalid);
             }
-            tc::mbar_wait(&sh.done[nj - 1], 0u);
-            tc::fence_after_sync();
-            fu_d_to_tile(sh, tmem, TC_COL_D0, warp, lane, nvalid);
-            tc::fence_before_sync();
+            csync();
+            tc2_acc_to_tile(sh, acc, warp, lane, nvalid);
             csync();
             for (int r = warp; r < nvalid; r += TC2_CWARPS) {
                 const size_t row = (size_t)(row0 + r);
@@ -156,7 +144,6 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) node_tc_kernel(const __grid_co
             }
         }
     }
-    tc2_teardown(tmem);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -208,7 +195,7 @@ __global__ void __launch_bounds__(NN_WARPS * 32) node_norm_fwd_kernel(int k, Mod
 // backward glue (warp per node): the per-node phase of node_bwd2_body around the partial products
 // ---------------------------------------------------------------------------------------------------------
 // `split`: the products arrive as one partial per K chunk (3 scalar, 3 + 2 vector) to be summed here; otherwise chunk 0
-// holds the complete product (the GEMM CTA accumulated its chunks in TMEM).
+// holds the complete product (the GEMM CTA accumulated its chunks).
 __global__ void __launch_bounds__(NN_WARPS * 32) node_norm_bwd_kernel(int k, ModelW mw, Workspace ws, float* __restrict__ GQKV,
                                                                       float* __restrict__ GVNMSG, float* __restrict__ GTU, int split) {
     pdl_entry();

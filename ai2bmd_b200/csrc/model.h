@@ -1,4 +1,4 @@
-// Weight table and workspace layout of the ViSNet sm_100a engine (host + device views).
+// Weight table and workspace layout of the ViSNet sm_90a engine (host + device views).
 #pragma once
 #include <cuda_runtime.h>
 #include <stddef.h>

@@ -1,13 +1,13 @@
-// Blackwell (sm_100a) primitives used by the tensor-core edge kernels: mbarrier, 1-D TMA bulk copies,
-// TMEM allocation, tcgen05.mma (kind::tf32, A from TMEM, B from shared memory), tcgen05.ld/st, fences.
-// Inline PTX only (no CUTLASS dependency).  Layout facts used here:
-//   * TMEM address = (lane << 16) | column; a warp w of the row warpgroup may touch lanes 32*(w%4)..+31.
-//     tcgen05.ld/st .32x32b.xN: thread t of the warp <-> lane 32*(w%4)+t, N consecutive 32-bit columns.
-//   * A operand from TMEM (M = 128): row m of A lives in lane m, element k in column (base + k) (tf32 = 32 bit).
+// Hopper (sm_90a) primitives used by the tensor-core kernels: mbarrier, 1-D TMA bulk copies, warpgroup MMA
+// (wgmma.mma_async kind tf32, A from registers, B from shared memory).  Inline PTX only (no CUTLASS dependency).
+// Layout facts used here:
 //   * B operand from shared memory, K-major, 128-byte swizzle: one K-slab = 32 tf32 = 128 B per row;
 //     row n at byte n*128, its 16-byte chunk c stored at chunk position c ^ (n & 7); 8-row groups are
 //     1024 B apart (SBO = 1024).  One MMA consumes K = 8 (32 B): the descriptor start address advances by
-//     32 B per K-step inside the slab.
+//     32 B per K-step inside the slab; rows 64..127 of a plane (the second N = 64 half) start 8 KB in.
+//   * A operand in registers (m64n64k8, per warp 16 rows): a0 = (g, t), a1 = (g + 8, t), a2 = (g, t + 4),
+//     a3 = (g + 8, t + 4) with g = lane / 4, t = lane % 4 (row, k within the warp's 16 x 8 block).
+//   * accumulator (m64n64, f32): d[4i + 0/1] = row g, columns 8i + 2t + 0/1; d[4i + 2/3] = row g + 8, same columns.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -57,74 +57,32 @@ __device__ __forceinline__ void tma_prefetch_l2(const void* gmem_src, uint32_t b
     asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(gmem_src), "r"(bytes) : "memory");
 }
 
-// ---- TMEM allocation (one full warp executes these) -------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// ---- fences / waits -----------------------------------------------------------------------------------
-__device__ __forceinline__ void fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// ---- MMA ----------------------------------------------------------------------------------------------
-// instruction descriptor, kind::tf32, D = F32, A/B = TF32, both K-major, M = 128, N given
-__host__ __device__ constexpr uint32_t idesc_tf32(int M, int N) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-// shared-memory matrix descriptor: K-major, SWIZZLE_128B, SBO = 1024 B, version 1 (sm_100)
+// ---- warpgroup MMA --------------------------------------------------------------------------------------
+// shared-memory matrix descriptor (sm_90): K-major, SWIZZLE_128B, LBO unused (1), SBO = 1024 B
 __device__ __forceinline__ uint64_t smem_desc_sw128(uint32_t saddr) {
-    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
+    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 62);
 }
-// D[tmem_d] (+)= A[tmem_a] * B[desc_b]^T    (issued by ONE thread)
-__device__ __forceinline__ void mma_tf32_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                            uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// keeps a register live and unmodified up to this point (the A fragments of MMAs still in flight)
+__device__ __forceinline__ void reg_fence(uint32_t& r) { asm volatile("" : "+r"(r)::"memory"); }
+__device__ __forceinline__ void reg_fence(float& r) { asm volatile("" : "+f"(r)::"memory"); }
+
+// d[64 x 64] += A[64 x 8] (registers) * B[64 x 8]^T (descriptor), tf32 inputs, f32 accumulation
+__device__ __forceinline__ void mma_m64n64k8_tf32(float (&d)[32], const uint32_t (&a)[4], uint64_t desc_b) {
     asm volatile(
         "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t"
-        "}" ::"r"(tmem_d),
-        "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// all MMAs issued so far by this thread arrive on the mbarrier when they complete
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-// ---- TMEM <-> registers (thread = lane/row, 16 consecutive columns) ------------------------------------
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-    uint32_t r[16];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-    wait_ld();
-#pragma unroll
-    for (int i = 0; i < 16; i++) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_ld16_nowait(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::"r"(taddr),
-        "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-        "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, "
+        "{%32,%33,%34,%35}, %36, 1, 1, 1;\n\t"
+        "}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b)
         : "memory");
 }
 
@@ -133,15 +91,6 @@ __device__ __forceinline__ void split_tf32(float x, uint32_t& hi, uint32_t& lo) 
     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hi) : "f"(x));
     const float rest = x - __uint_as_float(hi);
     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(lo) : "f"(rest));
-}
-
-// store 16 consecutive fp32 values of this thread's row as the A operand (hi and lo planes) starting at column c0
-__device__ __forceinline__ void store_a16(uint32_t tmem_hi, uint32_t tmem_lo, int c0, const float (&v)[16]) {
-    uint32_t hi[16], lo[16];
-#pragma unroll
-    for (int i = 0; i < 16; i++) split_tf32(v[i], hi[i], lo[i]);
-    tmem_st16(tmem_hi + c0, hi);
-    tmem_st16(tmem_lo + c0, lo);
 }
 
 constexpr int SLAB_K = 32;                         // tf32 elements per K-slab (= 128 B, one swizzle row)

@@ -2,7 +2,7 @@
 
 PyTorch is used only as plumbing here (device tensors and streams owned by the caller); the binding
 itself passes raw pointers.  There is no CPU path: constructing an :class:`Engine` without a usable
-sm_100 device raises ``RuntimeError``, and a missing library raises at import of this module's users.
+sm_90 device raises ``RuntimeError``, and a missing library raises at import of this module's users.
 """
 from __future__ import annotations
 
@@ -54,7 +54,7 @@ def load_library(path: Optional[str] = None):
     path = path or _build.LIB_PATH
     if not os.path.exists(path):
         raise RuntimeError(f"{path} is missing: build it with `python -m ai2bmd_b200.build` "
-                           "(nvcc, sm_100a).  The engine has no CPU or PyTorch fallback.")
+                           "(nvcc, sm_90a).  The engine has no CPU or PyTorch fallback.")
     lib = C.CDLL(path)
     vp, i64, i32 = C.c_void_p, C.c_int64, C.c_int32
     lib.vb_weight_manifest.restype = C.c_char_p
@@ -372,7 +372,7 @@ class Engine:
 
 
 def tc_selftest(a: np.ndarray, w_nk: np.ndarray, reps: int = 1, device: int = 0):
-    """Run D = A @ W^T (A [128,128], W [128 out,128 in]) through the tcgen05 pipeline; returns (D, ms)."""
+    """Run D = A @ W^T (A [128,128], W [128 out,128 in]) through the wgmma pipeline; returns (D, ms)."""
     from .weights import tc_image
     lib = load_library()
     a = np.ascontiguousarray(a, dtype=np.float32)

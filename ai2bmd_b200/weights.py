@@ -122,7 +122,7 @@ def pack_weights(sd: Dict[str, np.ndarray], manifest: str) -> np.ndarray:
     return np.concatenate(parts)
 
 
-# ---- tensor-core weight images (tcgen05 path) -------------------------------------------------------------
+# ---- tensor-core weight images (wgmma path) -------------------------------------------------------------
 def round_tf32(x: np.ndarray) -> np.ndarray:
     """Round-to-nearest (ties away) to tf32: keep 10 explicit mantissa bits (PTX ``cvt.rna.tf32.f32``)."""
     b = np.ascontiguousarray(x, dtype=np.float32).view(np.uint32)
@@ -130,7 +130,7 @@ def round_tf32(x: np.ndarray) -> np.ndarray:
 
 
 def tc_image(w_nk: np.ndarray) -> np.ndarray:
-    """Shared-memory image of a GEMM chunk for ``tcgen05.mma`` (B operand, K-major, SWIZZLE_128B).
+    """Shared-memory image of a GEMM chunk for ``wgmma.mma_async`` (B operand, K-major, SWIZZLE_128B).
 
     ``w_nk`` is [128 output columns][K] (K multiple of 32): D[m][n] = sum_k A[m][k] * w_nk[n][k].
     Output: for every K-slab of 32 a 16 KB "hi" plane then a 16 KB "lo" plane (3xTF32 split); inside a plane

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- MD steps/s of the ViSNet energy/force hot path (BASELINE.json metric).
 
-    python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload chig]
+    python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload chig] [--dump-outputs DIR]
 
 A "step" is one pass of the hot path over one batch: neighbour build + ViSNet energy + analytic forces for
 every fragment of the protein + signed reduction to whole-protein energy/forces (what one MD step of the
@@ -18,6 +18,10 @@ BASELINE.json configs[1], Chignolin fully fragmented (19 fragments, 391 fragment
 * ``cpu_baseline`` / ``--impl reference``: the CPU oracle (pure-PyTorch port of the reference model) on the
                host cores -- the reference itself cannot be imported on this image (its third-party graph
                packages are absent), so kind = "port".
+* ``--dump-outputs DIR``: after the timed steps, the whole-protein forces and energy of the last timed step (what
+               ``DeviceShard.step`` hands its caller) as ``DIR/protein_forces.npy`` [n_protein, 3] and
+               ``DIR/protein_energy.npy`` [1], float32; the inputs are fixed by the workload, so two builds compare
+               output for output.
 N>1 (torchrun, one rank per GPU): fragments sharded over ranks (strong scaling: the protein is fixed), one
 NCCL all-reduce of the [3*N_prot+1] buffer per step; time = max over ranks between barriers.
 """
@@ -49,7 +53,13 @@ def parse():
     ap.add_argument("--skip-cpu-baseline", action="store_true")
     ap.add_argument("--nccl", action="store_true", help="N > 1: torch.distributed all-reduce instead of the peer-memory one")
     ap.add_argument("--no-c4", action="store_true", help="N > 1: skip the 512-fragment strong-scaling leg")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step to DIR/<name>.npy (float32)")
+    args = ap.parse_args()
+    if args.dump_outputs and args.impl != "ours":
+        ap.error("--dump-outputs writes the outputs of the engine's timed path; --impl reference times the CPU oracle "
+                 "on a bounded sample of the fragments and has none to write")
+    return args
 
 
 def load_workload(name, n_fragments=512):
@@ -161,7 +171,7 @@ def algorithmic_bytes(stage, n_atoms, n_edges):
 
 
 def tensor_roofline(stages, n_edges, seconds, edge_tc):
-    """Tensor-pipe view of the tcgen05 edge stages (SURVEY 8d: report against the measured bf16 rate, TF32 = 1/2 of it).
+    """Tensor-pipe view of the tensor-core edge stages (SURVEY 8d: report against the measured bf16 rate, TF32 = 1/2 of it).
 
     ``stages`` = names of the launches timed in ``seconds``.  Algorithmic MMA work per edge and layer: forward
     dk, dv, f (3 x 128x128) + s_proj (2 x 128x128), adjoint g_s.Ws (2) + g_P.W1 (3); the last layer has no f chunk.
@@ -179,7 +189,7 @@ def tensor_roofline(stages, n_edges, seconds, edge_tc):
     if os.path.exists(p):
         bf16, kind = float(json.load(open(p))["bf16_tflops_sustained"]), "measured bf16 sustained / 2"
     else:
-        bf16, kind = 1590.0, "fallback bf16 / 2"
+        bf16, kind = 989.0, "H100 SXM data-sheet dense bf16 / 2"
     achieved = 3.0 * fp32_equiv / seconds / 1e12
     return {"bound": "tensor", "achieved": achieved, "peak": bf16 / 2, "peak_kind": kind, "unit": "TFLOP/s",
             "frac": achieved / (bf16 / 2), "fp32_equivalent_tflops": fp32_equiv / seconds / 1e12,
@@ -191,7 +201,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured"
-    return 6650.0, "fallback"
+    return 3350.0, "H100 SXM data sheet"
 
 
 def host_threads():
@@ -296,6 +306,13 @@ def time_shard_steps(torch, dist, shard, steps, warmup, world, flush=None):
     return float(t.item())
 
 
+def dump_outputs(out_dir, ef):
+    """Whole-protein forces and energy of one step (the [3 * n_protein + 1] buffer) as .npy files, float32."""
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "protein_forces.npy"), np.asarray(ef[:-1], dtype=np.float32).reshape(-1, 3))
+    np.save(os.path.join(out_dir, "protein_energy.npy"), np.asarray(ef[-1:], dtype=np.float32))
+
+
 def golden_reference(workload):
     """Outputs of the reference's own model source on this workload (tests/golden/make_golden.py), if committed."""
     path = os.path.join(ROOT, "tests", "golden", "reference_outputs.npz")
@@ -344,6 +361,8 @@ def run_ours(args):
     t_dev = time_shard_steps(torch, dist, shard, args.steps, args.warmup, world, flush)
     wall = time.perf_counter() - wall0
     ef = shard.ef.clone()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, ef.cpu().numpy())
     n_edges_local = int(shard.engine.get_edges()[1].sum()) if shard.engine is not None else 0   # edges of the timed positions
     # ---- warm-L2 variant (diagnostic) ----
     barrier()
@@ -535,14 +554,10 @@ def run_ours(args):
     ab = sum(algorithmic_bytes(n, loc_atoms, n_edges) or 0 for n, _ in launches)
     t_fam = fam_ms[top_fam] * 1e-3
     achieved = (ab / t_fam / 1e9) if ab else None
-    traffic = None      # dram__bytes_read.sum + dram__bytes_write.sum per launch, from the committed ncu --set full capture
-    tpath = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    if os.path.exists(tpath) and world == 1:
-        traffic = json.load(open(tpath)).get(f"{args.workload}:{top_fam}")
     roofline = {"bound": "hbm", "kernel": top_fam, "launches_per_step": len(launches),
                 "kernel_ms": fam_ms[top_fam] / len(launches), "algorithmic_bytes": ab / len(launches) if ab else None,
                 "achieved": achieved, "peak": peak, "peak_kind": peak_kind, "unit": "GB/s",
-                "frac": (achieved / peak) if achieved else None, "traffic": traffic,
+                "frac": (achieved / peak) if achieved else None,
                 "note": "algorithmic bytes = SURVEY 8d fused lower bound per launch (N, E of the timed positions); this stage is "
                         "contraction/latency bound, not HBM bound (DESIGN.md section 5); workloads below ~2k atoms are L2 resident",
                 "share_of_step": fam_ms[top_fam] / total_ms,
@@ -577,7 +592,7 @@ def run_ours(args):
                          f"pure-PyTorch CPU oracle, fp32, {threads} threads (fastest of the candidates tried); "
                          f"scaled by atom count"}
 
-    # ---- B1 (BASELINE.md section 3): the same oracle as eager PyTorch on this B200 -- "the reference on a modern GPU" ----
+    # ---- B1 (BASELINE.md section 3): the same oracle as eager PyTorch on this GPU -- "the reference on a modern GPU" ----
     gpu_eager = None
     if not args.skip_cpu_baseline and world == 1:
         from oracle import visnet_ref as O
@@ -657,8 +672,9 @@ def run_ours(args):
                    "timing": "CUDA events around each step on the launching stream, max over ranks",
                    "cuda_graph": True,
                    "launch_plan": "fused per-layer kernels" if shard.engine.get_option("fused") == 1 else "separate node / edge stages",
-                   "edge_kernels": "tcgen05 (TMEM accumulators, TMA weight ring, 3xTF32)" if edge_tc == 3
-                                   else ("fp32 SIMT" if edge_tc == 0 else f"mixed ({edge_tc})")},
+                   "edge_kernels": {0: "fp32 SIMT", 1: "forward wgmma (TMA weight ring, 3xTF32), adjoint fp32 SIMT",
+                                    2: "forward fp32 SIMT, adjoint wgmma (TMA weight ring, 3xTF32)",
+                                    3: "wgmma (TMA weight ring, 3xTF32)"}[edge_tc]},
         "value_l2_warm": args.steps / float(t_warm.item()),
         "wall_s_timed_region": wall,
         "e2e": e2e,

@@ -1,10 +1,10 @@
-/* visnet_b200.h -- C ABI of the B200-native ViSNet energy/force engine.
+/* visnet_b200.h -- C ABI of the H100-native ViSNet energy/force engine.
  *
  * Drop-in boundary for the one hot path of microsoft/AI2BMD: the per-MD-step ViSNet evaluation over a
  * packed batch of protein fragments.  Each entry point names the reference interface it replaces
  * (paths relative to the reference tree).  Plain pointers and sizes only -- no torch types.  Every
  * function returns 0 on success or a negative vb_status; the message is available from vb_last_error().
- * There is no CPU fallback: every compute entry fails with VB_ERR_CUDA when no sm_100 device is usable.
+ * There is no CPU fallback: every compute entry fails with VB_ERR_CUDA when no sm_90 device is usable.
  *
  * Units/dtypes are the reference's: positions in Angstrom, energies in eV, forces in eV/Angstrom, fp32.
  */
@@ -181,11 +181,11 @@ int vb_get_edges(vb_handle* h, int32_t* slots_host, int32_t* deg_host);
 /* Number of kernel launches of one vb_forward(), and whether it replays a captured CUDA graph. */
 int vb_launches_per_forward(const vb_handle* h);
 /* Tuning knobs: "use_graph" 0/1, "use_pdl" 0/1 (programmatic dependent launch between the stages, default off), "npw" 1/2, "te_fwd" 32/64, "te_bwd" 32/64, "node_impl" 0/1,
- * "edge_tc" bit0 = forward / bit1 = adjoint edge stage on tcgen05, "tc_rows" 32/64/96/128 fixed edges per tcgen05 tile
+ * "edge_tc" bit0 = forward / bit1 = adjoint edge stage on tensor cores (default 1: forward only), "tc_rows" 32/64/96/128 fixed edges per tensor-core tile
  * (0 = default: tile length planned so the tiles fill whole waves of CTAs, from an estimate of 17 edges per atom or,
- * after "calibrate" 1, from the edge count of the last evaluation -- synchronises), "timeline" 0/1 in-kernel phase stamps of the tcgen05 edge kernels and the SIMT node kernels (vb_debug_read "TL" / "TLN"),
+ * after "calibrate" 1, from the edge count of the last evaluation -- synchronises), "timeline" 0/1 in-kernel phase stamps of the tensor-core edge kernels and the SIMT node kernels (vb_debug_read "TL" / "TLN"),
  * "fused" 0/1 one launch per layer and direction (edge stage + node stage of a 4-node block; default off), "node_tc" 0/1
- * node stage on tcgen05 (default: from 600 atoms), "node_nb" 0/1/2/3/4/8 nodes per CTA of the SIMT node kernels (0 = the
+ * node stage on tensor cores (default: from 600 atoms), "node_nb" 0/1/2/3/4/8 nodes per CTA of the SIMT node kernels (0 = the
  * fewest that fit one wave), "krot" 0/1 every CTA of the SIMT node kernels walks the K dimension of its weight chunks from a
  * different row (default 1: the CTAs of a wave otherwise ask the same L2 slices for the same rows at the same time),
  * "embed_batch" -1/0..3 batch variants of the embedding kernels, "comm_auto" 0/1.  vb_get_option also answers "edge_overflow" (1 after a step exceeded a trimmed max_edges),
@@ -201,7 +201,7 @@ int vb_debug_run(vb_handle* h, const float* pos_dev, int n_stages);
 /* Per-launch device time (ms, CUDA events on the launching stream, average of n_iter eager evaluations after
  * one warm-up) for each of the vb_num_stages() launches; used by bench.py for the live roofline numbers. */
 int vb_profile_stages(vb_handle* h, const float* pos_dev, int n_iter, float* ms_per_stage_host);
-/* Self-test of the tcgen05/TMEM/TMA GEMM pipeline: d[128][128] = a[128][128] * W^T, W given as a tensor-core
+/* Self-test of the wgmma/TMA GEMM pipeline: d[128][128] = a[128][128] * W^T, W given as a tensor-core
  * weight image (ai2bmd_b200.weights.tc_image); repeated `reps` times inside one launch; *ms_out = kernel time. */
 int vb_tc_selftest(int device, const float* a_host, const float* img_host, float* d_host, int reps, float* ms_out);
 /* Copy an internal buffer to the host.  name: "X","V","F","VN","QKV","V123","VDOT","TU","O" (per layer),

@@ -14,7 +14,7 @@ sys.path.insert(0, os.path.join(ROOT, "tools"))
 pytestmark = pytest.mark.gpu
 
 
-@pytest.mark.parametrize("opts", ["fused=0", "fused=1", "fused=0,edge_tc=0", "node_tc=1",
+@pytest.mark.parametrize("opts", ["fused=0", "fused=1", "fused=0,edge_tc=0", "fused=0,edge_tc=3", "node_tc=1",
                                   "node_nb=2", "node_nb=3", "node_nb=4", "node_nb=8"])     # default here: node_nb=1 (one wave)
 @pytest.mark.parametrize("weights", ["real", "3"])
 def test_every_stage_against_the_fp64_adjoint_oracle(opts, weights):

@@ -2,7 +2,7 @@
 """Per-launch device times of one evaluation (CUDA events inside the library, eager launches) and the graph-replay time,
 for a workload and a set of engine options.  GPU box diagnostic:
 
-    python tools/stage_times.py --workload chig --opts fused=1 [--out profiles/r02_stages_19frag.txt]
+    python tools/stage_times.py --workload chig --opts fused=1 [--out stages.txt]
 """
 import argparse
 import os

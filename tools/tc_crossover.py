@@ -1,11 +1,11 @@
 #!/usr/bin/env python
-"""Where do the tcgen05 edge kernels start to pay?  Sweep the fragment count of the synthetic batch and time one
+"""Where do the tensor-core edge kernels start to pay?  Sweep the fragment count of the synthetic batch and time one
 evaluation (CUDA events, L2 flushed) with edge_tc = 0 (SIMT), 1 (TC forward), 3 (TC forward + adjoint) at every tile
 length, and with the engine's automatic choice.
 
     python tools/tc_crossover.py [--fragments 1,2,4,8,12,19,32] [--steps 40]
 
-The engine's automatic policy (engine.cu choose_defaults) is set from this table (profiles/README.md).
+The engine's automatic policy (engine.cu choose_defaults) is meant to follow this table.
 """
 import argparse
 import os

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""GPU self-test of the tcgen05/TMEM/TMA GEMM pipeline against fp64 numpy (run under `timeout`)."""
+"""GPU self-test of the wgmma/TMA GEMM pipeline against fp64 numpy (run under `timeout`)."""
 import os
 import sys
 

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""In-kernel timeline of the tcgen05 edge kernels: SM-clock stamps taken by CTA 0 (first tile) at every phase
+"""In-kernel timeline of the tensor-core edge kernels: SM-clock stamps taken by CTA 0 (first tile) at every phase
 boundary (engine option "timeline"; slots documented next to TC_TL in csrc/k_edge_tc.cuh).
 
     python tools/tc_timeline.py [--workload chig] [--layer 2] [--mhz 1920]
@@ -21,16 +21,16 @@ from ai2bmd_b200.fixtures import WEIGHTS, load_fragments   # noqa: E402
 from ai2bmd_b200.synth import synthetic_batch    # noqa: E402
 from ai2bmd_b200.weights import load_state_dict  # noqa: E402
 
-FWD = {0: "kernel start", 1: "setup done (barriers, TMEM alloc)", 2: "f tile + meta loaded", 3: "A=f in TMEM, go dk/dv",
-       4: "dk done seen", 5: "D0 -> tile", 6: "attention weights done", 7: "dv done seen", 8: "D1 -> tile",
-       9: "messages m done", 10: "xa aggregation done", 11: "A=m in TMEM, go s1", 12: "edge update (f) done",
-       13: "s1 done seen", 14: "D1 -> tile", 15: "s1 aggregation done", 16: "s2 done seen", 17: "D0 -> tile",
+FWD = {0: "kernel start", 1: "setup done (barriers)", 2: "f tile + meta loaded", 3: "A=f copied",
+       4: "dk MMAs done", 5: "dk -> tile", 6: "attention weights done", 7: "dv MMAs done", 8: "dv -> tile",
+       9: "messages m done", 10: "xa aggregation done", 11: "A=m copied", 12: "edge update (f) done",
+       13: "s1 MMAs done", 14: "s1 -> tile", 15: "s1 aggregation done", 16: "s2 MMAs done", 17: "s2 -> tile",
        18: "s2 aggregation done", 31: "teardown done"}
-BWD = {0: "kernel start", 1: "setup done", 2: "meta loaded", 3: "s1-half SIMT done", 4: "A in TMEM, go g3a",
-       5: "s2-half SIMT done", 6: "g3a done seen", 7: "A in TMEM, go g3b", 8: "g3b done seen", 9: "D1 -> tile",
-       10: "g_m / g_Pdv SIMT done", 11: "A in TMEM, go g4dv", 12: "g_Pdk SIMT done", 13: "g4dv done seen",
-       14: "A in TMEM, go g4dk", 15: "g_q tile + aggregation done", 16: "g_Pf SIMT done", 17: "g4dk done seen",
-       18: "A in TMEM, go g4f", 19: "g_wdot tile + aggregation done", 20: "last job done seen", 21: "D0 -> tile",
+BWD = {0: "kernel start", 1: "setup done", 2: "meta loaded", 3: "s1-half SIMT done", 4: "A copied (g3a)",
+       5: "s2-half SIMT done", 6: "g3a MMAs done", 7: "A copied (g3b)", 8: "g3b MMAs done", 9: "g_m -> tile",
+       10: "g_m / g_Pdv SIMT done", 11: "A copied (g4dv)", 12: "g_Pdk SIMT done", 13: "g4dv MMAs done",
+       14: "A copied (g4dk)", 15: "g_q tile + aggregation done", 16: "g_Pf SIMT done", 17: "g4dk MMAs done",
+       18: "A copied (g4f)", 19: "g_wdot tile + aggregation done", 20: "last job MMAs done", 21: "g_f -> tile",
        22: "g_f written", 31: "teardown done"}
 
 
@@ -39,7 +39,7 @@ NFWD = {0: "start", 1: "xa rows staged", 2: "o_proj unit done", 4: "K-quarters s
 NBWD = {0: "start", 1: "A rows staged", 3: "adjoint unit done", 5: "per-node phase done", 7: "o_proj adjoint unit done", 9: "g_xa written"}
 
 
-def show(title, tl, names, mhz, jobs):
+def show(title, tl, names, mhz):
     t0 = int(tl[0])
     print(f"--- {title} ---")
     prev = t0
@@ -49,10 +49,6 @@ def show(title, tl, names, mhz, jobs):
         t = int(tl[k])
         print(f"  [{k:2d}] {names[k]:<36} {(t - t0) / mhz:8.2f} us   (+{(t - prev) / mhz:6.2f})")
         prev = t
-    for j in range(jobs):
-        a, b = int(tl[32 + 2 * j]), int(tl[33 + 2 * j])
-        if a:
-            print(f"  issuer job {j}: go seen {(a - t0) / mhz:8.2f} us, MMAs issued {(b - t0) / mhz:8.2f} us (+{(b - a) / mhz:5.2f})")
 
 
 def main():
@@ -88,8 +84,8 @@ def main():
     nl = 6
     tf = eng.debug_read("TL", args.layer, (64,), dtype=np.uint64)
     tb = eng.debug_read("TL", nl + args.layer, (64,), dtype=np.uint64)
-    show("edge_fwd_tc", tf, FWD, mhz, 5)
-    show("edge_bwd_tc", tb, BWD, mhz, 5)
+    show("edge_fwd_tc", tf, FWD, mhz)
+    show("edge_bwd_tc", tb, BWD, mhz)
     if eng.get_option("node_tc") == 0 and eng.get_option("fused") == 0:
         EMB = {0: "start", 1: "previous kernel complete (pdl)", 2: "loads issued, rows staged", 3: "aggregation done", 4: "combine done", 5: "x written"}
         for title, idx, names in ((f"node_fwd2 stage {args.layer}", args.layer, NFWD), (f"node_bwd2 stage {args.layer}", nl + 1 + args.layer, NBWD),
