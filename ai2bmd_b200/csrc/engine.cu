@@ -937,20 +937,23 @@ void choose_defaults(vb_handle* h) {
     const int N = h->ws.N;
     h->npw = h->npw_opt; h->te_fwd = h->te_fwd_opt; h->edge_tc = h->edge_tc_opt;
     // fused per-layer launches (k_fused.cuh) are opt-in: inside a graph a launch boundary costs little, and the fused kernels
-    // run the node stage under the 96-register budget of the tensor-core CTA
+    // run the node stage under the 128-register budget of the tensor-core CTA (fused_bwd spills)
     h->fused = h->fused_opt >= 0 ? h->fused_opt : 0;
     // node stage on tensor cores from ~600 atoms on: the three-launch stage has a higher fixed latency than the single SIMT
-    // kernel, which wins on small systems (threshold not yet re-measured on H100)
+    // kernel, which wins on small systems (H100, 700 W, graph replay, SIMT vs tensor-core node stage: Chignolin, 391 atoms,
+    // 0.96 vs 1.12 ms; Trp-cage, 737 atoms, 1.48 vs 1.43 ms)
     h->node_tc = h->node_tc_opt >= 0 ? h->node_tc_opt : (N >= 600 ? 1 : 0);
     if (h->fused) h->node_tc = 0;
     set_gxa_parts(h);
     if (h->npw == 0) h->npw = (N > 4096) ? 2 : 1;
     if (h->te_fwd == 0) h->te_fwd = ((long long)N * 17 / 64 >= 2LL * h->sm_count) ? 64 : 32;
-    // forward edge stage on tensor cores, adjoint edge stage on the fp32 SIMT kernel.  Measured per launch on an H100
-    // (tools/stage_times.py, 700 W): forward wgmma 60 us vs SIMT 80 us on Chignolin, 1.32 vs 1.57 ms on the 512-fragment
-    // batch; adjoint wgmma 103 us vs SIMT 72 us, 2.55 vs 2.00 ms -- the wgmma adjoint keeps its accumulator live across
-    // SIMT phases under the 96-register budget of its 17-warp CTA and spills.  "edge_tc" 0..3 selects any combination.
-    if (h->edge_tc < 0) h->edge_tc = 1;
+    // both edge stages on tensor cores.  The 512-thread CTA (no producer warp, 128 registers) keeps the adjoint's
+    // accumulator in registers without spilling, and the adjoint then beats the fp32 SIMT kernel on every workload.
+    // Measured on one H100 80GB HBM3 at 700 W (tools/stage_times.py, graph replay per evaluation, edge_tc 1 -> 3):
+    // Chignolin 988 -> 948 us (adjoint 72 -> 67 us per launch), Trp-cage 1.73 -> 1.42 ms, WW 2.78 -> 2.54 ms,
+    // ABD 3.70 -> 3.30 ms, the 512-fragment batch 22.2 -> 19.7 ms (adjoint 1.98 -> 1.54 ms per launch), C5 86.0 -> 76.8 ms.
+    // "edge_tc" 0..3 still selects any combination.
+    if (h->edge_tc < 0) h->edge_tc = 3;
     plan_tiles(h, h->edges_plan > 0 ? h->edges_plan : (long long)N * 17);
 }
 
@@ -1793,8 +1796,13 @@ int vb_profile_stages(vb_handle* h, const float* pos_dev, int n_iter, float* ms_
 }
 
 int vb_tc_selftest(int device, const float* a_host, const float* img_host, float* d_host, int reps, float* ms_out) {
-    // D[128][128] = A[128][128] * W^T through the wgmma / TMA pipeline of the tensor-core edge kernels.
-    if (!a_host || !img_host || !d_host || reps <= 0) return VB_ERR_ARG;
+    return vb_tc_selftest_rows(device, TC_TE, a_host, img_host, d_host, reps, ms_out);
+}
+
+int vb_tc_selftest_rows(int device, int rows, const float* a_host, const float* img_host, float* d_host, int reps, float* ms_out) {
+    // D[rows][128] = A[rows][128] * W^T through the wgmma / TMA pipeline of the tensor-core edge kernels (tile capacity
+    // `rows`: 32 / 64 run the three-stage ring, 128 the two-stage one); A and D are [128][128], rows past `rows` unused.
+    if (!a_host || !img_host || !d_host || reps <= 0 || (rows != 32 && rows != 64 && rows != TC_TE)) return VB_ERR_ARG;
     if (cudaSetDevice(device) != cudaSuccess) { g_create_error = "vb_tc_selftest: cudaSetDevice failed"; return VB_ERR_CUDA; }
     float *dA = nullptr, *dI = nullptr, *dD = nullptr;
     const size_t nA = (size_t)TC_TE * D * sizeof(float), nI = (size_t)(D / tc::SLAB_K) * tc::STAGE_BYTES;
@@ -1802,11 +1810,13 @@ int vb_tc_selftest(int device, const float* a_host, const float* img_host, float
     cudaMemcpy(dA, a_host, nA, cudaMemcpyHostToDevice);
     cudaMemcpy(dI, img_host, nI, cudaMemcpyHostToDevice);
     cudaMemset(dD, 0, nA);
-    cudaFuncSetAttribute(tc_selftest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM_BYTES);
+    void (*kernel)(const float*, const float*, float*, int) =
+        rows == 32 ? tc_selftest_kernel<32> : rows == 64 ? tc_selftest_kernel<64> : tc_selftest_kernel<TC_TE>;
+    cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM_BYTES);
     cudaEvent_t e0, e1;
     cudaEventCreate(&e0); cudaEventCreate(&e1);
     cudaEventRecord(e0);
-    tc_selftest_kernel<<<1, TC2_THREADS, TC_SMEM_BYTES>>>(dA, dI, dD, reps);
+    kernel<<<1, TC2_THREADS, TC_SMEM_BYTES>>>(dA, dI, dD, reps);
     cudaEventRecord(e1);
     cudaError_t err = cudaDeviceSynchronize();
     float ms = 0.f;

@@ -62,85 +62,81 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) node_tc_kernel(const __grid_co
         j.accumulate = (KCHUNKS && threadIdx.x > 0) ? 1 : 0;
         jl[threadIdx.x] = j;
     }
-    tc2_setup(sh);                                     // (its __syncthreads publishes jl)
+    TcRing<TC_TE> ring;
+    tc2_setup(sh, ring, jl, nj, 1);                    // (its __syncthreads publishes jl)
 
-    if (warp == TC2_CWARPS) {
-        if (lane == 0) tc_producer(sh, jl, nj, 1);
-    } else {
-        TcRing ring;
-        float acc[32];
-        // A operand rows of job jj -> staging tile (warp per row, lane owns 4 channels: coalesced 512 B rows)
-        auto load_a = [&](int jj) {
-            for (int r = warp; r < nvalid; r += TC2_CWARPS) {
-                const size_t row = (size_t)(row0 + r);
-                float4 v;
-                if (MODE == NT_OPROJ) {
-                    v = ld4(ws.XA + row * D + col);
-                } else if (MODE == NT_PROJ) {
-                    v = is_x ? ld4(ws.XN + row * D + col) : ld4(ws.VN[k] + row * D + col);
-                } else if (MODE == NT_BWDA) {
-                    if (is_x) {
-                        v = ld4(a.acc_qkv + row * 3 * D + jj * D + col);
-                    } else if (jj >= 3) {
-                        v = ld4(a.acc_tu + row * 2 * D + (jj - 3) * D + col);
-                    } else {
-                        const size_t node = row / 3;
-                        const float* orow = ws.O[k] + node * 3 * D;
-                        if (jj == 2) {
-                            v = ld4(ws.GVEC + row * D + col) * ld4(orow + col);                         // g_vec * o1
-                        } else {
-                            const float4 g_vdot = ld4(ws.GX + node * D + col) * ld4(orow + D + col);    // g_x * o2
-                            v = g_vdot * ld4(ws.V123[k] + row * 3 * D + (jj == 0 ? D : 0) + col);       // * v2 | * v1
-                        }
-                    }
+    float acc[32];
+    // A operand rows of job jj -> staging tile (warp per row, lane owns 4 channels: coalesced 512 B rows)
+    auto load_a = [&](int jj) {
+        for (int r = warp; r < nvalid; r += TC2_CWARPS) {
+            const size_t row = (size_t)(row0 + r);
+            float4 v;
+            if (MODE == NT_OPROJ) {
+                v = ld4(ws.XA + row * D + col);
+            } else if (MODE == NT_PROJ) {
+                v = is_x ? ld4(ws.XN + row * D + col) : ld4(ws.VN[k] + row * D + col);
+            } else if (MODE == NT_BWDA) {
+                if (is_x) {
+                    v = ld4(a.acc_qkv + row * 3 * D + jj * D + col);
+                } else if (jj >= 3) {
+                    v = ld4(a.acc_tu + row * 2 * D + (jj - 3) * D + col);
                 } else {
-                    v = ld4(ws.GO + row * 3 * D + jj * D + col);
-                }
-                st4(&sh.tile[r][col], v);
-            }
-        };
-        if (!KCHUNKS) {
-            // ---- column chunks of one product: one A operand ----
-            load_a(0);
-            tc2_tile_to_a(sh, nvalid);
-            for (int j = 0; j < nj; j++) {
-                tc2_mma(sh, ring, acc, jl[j].accumulate, warp, lane, nvalid);
-                csync();                                          // the tile is free (A copied / previous chunk stored)
-                tc2_acc_to_tile(sh, acc, warp, lane, nvalid);
-                csync();
-                const int jj = j0 + j;
-                for (int r = warp; r < nvalid; r += TC2_CWARPS) {
-                    const size_t row = (size_t)(row0 + r);
-                    const float4 v = ld4(&sh.tile[r][col]);
-                    if (MODE == NT_OPROJ) {
-                        st4(ws.O[k - 1] + row * 3 * D + jj * D + col, v + ldg4(a.mw.layer[k - 1].bo + jj * D + col));
+                    const size_t node = row / 3;
+                    const float* orow = ws.O[k] + node * 3 * D;
+                    if (jj == 2) {
+                        v = ld4(ws.GVEC + row * D + col) * ld4(orow + col);                         // g_vec * o1
                     } else {
-                        if (is_x) st4(ws.QKV[k] + row * 3 * D + jj * D + col, v + ldg4(a.mw.layer[k].bqkv + jj * D + col));
-                        else if (jj < 3) st4(ws.V123[k] + row * 3 * D + jj * D + col, v);
-                        else st4(ws.TU[k] + row * 2 * D + (jj - 3) * D + col, v);
+                        const float4 g_vdot = ld4(ws.GX + node * D + col) * ld4(orow + D + col);    // g_x * o2
+                        v = g_vdot * ld4(ws.V123[k] + row * 3 * D + (jj == 0 ? D : 0) + col);       // * v2 | * v1
                     }
                 }
+            } else {
+                v = ld4(ws.GO + row * 3 * D + jj * D + col);
             }
-        } else {
-            // ---- K chunks of one product: every chunk has its own A operand, all accumulate into one product; with one
-            //      chunk per CTA the result is the partial of chunk j0 (the glue kernel / the edge adjoint sums the partials) ----
-            for (int j = 0; j < nj; j++) {
-                load_a(j0 + j);                                   // (the previous chunk's MMAs began with a barrier: tile free)
-                tc2_tile_to_a(sh, nvalid);
-                tc2_mma(sh, ring, acc, jl[j].accumulate, warp, lane, nvalid);
-            }
-            csync();
+            st4(&sh.tile[r][col], v);
+        }
+    };
+    if (!KCHUNKS) {
+        // ---- column chunks of one product: one A operand ----
+        load_a(0);
+        tc2_tile_to_a(sh, nvalid);
+        for (int j = 0; j < nj; j++) {
+            tc2_mma(sh, ring, acc, jl[j].accumulate, warp, lane, nvalid);
+            csync();                                          // the tile is free (A copied / previous chunk stored)
             tc2_acc_to_tile(sh, acc, warp, lane, nvalid);
             csync();
+            const int jj = j0 + j;
             for (int r = warp; r < nvalid; r += TC2_CWARPS) {
                 const size_t row = (size_t)(row0 + r);
                 const float4 v = ld4(&sh.tile[r][col]);
-                if (MODE == NT_BWDA) {
-                    if (is_x) st4(ws.PX + ((size_t)j0 * ws.N + row) * D + col, v);
-                    else st4(ws.PV + ((size_t)j0 * 3 * ws.N + row) * D + col, v);
+                if (MODE == NT_OPROJ) {
+                    st4(ws.O[k - 1] + row * 3 * D + jj * D + col, v + ldg4(a.mw.layer[k - 1].bo + jj * D + col));
                 } else {
-                    st4(ws.GXA + ((size_t)j0 * ws.N + row) * D + col, v);
+                    if (is_x) st4(ws.QKV[k] + row * 3 * D + jj * D + col, v + ldg4(a.mw.layer[k].bqkv + jj * D + col));
+                    else if (jj < 3) st4(ws.V123[k] + row * 3 * D + jj * D + col, v);
+                    else st4(ws.TU[k] + row * 2 * D + (jj - 3) * D + col, v);
                 }
+            }
+        }
+    } else {
+        // ---- K chunks of one product: every chunk has its own A operand, all accumulate into one product; with one
+        //      chunk per CTA the result is the partial of chunk j0 (the glue kernel / the edge adjoint sums the partials) ----
+        for (int j = 0; j < nj; j++) {
+            load_a(j0 + j);                                   // (the previous chunk's MMAs began with a barrier: tile free)
+            tc2_tile_to_a(sh, nvalid);
+            tc2_mma(sh, ring, acc, jl[j].accumulate, warp, lane, nvalid);
+        }
+        csync();
+        tc2_acc_to_tile(sh, acc, warp, lane, nvalid);
+        csync();
+        for (int r = warp; r < nvalid; r += TC2_CWARPS) {
+            const size_t row = (size_t)(row0 + r);
+            const float4 v = ld4(&sh.tile[r][col]);
+            if (MODE == NT_BWDA) {
+                if (is_x) st4(ws.PX + ((size_t)j0 * ws.N + row) * D + col, v);
+                else st4(ws.PV + ((size_t)j0 * 3 * ws.N + row) * D + col, v);
+            } else {
+                st4(ws.GXA + ((size_t)j0 * ws.N + row) * D + col, v);
             }
         }
     }

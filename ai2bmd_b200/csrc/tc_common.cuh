@@ -30,6 +30,13 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t by
                  "r"(bytes)
                  : "memory");
 }
+// shared-memory counter add, acquire-release at CTA scope (orders a warp's retired reads of a ring stage before the refill
+// that the last releasing warp issues); returns the old value
+__device__ __forceinline__ uint32_t atom_add_acq_rel(uint32_t* p, uint32_t v) {
+    uint32_t old;
+    asm volatile("atom.acq_rel.cta.shared::cta.add.u32 %0, [%1], %2;" : "=r"(old) : "r"(smem_u32(p)), "r"(v) : "memory");
+    return old;
+}
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     asm volatile(
         "{\n\t"

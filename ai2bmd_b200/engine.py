@@ -38,7 +38,7 @@ class _CaphProblem(C.Structure):
 EXPORTED_SYMBOLS = [
     "vb_weight_manifest", "vb_create", "vb_destroy", "vb_last_error", "vb_set_topology", "vb_forward",
     "vb_forward_host", "vb_set_protein_map", "vb_forward_protein", "vb_get_edges", "vb_launches_per_forward",
-    "vb_set_option", "vb_get_option", "vb_num_stages", "vb_stage_name", "vb_debug_run", "vb_debug_read", "vb_profile_stages", "vb_tc_selftest",
+    "vb_set_option", "vb_get_option", "vb_num_stages", "vb_stage_name", "vb_debug_run", "vb_debug_read", "vb_profile_stages", "vb_tc_selftest", "vb_tc_selftest_rows",
     "vb_md_setup", "vb_md_set_normals", "vb_md_set_state", "vb_md_kick1", "vb_md_eval", "vb_md_kick2", "vb_md_run", "vb_md_get_state",
     "vb_set_nonbonded", "vb_nonbonded",
     "vb_comm_init", "vb_comm_connect", "vb_comm_allreduce",
@@ -93,6 +93,8 @@ def load_library(path: Optional[str] = None):
     lib.vb_profile_stages.argtypes = [vp, vp, C.c_int, vp]
     lib.vb_tc_selftest.restype = C.c_int
     lib.vb_tc_selftest.argtypes = [C.c_int, vp, vp, vp, C.c_int, vp]
+    lib.vb_tc_selftest_rows.restype = C.c_int
+    lib.vb_tc_selftest_rows.argtypes = [C.c_int, C.c_int, vp, vp, vp, C.c_int, vp]
     lib.vb_debug_read.restype = i64
     lib.vb_debug_read.argtypes = [vp, C.c_char_p, C.c_int, vp, i64]
     lib.vb_md_setup.restype = C.c_int
@@ -371,15 +373,17 @@ class Engine:
         return out
 
 
-def tc_selftest(a: np.ndarray, w_nk: np.ndarray, reps: int = 1, device: int = 0):
-    """Run D = A @ W^T (A [128,128], W [128 out,128 in]) through the wgmma pipeline; returns (D, ms)."""
+def tc_selftest(a: np.ndarray, w_nk: np.ndarray, reps: int = 1, device: int = 0, rows: int = 128):
+    """Run D = A @ W^T (A [rows,128], W [128 out,128 in]) through the wgmma pipeline of a tile capacity of `rows`
+    (32, 64: three-stage weight ring; 128: two stages); returns (D [rows,128], ms)."""
     from .weights import tc_image
     lib = load_library()
-    a = np.ascontiguousarray(a, dtype=np.float32)
+    a_full = np.zeros((128, 128), dtype=np.float32)
+    a_full[:rows] = np.asarray(a, dtype=np.float32)[:rows]
     img = tc_image(w_nk)
     d = np.zeros((128, 128), dtype=np.float32)
     ms = C.c_float(0)
-    rc = lib.vb_tc_selftest(int(device), a.ctypes.data, img.ctypes.data, d.ctypes.data, int(reps), C.byref(ms))
+    rc = lib.vb_tc_selftest_rows(int(device), int(rows), a_full.ctypes.data, img.ctypes.data, d.ctypes.data, int(reps), C.byref(ms))
     if rc != 0:
-        raise RuntimeError(f"vb_tc_selftest failed ({rc}): {lib.vb_last_error(None).decode()}")
-    return d, float(ms.value)
+        raise RuntimeError(f"vb_tc_selftest_rows failed ({rc}): {lib.vb_last_error(None).decode()}")
+    return d[:rows], float(ms.value)

@@ -181,7 +181,7 @@ int vb_get_edges(vb_handle* h, int32_t* slots_host, int32_t* deg_host);
 /* Number of kernel launches of one vb_forward(), and whether it replays a captured CUDA graph. */
 int vb_launches_per_forward(const vb_handle* h);
 /* Tuning knobs: "use_graph" 0/1, "use_pdl" 0/1 (programmatic dependent launch between the stages, default off), "npw" 1/2, "te_fwd" 32/64, "te_bwd" 32/64, "node_impl" 0/1,
- * "edge_tc" bit0 = forward / bit1 = adjoint edge stage on tensor cores (default 1: forward only), "tc_rows" 32/64/96/128 fixed edges per tensor-core tile
+ * "edge_tc" bit0 = forward / bit1 = adjoint edge stage on tensor cores (default 3: both), "tc_rows" 32/64/96/128 fixed edges per tensor-core tile
  * (0 = default: tile length planned so the tiles fill whole waves of CTAs, from an estimate of 17 edges per atom or,
  * after "calibrate" 1, from the edge count of the last evaluation -- synchronises), "timeline" 0/1 in-kernel phase stamps of the tensor-core edge kernels and the SIMT node kernels (vb_debug_read "TL" / "TLN"),
  * "fused" 0/1 one launch per layer and direction (edge stage + node stage of a 4-node block; default off), "node_tc" 0/1
@@ -204,6 +204,9 @@ int vb_profile_stages(vb_handle* h, const float* pos_dev, int n_iter, float* ms_
 /* Self-test of the wgmma/TMA GEMM pipeline: d[128][128] = a[128][128] * W^T, W given as a tensor-core
  * weight image (ai2bmd_b200.weights.tc_image); repeated `reps` times inside one launch; *ms_out = kernel time. */
 int vb_tc_selftest(int device, const float* a_host, const float* img_host, float* d_host, int reps, float* ms_out);
+/* The same for a tile capacity of `rows` (32, 64 or 128): only the first `rows` rows of a and d are used; 32 and 64 run the
+ * three-stage weight ring of the small-tile edge kernels. */
+int vb_tc_selftest_rows(int device, int rows, const float* a_host, const float* img_host, float* d_host, int reps, float* ms_out);
 /* Copy an internal buffer to the host.  name: "X","V","F","VN","QKV","V123","VDOT","TU","O" (per layer),
  * "XA","VA","GX","GVEC","GF","GXA","GQKV","GVNMSG","GTU","GQKV2","GVNMSG2","GTU2","geom","rbf","eacc","grbf","esrc","edst","rowptr",
  * "eatom","energy","forces".  Returns the number of bytes copied (<= cap_bytes) or a negative status. */

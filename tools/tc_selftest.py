@@ -28,4 +28,11 @@ for case, (a, w) in {
               " ref:", ref[tuple(bad[0])] if len(bad) else None)
 d, ms = tc_selftest(a, w, reps=200)
 print(f"200 reps in one launch: {ms:.3f} ms -> {ms / 200 * 1e3:.2f} us per 128x128x128 3xTF32 GEMM incl. A store + D load")
+# tile capacities of <= 64 rows run the three-stage weight ring; 7 reps wrap it with both barrier parities
+for rows in (64, 32):
+    d, ms = tc_selftest(a, w, reps=7, rows=rows)
+    ref = a[:rows].astype(np.float64) @ w.astype(np.float64).T
+    rel = np.abs(d - ref).max() / np.abs(ref).max()
+    print(f"rows {rows:3d}, 7 reps: rel err {rel:.2e}; {ms:.3f} ms")
+    ok = ok and rel < 2e-6
 print("SELFTEST", "PASS" if ok else "FAIL")

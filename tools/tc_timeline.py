@@ -21,14 +21,14 @@ from ai2bmd_b200.fixtures import WEIGHTS, load_fragments   # noqa: E402
 from ai2bmd_b200.synth import synthetic_batch    # noqa: E402
 from ai2bmd_b200.weights import load_state_dict  # noqa: E402
 
-FWD = {0: "kernel start", 1: "setup done (barriers)", 2: "f tile + meta loaded", 3: "A=f copied",
+FWD = {0: "kernel start", 1: "setup done (barriers)", 2: "f rows (= A) + meta loaded",
        4: "dk MMAs done", 5: "dk -> tile", 6: "attention weights done", 7: "dv MMAs done", 8: "dv -> tile",
        9: "messages m done", 10: "xa aggregation done", 11: "A=m copied", 12: "edge update (f) done",
        13: "s1 MMAs done", 14: "s1 -> tile", 15: "s1 aggregation done", 16: "s2 MMAs done", 17: "s2 -> tile",
        18: "s2 aggregation done", 31: "teardown done"}
-BWD = {0: "kernel start", 1: "setup done", 2: "meta loaded", 3: "s1-half SIMT done", 4: "A copied (g3a)",
+BWD = {0: "kernel start", 1: "setup done", 2: "meta loaded", 3: "s1-half SIMT done (= A of g3a)",
        5: "s2-half SIMT done", 6: "g3a MMAs done", 7: "A copied (g3b)", 8: "g3b MMAs done", 9: "g_m -> tile",
-       10: "g_m / g_Pdv SIMT done", 11: "A copied (g4dv)", 12: "g_Pdk SIMT done", 13: "g4dv MMAs done",
+       10: "g_m / g_Pdv SIMT done (= A of g4dv)", 12: "g_Pdk SIMT done", 13: "g4dv MMAs done",
        14: "A copied (g4dk)", 15: "g_q tile + aggregation done", 16: "g_Pf SIMT done", 17: "g4dk MMAs done",
        18: "A copied (g4f)", 19: "g_wdot tile + aggregation done", 20: "last job MMAs done", 21: "g_f -> tile",
        22: "g_f written", 31: "teardown done"}
