@@ -16,7 +16,6 @@
 #include "k_caph.cuh"
 #include "k_comm.cuh"
 #include "k_edge_tc.cuh"
-#include "k_fused.cuh"
 #include "k_graph_embed.cuh"
 #include <nvtx3/nvToolsExt.h>
 #include "k_head.cuh"
@@ -165,8 +164,6 @@ struct vb_handle {
     long long edges_plan = 0;                            // edge count the tile length was planned for (estimate or calibrated)
     int krot = 1;      // rotate the K loops of the SIMT node GEMM units per CTA (L2 slice hot-spotting: all CTAs walk the same weights)
     int node_nb = 0;   // nodes per CTA of the CTA-cooperative SIMT node kernels (0 = automatic)
-    int node_impl = 1; // 0: warp-per-node kernels (k_node.cuh), 1: CTA-cooperative kernels (k_node2.cuh)
-    int fused = 0, fused_opt = -1;   // 1: one launch per layer and direction (k_fused.cuh); -1 = choose by problem size
     int node_tc = 0, node_tc_opt = -1;   // 1: node stage on tensor cores (k_node_tc.cuh); -1 = choose by problem size
     int embed_batch_opt = -1;            // embedding kernels: several nodes per CTA (1), one (0), by size (-1)
     int edge_tc = -1;  // bit 0: forward edge stage on tensor cores, bit 1: adjoint edge stage on tensor cores; -1 = by size
@@ -336,9 +333,6 @@ void layout_workspace(vb_handle* h, char* base, ArenaPlan& plan, int*& z, int*& 
     carve(plan, base, ws.GQKV, N * 3 * D);
     carve(plan, base, ws.GVNMSG, N * 3 * D);
     carve(plan, base, ws.GTU, N * 6 * D);
-    carve(plan, base, ws.GQKV2, N * 3 * D);
-    carve(plan, base, ws.GVNMSG2, N * 3 * D);
-    carve(plan, base, ws.GTU2, N * 6 * D);
     carve(plan, base, ws.eatom, N);
     carve(plan, base, h->d_pos, N * 3);
     carve(plan, base, h->d_forces, N * 3 + G);          // forces, then the fragment energies: one D2H copy brings both back
@@ -383,22 +377,6 @@ struct Launcher {
 };
 
 template <int NPW>
-void launch_node_fwd(Launcher& Lc, int k) {
-    vb_handle* h = Lc.h;
-    NodeArgs a{k, h->mw, h->ws};
-    const int blocks = (h->ws.N + NODE_WARPS * NPW - 1) / (NODE_WARPS * NPW);
-    Lc.launch(node_fwd_kernel<NPW>, dim3(blocks), dim3(NODE_WARPS * 32), 0, a);
-    Lc.check();
-}
-template <int NPW>
-void launch_node_bwd(Launcher& Lc, int k) {
-    vb_handle* h = Lc.h;
-    NodeArgs a{k, h->mw, h->ws};
-    const int blocks = (h->ws.N + NODE_WARPS * NPW - 1) / (NODE_WARPS * NPW);
-    Lc.launch(node_bwd_kernel<NPW>, dim3(blocks), dim3(NODE_WARPS * 32), node_bwd_smem_bytes<NPW>(), a);
-    Lc.check();
-}
-template <int NPW>
 void launch_head(Launcher& Lc) {
     vb_handle* h = Lc.h;
     const int blocks = (h->ws.N + NODE_WARPS * NPW - 1) / (NODE_WARPS * NPW);
@@ -428,14 +406,14 @@ template <int NB>
 void launch_node_fwd2(Launcher& Lc, int k) {
     vb_handle* h = Lc.h;
     NodeArgs a{k, h->mw, h->ws, h->timeline ? h->d_tl + (size_t)2 * L * TC_TL_SLOTS + (size_t)k * N2_TL_SLOTS : nullptr, h->krot};
-    Lc.launch(node_fwd2_kernel<NB>, dim3((h->ws.N + NB - 1) / NB), dim3(N2Cfg<NB>::THREADS), sizeof(NodeFwd2SmemK<NB>), a);
+    Lc.launch(node_fwd2_kernel<NB>, dim3((h->ws.N + NB - 1) / NB), dim3(N2Cfg<NB>::THREADS), sizeof(NodeFwd2Smem<NB>), a);
     Lc.check();
 }
 template <int NB>
 void launch_node_bwd2(Launcher& Lc, int k) {
     vb_handle* h = Lc.h;
     NodeArgs a{k, h->mw, h->ws, h->timeline ? h->d_tl + (size_t)2 * L * TC_TL_SLOTS + (size_t)(L + 1 + k) * N2_TL_SLOTS : nullptr, h->krot};
-    Lc.launch(node_bwd2_kernel<NB>, dim3((h->ws.N + NB - 1) / NB), dim3(N2Cfg<NB>::THREADS), sizeof(NodeBwd2SmemK<NB>), a);
+    Lc.launch(node_bwd2_kernel<NB>, dim3((h->ws.N + NB - 1) / NB), dim3(N2Cfg<NB>::THREADS), sizeof(NodeBwd2Smem<NB>), a);
     Lc.check();
 }
 // nodes per CTA of the CTA-cooperative SIMT node kernels: the fewest (1..4) that still fit one wave, else 8
@@ -446,31 +424,23 @@ int node_nb(const vb_handle* h) {
     return 8;
 }
 void node_fwd(Launcher& Lc, int k) {
-    if (Lc.h->node_impl == 1) {
-        if (Lc.h->npw == 2) launch_node_fwd2<16>(Lc, k);
-        else switch (node_nb(Lc.h)) {           // one wave of 16-warp CTAs with as few nodes each as that allows
-            case 1: launch_node_fwd2<1>(Lc, k); break;
-            case 2: launch_node_fwd2<2>(Lc, k); break;
-            case 3: launch_node_fwd2<3>(Lc, k); break;
-            case 4: launch_node_fwd2<4>(Lc, k); break;
-            default: launch_node_fwd2<8>(Lc, k);
-        }
-        return;
+    if (Lc.h->npw == 2) launch_node_fwd2<16>(Lc, k);
+    else switch (node_nb(Lc.h)) {           // one wave of 16-warp CTAs with as few nodes each as that allows
+        case 1: launch_node_fwd2<1>(Lc, k); break;
+        case 2: launch_node_fwd2<2>(Lc, k); break;
+        case 3: launch_node_fwd2<3>(Lc, k); break;
+        case 4: launch_node_fwd2<4>(Lc, k); break;
+        default: launch_node_fwd2<8>(Lc, k);
     }
-    Lc.h->npw == 2 ? launch_node_fwd<2>(Lc, k) : launch_node_fwd<1>(Lc, k);
 }
 void node_bwd(Launcher& Lc, int k) {
-    if (Lc.h->node_impl == 1) {
-        switch (node_nb(Lc.h)) {
-            case 1: launch_node_bwd2<1>(Lc, k); break;
-            case 2: launch_node_bwd2<2>(Lc, k); break;
-            case 3: launch_node_bwd2<3>(Lc, k); break;
-            case 4: launch_node_bwd2<4>(Lc, k); break;
-            default: launch_node_bwd2<8>(Lc, k);
-        }
-        return;
+    switch (node_nb(Lc.h)) {
+        case 1: launch_node_bwd2<1>(Lc, k); break;
+        case 2: launch_node_bwd2<2>(Lc, k); break;
+        case 3: launch_node_bwd2<3>(Lc, k); break;
+        case 4: launch_node_bwd2<4>(Lc, k); break;
+        default: launch_node_bwd2<8>(Lc, k);
     }
-    Lc.h->npw == 2 ? launch_node_bwd<2>(Lc, k) : launch_node_bwd<1>(Lc, k);
 }
 void head(Launcher& Lc) {
     vb_handle* h = Lc.h;
@@ -541,51 +511,6 @@ void edge_bwd(Launcher& Lc, int l) {
     if (Lc.h->edge_tc & 2) { launch_edge_bwd_tc(Lc, l); return; }
     if (Lc.h->te_bwd == 64) launch_edge_bwd<64, 8>(Lc, l, 1);
     else launch_edge_bwd<32, 8>(Lc, l, 2);
-}
-
-void fill_fwd_jobs(const LayerW& lw, int l, TcJob* jobs, int& n) {
-    const size_t chunk = 4 * 8192;
-    n = 0;
-    jobs[n++] = TcJob{lw.tcW1, 0};                       // dk
-    jobs[n++] = TcJob{lw.tcW1 + chunk, 0};               // dv
-    if (l < L - 1) jobs[n++] = TcJob{lw.tcW1 + 2 * chunk, 0};   // f
-    jobs[n++] = TcJob{lw.tcWs, 0};                       // s1
-    jobs[n++] = TcJob{lw.tcWs + chunk, 0};               // s2
-}
-void fill_bwd_jobs(const LayerW& lw, int l, TcJob* jobs, int& n) {
-    const size_t chunk = 4 * 8192;
-    n = 0;
-    jobs[n++] = TcJob{lw.tcWsN, 0};                        // g_m  = g_s1' Ws[0:128]
-    jobs[n++] = TcJob{lw.tcWsN + chunk, 1};                //      + g_s2' Ws[128:256]
-    jobs[n++] = TcJob{lw.tcW1N + chunk, 0};                // g_f  = g_Pdv Wdv
-    jobs[n++] = TcJob{lw.tcW1N, 1};                        //      + g_Pdk Wdk
-    if (l < L - 1) jobs[n++] = TcJob{lw.tcW1N + 2 * chunk, 1};   //      + g_Pf  Wf
-}
-int fused_grid(const vb_handle* h) {
-    const int nblocks = (h->ws.N + FU_NB - 1) / FU_NB;
-    return std::max(1, std::min(nblocks, h->sm_count));
-}
-// edge stage l + node stage l+1 (forward) / node adjoint l+1 + edge adjoint l (backward), one launch each
-void launch_fused_fwd(Launcher& Lc, int l) {
-    vb_handle* h = Lc.h;
-    FusedArgs a{};
-    a.layer = l; a.mw = h->mw; a.ws = h->ws;
-    fill_fwd_jobs(h->mw.layer[l], l, a.jobs, a.njobs);
-    Lc.launch(fused_fwd_kernel, dim3(fused_grid(h)), dim3(TC2_THREADS), TC_SMEM_BYTES, a);
-    Lc.check();
-}
-void launch_fused_bwd(Launcher& Lc, int l) {
-    vb_handle* h = Lc.h;
-    const Workspace& ws = h->ws;
-    FusedArgs a{};
-    a.layer = l; a.mw = h->mw; a.ws = ws;
-    fill_bwd_jobs(h->mw.layer[l], l, a.jobs, a.njobs);
-    float* set[2][3] = {{ws.GQKV, ws.GVNMSG, ws.GTU}, {ws.GQKV2, ws.GVNMSG2, ws.GTU2}};
-    const int pa = l & 1, pc = (l + 1) & 1;
-    a.acc_qkv = set[pa][0]; a.acc_vn = set[pa][1]; a.acc_tu = set[pa][2];
-    a.con_qkv = set[pc][0]; a.con_vn = set[pc][1]; a.con_tu = set[pc][2];
-    Lc.launch(fused_bwd_kernel, dim3(fused_grid(h)), dim3(TC2_THREADS), TC_SMEM_BYTES, a);
-    Lc.check();
 }
 
 // ---- node stage on tensor cores (k_node_tc.cuh) --------------------------------------------------------------
@@ -712,20 +637,7 @@ void enqueue_all(Launcher& Lc, const StepIO& io) {
     }
     const int eblocks = std::max(1, std::min((ws.Ecap + 3) / 4, h->sm_count * 16));     // four edges per block and pass
     if (Lc.next("embed_edge")) { Lc.launch(embed_edge_kernel, dim3(eblocks), dim3(128), 0, h->mw, ws); Lc.check(); }
-    if (h->fused) {
-        // one launch per layer and direction: "fwdL" = edge stage L + node stage L+1, "bwdL" = node adjoint L+1 + edge adjoint L
-        if (Lc.next("node_fwd0")) launch_node_fwd2<4>(Lc, 0);
-        for (int l = 0; l < L; l++) {
-            snprintf(name, sizeof(name), "fwd%d", l);
-            if (Lc.next(name)) launch_fused_fwd(Lc, l);
-        }
-        if (Lc.next("head")) head(Lc);
-        for (int l = L - 1; l >= 0; l--) {
-            snprintf(name, sizeof(name), "bwd%d", l);
-            if (Lc.next(name)) launch_fused_bwd(Lc, l);
-        }
-        if (Lc.next("node_bwd0")) launch_node_bwd2<4>(Lc, 0);
-    } else if (h->node_tc) {
+    if (h->node_tc) {
         // node stage on tensor cores: three launches per stage (GEMM tiles / warp-per-node glue / GEMM tiles)
         for (int l = 0; l < L; l++) {
             node_fwd_tc(Lc, l);
@@ -779,8 +691,6 @@ int configure_kernels(vb_handle* h) {
     CUDA_TRY(h, opt_in_smem(edge_fwd_kernel<64, 8>, edge_fwd_smem_bytes<64>()));
     CUDA_TRY(h, opt_in_smem(edge_bwd_kernel<32, 8>, edge_bwd_smem_bytes<32>()));
     CUDA_TRY(h, opt_in_smem(edge_bwd_kernel<64, 8>, edge_bwd_smem_bytes<64>()));
-    CUDA_TRY(h, opt_in_smem(node_bwd_kernel<1>, node_bwd_smem_bytes<1>()));
-    CUDA_TRY(h, opt_in_smem(node_bwd_kernel<2>, node_bwd_smem_bytes<2>()));
     CUDA_TRY(h, opt_in_smem(head_kernel<1>, HeadSmem<1>::BYTES));
     CUDA_TRY(h, opt_in_smem(head_kernel<2>, HeadSmem<2>::BYTES));
     CUDA_TRY(h, opt_in_smem(edge_fwd_tc_kernel<32>, TC_SMEM_BYTES));
@@ -791,24 +701,22 @@ int configure_kernels(vb_handle* h) {
     CUDA_TRY(h, opt_in_smem(edge_bwd_tc_kernel<64>, TC_SMEM_BYTES));
     CUDA_TRY(h, opt_in_smem(edge_bwd_tc_kernel<96>, TC_SMEM_BYTES));
     CUDA_TRY(h, opt_in_smem(edge_bwd_tc_kernel<128>, TC_SMEM_BYTES));
-    CUDA_TRY(h, opt_in_smem(fused_fwd_kernel, TC_SMEM_BYTES));
-    CUDA_TRY(h, opt_in_smem(fused_bwd_kernel, TC_SMEM_BYTES));
     CUDA_TRY(h, opt_in_smem(node_tc_kernel<NT_OPROJ>, TC_SMEM_BYTES));
     CUDA_TRY(h, opt_in_smem(node_tc_kernel<NT_PROJ>, TC_SMEM_BYTES));
     CUDA_TRY(h, opt_in_smem(node_tc_kernel<NT_BWDA>, TC_SMEM_BYTES));
     CUDA_TRY(h, opt_in_smem(node_tc_kernel<NT_BWDB>, TC_SMEM_BYTES));
 
-    CUDA_TRY(h, opt_in_smem(node_fwd2_kernel<1>, sizeof(NodeFwd2SmemK<1>)));
-    CUDA_TRY(h, opt_in_smem(node_bwd2_kernel<1>, sizeof(NodeBwd2SmemK<1>)));
-    CUDA_TRY(h, opt_in_smem(node_fwd2_kernel<2>, sizeof(NodeFwd2SmemK<2>)));
-    CUDA_TRY(h, opt_in_smem(node_bwd2_kernel<2>, sizeof(NodeBwd2SmemK<2>)));
-    CUDA_TRY(h, opt_in_smem(node_fwd2_kernel<3>, sizeof(NodeFwd2SmemK<3>)));
-    CUDA_TRY(h, opt_in_smem(node_bwd2_kernel<3>, sizeof(NodeBwd2SmemK<3>)));
-    CUDA_TRY(h, opt_in_smem(node_fwd2_kernel<4>, sizeof(NodeFwd2SmemK<4>)));
-    CUDA_TRY(h, opt_in_smem(node_bwd2_kernel<4>, sizeof(NodeBwd2SmemK<4>)));
-    CUDA_TRY(h, opt_in_smem(node_fwd2_kernel<8>, sizeof(NodeFwd2SmemK<8>)));
-    CUDA_TRY(h, opt_in_smem(node_fwd2_kernel<16>, sizeof(NodeFwd2SmemK<16>)));
-    CUDA_TRY(h, opt_in_smem(node_bwd2_kernel<8>, sizeof(NodeBwd2SmemK<8>)));
+    CUDA_TRY(h, opt_in_smem(node_fwd2_kernel<1>, sizeof(NodeFwd2Smem<1>)));
+    CUDA_TRY(h, opt_in_smem(node_bwd2_kernel<1>, sizeof(NodeBwd2Smem<1>)));
+    CUDA_TRY(h, opt_in_smem(node_fwd2_kernel<2>, sizeof(NodeFwd2Smem<2>)));
+    CUDA_TRY(h, opt_in_smem(node_bwd2_kernel<2>, sizeof(NodeBwd2Smem<2>)));
+    CUDA_TRY(h, opt_in_smem(node_fwd2_kernel<3>, sizeof(NodeFwd2Smem<3>)));
+    CUDA_TRY(h, opt_in_smem(node_bwd2_kernel<3>, sizeof(NodeBwd2Smem<3>)));
+    CUDA_TRY(h, opt_in_smem(node_fwd2_kernel<4>, sizeof(NodeFwd2Smem<4>)));
+    CUDA_TRY(h, opt_in_smem(node_bwd2_kernel<4>, sizeof(NodeBwd2Smem<4>)));
+    CUDA_TRY(h, opt_in_smem(node_fwd2_kernel<8>, sizeof(NodeFwd2Smem<8>)));
+    CUDA_TRY(h, opt_in_smem(node_fwd2_kernel<16>, sizeof(NodeFwd2Smem<16>)));
+    CUDA_TRY(h, opt_in_smem(node_bwd2_kernel<8>, sizeof(NodeBwd2Smem<8>)));
     return VB_OK;
 }
 
@@ -821,9 +729,6 @@ int clean_accumulators(vb_handle* h, cudaStream_t st) {
     CUDA_TRY(h, cudaMemsetAsync(ws.GQKV, 0, N * 3 * D * 4, st));
     CUDA_TRY(h, cudaMemsetAsync(ws.GVNMSG, 0, N * 3 * D * 4, st));
     CUDA_TRY(h, cudaMemsetAsync(ws.GTU, 0, N * 6 * D * 4, st));
-    CUDA_TRY(h, cudaMemsetAsync(ws.GQKV2, 0, N * 3 * D * 4, st));
-    CUDA_TRY(h, cudaMemsetAsync(ws.GVNMSG2, 0, N * 3 * D * 4, st));
-    CUDA_TRY(h, cudaMemsetAsync(ws.GTU2, 0, N * 6 * D * 4, st));
     CUDA_TRY(h, cudaMemsetAsync(ws.GX, 0, N * D * 4, st));
     CUDA_TRY(h, cudaMemsetAsync(ws.GXA, 0, 3 * N * D * 4, st));
     h->accum_dirty = false;
@@ -936,14 +841,10 @@ void plan_tiles(vb_handle* h, long long edges) {
 void choose_defaults(vb_handle* h) {
     const int N = h->ws.N;
     h->npw = h->npw_opt; h->te_fwd = h->te_fwd_opt; h->edge_tc = h->edge_tc_opt;
-    // fused per-layer launches (k_fused.cuh) are opt-in: inside a graph a launch boundary costs little, and the fused kernels
-    // run the node stage under the 128-register budget of the tensor-core CTA (fused_bwd spills)
-    h->fused = h->fused_opt >= 0 ? h->fused_opt : 0;
     // node stage on tensor cores from ~600 atoms on: the three-launch stage has a higher fixed latency than the single SIMT
     // kernel, which wins on small systems (H100, 700 W, graph replay, SIMT vs tensor-core node stage: Chignolin, 391 atoms,
     // 0.96 vs 1.12 ms; Trp-cage, 737 atoms, 1.48 vs 1.43 ms)
     h->node_tc = h->node_tc_opt >= 0 ? h->node_tc_opt : (N >= 600 ? 1 : 0);
-    if (h->fused) h->node_tc = 0;
     set_gxa_parts(h);
     if (h->npw == 0) h->npw = (N > 4096) ? 2 : 1;
     if (h->te_fwd == 0) h->te_fwd = ((long long)N * 17 / 64 >= 2LL * h->sm_count) ? 64 : 32;
@@ -1019,8 +920,6 @@ int vb_create(const float* weights_host, size_t n_floats, const vb_hparams* hp, 
     if (const char* s = getenv("VB_EDGE_TC")) h->edge_tc_opt = atoi(s);
     if (const char* s = getenv("VB_USE_PDL")) h->use_pdl = atoi(s) ? 1 : 0;
     if (const char* s = getenv("VB_TC_ROWS")) { const int v = atoi(s); if (v == 32 || v == 64 || v == 96 || v == 128) h->tc_rows_opt = v; }
-    if (const char* s = getenv("VB_NODE_IMPL")) h->node_impl = atoi(s);
-    if (const char* s = getenv("VB_FUSED")) h->fused_opt = atoi(s) ? 1 : 0;
     if (const char* s = getenv("VB_NODE_TC")) h->node_tc_opt = atoi(s) ? 1 : 0;
     *out = h;
     return VB_OK;
@@ -1683,11 +1582,9 @@ int vb_set_option(vb_handle* h, const char* key, int64_t value) {
         }
         if (e > 0) plan_tiles(h, e);
     }
-    else if (k == "node_impl" && (value == 0 || value == 1)) h->node_impl = (int)value;
     else if (k == "node_nb" && (value == 0 || value == 1 || value == 2 || value == 3 || value == 4 || value == 8)) h->node_nb = (int)value;
     else if (k == "krot" && (value == 0 || value == 1)) h->krot = (int)value;
-    else if (k == "fused" && (value == 0 || value == 1)) { h->fused = h->fused_opt = (int)value; if (value) h->node_tc = 0; set_gxa_parts(h); }
-    else if (k == "node_tc" && (value == 0 || value == 1)) { h->node_tc = h->node_tc_opt = (int)value; if (value) h->fused = 0; set_gxa_parts(h); }
+    else if (k == "node_tc" && (value == 0 || value == 1)) { h->node_tc = h->node_tc_opt = (int)value; set_gxa_parts(h); }
     else if (k == "comm_auto" && (value == 0 || value == 1)) h->comm_auto = (int)value;
     else if (k == "embed_batch" && value >= -1 && value <= 3) h->embed_batch_opt = (int)value;
     else if (k == "timeline" && (value == 0 || value == 1)) {
@@ -1714,10 +1611,8 @@ int64_t vb_get_option(const vb_handle* h, const char* key) {
     if (k == "te_fwd") return h->te_fwd;
     if (k == "te_bwd") return h->te_bwd;
     if (k == "edge_tc") return h->edge_tc;
-    if (k == "node_impl") return h->node_impl;
     if (k == "node_nb") return h->has_topology ? node_nb(h) : h->node_nb;
     if (k == "krot") return h->krot;
-    if (k == "fused") return h->fused;
     if (k == "node_tc") return h->node_tc;
     if (k == "comm_auto") return h->comm_auto;
     if (k == "caph_ready") return h->caph_ready ? 1 : 0;
@@ -1864,9 +1759,6 @@ int64_t vb_debug_read(vb_handle* h, const char* name, int layer, void* host_dst,
     else BUF("GQKV", ws.GQKV, N * 3 * D, 4)
     else BUF("GVNMSG", ws.GVNMSG, N * 3 * D, 4)
     else BUF("GTU", ws.GTU, N * 6 * D, 4)
-    else BUF("GQKV2", ws.GQKV2, N * 3 * D, 4)
-    else BUF("GVNMSG2", ws.GVNMSG2, N * 3 * D, 4)
-    else BUF("GTU2", ws.GTU2, N * 6 * D, 4)
     else BUF("geom", ws.geom, E * 8, 4)
     else BUF("rbf", ws.rbf, E * NR, 4)
     else BUF("eacc", ws.eacc, E * 4, 4)

@@ -16,7 +16,6 @@ constexpr int TC_SLABS = D / tc::SLAB_K;   // K-slabs (ring stages) per product
 static_assert((TC_SLABS & (TC_SLABS - 1)) == 0, "tc_slab rotates the slab order with a mask: TC_SLABS must be a power of two");
 constexpr int TC_MAXJOBS = 12;
 constexpr int TC_LT = D + LDS_PAD;   // padded row length of the staging tile and of the A operand (132 floats)
-constexpr int TC_TILE_EXT = 1792;    // floats appended to the staging tile for the fused kernels' node stage (7 KB)
 
 struct TcJob {
     const float* img;   // weight image of this 128x128 chunk (4 slabs x 32 KB)
@@ -26,7 +25,6 @@ struct TcJob {
 struct TcShared {
     alignas(1024) uint8_t ring[TC_STAGES][tc::STAGE_BYTES];
     alignas(16) float tile[TC_TE][TC_LT];
-    float tile_ext[TC_TILE_EXT];        // fused kernels (k_fused.cuh): the node stage's shared rows start at `tile` and may run on into here
     alignas(16) float abuf[TC_TE][TC_LT];   // A operand of the products in flight (fp32; split into tf32 hi / lo as it is loaded)
     EdgeMeta<TC_TE> meta;
     alignas(8) uint64_t b_full[TC_MAX_STAGES];

@@ -1,9 +1,7 @@
-// Per-node stages of a ViS_MP layer (forward and adjoint).
-//   reference: visnet_block.py:237-250 (LayerNorm, VecLayerNorm, q/k/v, vec_proj, vec_dot),
-//              :271-273 (o_proj, dx, dvec), :129-131,136-137 (residual updates),
-//              utils.py:200-228 (VecLayerNorm max_min), :290-292 (w_trg/w_src applied per node here:
-//              the reference applies them per edge after the gather; same per-row arithmetic).
-// One warp owns NPW nodes end to end; lane owns channels lane*4..lane*4+3.
+// Helpers shared by the node stages (k_node2.cuh, k_node_tc.cuh) and the head (k_head.cuh): the launch arguments of a
+// node stage and the per-node LayerNorm / VecLayerNorm (max_min) forward and adjoint, one warp per node with lane owning
+// channels lane*4..lane*4+3.
+//   reference: visnet_block.py:238-239 (LayerNorm, VecLayerNorm), utils.py:200-228 (VecLayerNorm max_min).
 #pragma once
 #include "model.h"
 
@@ -149,313 +147,6 @@ __device__ __forceinline__ void vecln_backward(const float4 (&v)[3], const float
     }
 #pragma unroll
     for (int s = 0; s < 3; s++) gv[s] = f4(outv[s][0], outv[s][1], outv[s][2], outv[s][3]);
-}
-
-// ---------------------------------------------------------------------------------------------
-// Forward node stage k (k = 0..L):
-//   if k >= 1: finish layer k-1:  o = xa Wo^T + bo ; x += vdot*o2 + o3 ; vec += v3*o1 + va
-//   if k <  L: start layer k:     xn = LN(x) ; vn = VecLN(vec) ; q,k,v ; [v1|v2|v3] = vn Wvec^T ; vdot ;
-//                                 [t|u] = vn [Wtrg|Wsrc]^T (k < L-1)
-//   zeroes XA / VA for the edge stage that follows.
-// ---------------------------------------------------------------------------------------------
-template <int NPW>
-__global__ void __launch_bounds__(NODE_WARPS * 32) node_fwd_kernel(NodeArgs a) {
-    pdl_entry();
-    constexpr int LDA = D + LDS_PAD;
-    __shared__ __align__(16) float smem[NODE_WARPS][4 * NPW][LDA];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int k = a.layer;
-    const Workspace& ws = a.ws;
-    float(*xs)[LDA] = smem[warp];             // rows [0, NPW): scalar rows; rows [NPW, 4*NPW): vector rows
-    float(*vs)[LDA] = smem[warp] + NPW;
-    const int n0 = (blockIdx.x * NODE_WARPS + warp) * NPW;
-    if (n0 >= ws.N) return;
-    const int col = lane * 4;
-
-    float4 x[NPW], vec[NPW][3];
-    if (k >= 1) {
-        const LayerW& lw = a.mw.layer[k - 1];
-#pragma unroll
-        for (int nd = 0; nd < NPW; nd++) {
-            const int node = n0 + nd;
-            st4(&xs[nd][col], node < ws.N ? ld4(ws.XA + (size_t)node * D + col) : f4s(0.f));
-        }
-        __syncwarp();
-        float o1[NPW][4], o2[NPW][4], o3[NPW][4];
-        acc_set_bias<NPW>(o1, lw.bo, lane);
-        acc_set_bias<NPW>(o2, lw.bo + D, lane);
-        acc_set_bias<NPW>(o3, lw.bo + 2 * D, lane);
-        warp_gemm<NPW, D, LDA>(o1, &xs[0][0], lw.WoT, 3 * D, lane);
-        warp_gemm<NPW, D, LDA>(o2, &xs[0][0], lw.WoT + D, 3 * D, lane);
-        warp_gemm<NPW, D, LDA>(o3, &xs[0][0], lw.WoT + 2 * D, 3 * D, lane);
-        __syncwarp();
-#pragma unroll
-        for (int nd = 0; nd < NPW; nd++) {
-            const int node = n0 + nd;
-            if (node >= ws.N) { x[nd] = f4s(0.f); vec[nd][0] = vec[nd][1] = vec[nd][2] = f4s(0.f); continue; }
-            const float4 vo1 = arr4(o1[nd]), vo2 = arr4(o2[nd]), vo3 = arr4(o3[nd]);
-            float* orow = ws.O[k - 1] + (size_t)node * 3 * D;
-            st4(orow + col, vo1); st4(orow + D + col, vo2); st4(orow + 2 * D + col, vo3);
-            const float4 vd = ld4(ws.VDOT[k - 1] + (size_t)node * D + col);
-            x[nd] = ld4(ws.X[k - 1] + (size_t)node * D + col) + vd * vo2 + vo3;
-            st4(ws.X[k] + (size_t)node * D + col, x[nd]);
-#pragma unroll
-            for (int s = 0; s < 3; s++) {
-                const size_t r3 = (size_t)node * 3 + s;
-                const float4 v3 = ld4(ws.V123[k - 1] + r3 * 3 * D + 2 * D + col);
-                vec[nd][s] = ld4(ws.V[k - 1] + r3 * D + col) + v3 * vo1 + ld4(ws.VA + r3 * D + col);
-                st4(ws.V[k] + r3 * D + col, vec[nd][s]);
-            }
-        }
-    } else {
-#pragma unroll
-        for (int nd = 0; nd < NPW; nd++) {
-            const int node = n0 + nd;
-            x[nd] = node < ws.N ? ld4(ws.X[0] + (size_t)node * D + col) : f4s(0.f);
-            vec[nd][0] = vec[nd][1] = vec[nd][2] = f4s(0.f);   // vec starts at zero (visnet_block.py:119-121)
-        }
-    }
-    // clear the aggregation targets of the next edge stage
-#pragma unroll
-    for (int nd = 0; nd < NPW; nd++) {
-        const int node = n0 + nd;
-        if (node < ws.N) {
-            st4(ws.XA + (size_t)node * D + col, f4s(0.f));
-#pragma unroll
-            for (int s = 0; s < 3; s++) st4(ws.VA + ((size_t)node * 3 + s) * D + col, f4s(0.f));
-        }
-    }
-    if (k >= L) return;
-
-    const LayerW& lw = a.mw.layer[k];
-#pragma unroll
-    for (int nd = 0; nd < NPW; nd++) {
-        const int node = n0 + nd;
-        const float4 xn = ln_forward(x[nd], lw.ln_w, lw.ln_b, lane);
-        st4(&xs[nd][col], xn);
-        float4 vn[3];
-        vecln_forward(vec[nd], vn, lw.vln_w, lane);
-#pragma unroll
-        for (int s = 0; s < 3; s++) {
-            st4(&vs[nd * 3 + s][col], vn[s]);
-            if (node < ws.N) st4(ws.VN[k] + ((size_t)node * 3 + s) * D + col, vn[s]);
-        }
-    }
-    __syncwarp();
-    // q, k, v
-#pragma unroll 1
-    for (int ch = 0; ch < 3; ch++) {
-        float acc[NPW][4];
-        acc_set_bias<NPW>(acc, lw.bqkv + ch * D, lane);
-        warp_gemm<NPW, D, LDA>(acc, &xs[0][0], lw.WqkvT + ch * D, 3 * D, lane);
-#pragma unroll
-        for (int nd = 0; nd < NPW; nd++)
-            if (n0 + nd < ws.N) st4(ws.QKV[k] + (size_t)(n0 + nd) * 3 * D + ch * D + col, arr4(acc[nd]));
-    }
-    // vec_proj -> v1, v2, v3 ; vec_dot
-    {
-        float p1[3 * NPW][4], p2[3 * NPW][4];
-        acc_zero<3 * NPW>(p1);
-        acc_zero<3 * NPW>(p2);
-        warp_gemm<3 * NPW, D, LDA>(p1, &vs[0][0], lw.WvecT, 3 * D, lane);
-        warp_gemm<3 * NPW, D, LDA>(p2, &vs[0][0], lw.WvecT + D, 3 * D, lane);
-#pragma unroll
-        for (int nd = 0; nd < NPW; nd++) {
-            const int node = n0 + nd;
-            if (node >= ws.N) continue;
-            float4 vd = f4s(0.f);
-#pragma unroll
-            for (int s = 0; s < 3; s++) {
-                const float4 a1 = arr4(p1[nd * 3 + s]), a2 = arr4(p2[nd * 3 + s]);
-                vd = vd + a1 * a2;
-                float* row = ws.V123[k] + ((size_t)node * 3 + s) * 3 * D;
-                st4(row + col, a1);
-                st4(row + D + col, a2);
-            }
-            st4(ws.VDOT[k] + (size_t)node * D + col, vd);
-        }
-        acc_zero<3 * NPW>(p1);
-        warp_gemm<3 * NPW, D, LDA>(p1, &vs[0][0], lw.WvecT + 2 * D, 3 * D, lane);
-#pragma unroll
-        for (int r = 0; r < 3 * NPW; r++) {
-            const int node = n0 + r / 3;
-            if (node < ws.N) st4(ws.V123[k] + ((size_t)node * 3 + r % 3) * 3 * D + 2 * D + col, arr4(p1[r]));
-        }
-    }
-    if (k < L - 1) {
-#pragma unroll 1
-        for (int ch = 0; ch < 2; ch++) {
-            float acc[3 * NPW][4];
-            acc_zero<3 * NPW>(acc);
-            warp_gemm<3 * NPW, D, LDA>(acc, &vs[0][0], lw.WtuT + ch * D, 2 * D, lane);
-#pragma unroll
-            for (int r = 0; r < 3 * NPW; r++) {
-                const int node = n0 + r / 3;
-                if (node < ws.N) st4(ws.TU[k] + ((size_t)node * 3 + r % 3) * 2 * D + ch * D + col, arr4(acc[r]));
-            }
-        }
-    }
-}
-
-// ---------------------------------------------------------------------------------------------
-// Backward node stage k (k = L..0):
-//   if k <= L-1: adjoint of the first half of layer k (needs the edge adjoint of layer k):
-//        g_xn = [gq|gk|gv] Wqkv ; g_vn = g_vn_msg + [g_vdot*v2 | g_vdot*v1 | gvec*o1] Wvec + [gt|gu] Wtu
-//        gvec += VecLN'(vec_in, g_vn) ; gx += LN'(x_in, g_xn)
-//   if k >= 1:   adjoint of the second half of layer k-1:
-//        g_xa = [sum_s gvec*v3 | gx*vdot | gx] Wo          (feeds the edge adjoint of layer k-1)
-//   also zeroes GQKV / GVNMSG / GTU (atomic targets of the next edge adjoint).
-// ---------------------------------------------------------------------------------------------
-template <int NPW>
-__global__ void __launch_bounds__(NODE_WARPS * 32) node_bwd_kernel(NodeArgs a) {
-    pdl_entry();
-    constexpr int LD3 = 3 * D + LDS_PAD;   // 388
-    constexpr int LD2 = 2 * D + LDS_PAD;   // 260
-    extern __shared__ __align__(16) float dyn_smem[];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int k = a.layer;
-    const Workspace& ws = a.ws;
-    float* base = dyn_smem + (size_t)warp * (NPW * LD3 + 3 * NPW * LD3 + 3 * NPW * LD2);
-    float* gq_s = base;                          // [NPW][LD3]
-    float* gvp_s = base + NPW * LD3;             // [3NPW][LD3]
-    float* gtu_s = gvp_s + 3 * NPW * LD3;        // [3NPW][LD2]
-    const int n0 = (blockIdx.x * NODE_WARPS + warp) * NPW;
-    if (n0 >= ws.N) return;
-    const int col = lane * 4;
-
-    float4 gx[NPW], gvec[NPW][3];
-#pragma unroll
-    for (int nd = 0; nd < NPW; nd++) {
-        const int node = n0 + nd;
-        if (node < ws.N) {
-            gx[nd] = ld4(ws.GX + (size_t)node * D + col);
-#pragma unroll
-            for (int s = 0; s < 3; s++) gvec[nd][s] = ld4(ws.GVEC + ((size_t)node * 3 + s) * D + col);
-        } else {
-            gx[nd] = f4s(0.f);
-            gvec[nd][0] = gvec[nd][1] = gvec[nd][2] = f4s(0.f);
-        }
-    }
-
-    if (k <= L - 1) {
-        const LayerW& lw = a.mw.layer[k];
-        const bool has_tu = (k < L - 1);
-#pragma unroll
-        for (int nd = 0; nd < NPW; nd++) {
-            const int node = n0 + nd;
-            const bool ok = node < ws.N;
-            const float4 z4 = f4s(0.f);
-            const float* orow = ws.O[k] + (size_t)node * 3 * D;
-            const float4 o1 = ok ? ld4(orow + col) : z4;
-            const float4 o2 = ok ? ld4(orow + D + col) : z4;
-            const float4 g_vdot = gx[nd] * o2;
-            const float* gq = ws.GQKV + (size_t)node * 3 * D;
-            st4(gq_s + nd * LD3 + col, ok ? ld4(gq + col) : z4);
-            st4(gq_s + nd * LD3 + D + col, ok ? ld4(gq + D + col) : z4);
-            st4(gq_s + nd * LD3 + 2 * D + col, ok ? ld4(gq + 2 * D + col) : z4);
-#pragma unroll
-            for (int s = 0; s < 3; s++) {
-                const size_t r3 = (size_t)node * 3 + s;
-                const float* vrow = ws.V123[k] + r3 * 3 * D;
-                const float4 v1 = ok ? ld4(vrow + col) : z4;
-                const float4 v2 = ok ? ld4(vrow + D + col) : z4;
-                float* dst = gvp_s + (nd * 3 + s) * LD3;
-                st4(dst + col, g_vdot * v2);
-                st4(dst + D + col, g_vdot * v1);
-                st4(dst + 2 * D + col, gvec[nd][s] * o1);
-                if (has_tu) {
-                    const float* gt = ws.GTU + r3 * 2 * D;
-                    st4(gtu_s + (nd * 3 + s) * LD2 + col, ok ? ld4(gt + col) : z4);
-                    st4(gtu_s + (nd * 3 + s) * LD2 + D + col, ok ? ld4(gt + D + col) : z4);
-                }
-            }
-        }
-        __syncwarp();
-        float gxn[NPW][4];
-        acc_zero<NPW>(gxn);
-        warp_gemm<NPW, 3 * D, LD3>(gxn, gq_s, lw.WqkvN, D, lane);
-        float gvn[3 * NPW][4];
-#pragma unroll
-        for (int r = 0; r < 3 * NPW; r++) {
-            const int node = n0 + r / 3;
-            const float4 t = node < ws.N ? ld4(ws.GVNMSG + ((size_t)node * 3 + r % 3) * D + col) : f4s(0.f);
-            gvn[r][0] = t.x; gvn[r][1] = t.y; gvn[r][2] = t.z; gvn[r][3] = t.w;
-        }
-        warp_gemm<3 * NPW, 3 * D, LD3>(gvn, gvp_s, lw.WvecN, D, lane);
-        if (has_tu) warp_gemm<3 * NPW, 2 * D, LD2>(gvn, gtu_s, lw.WtuN, D, lane);
-        __syncwarp();
-#pragma unroll
-        for (int nd = 0; nd < NPW; nd++) {
-            const int node = n0 + nd;
-            if (node >= ws.N) continue;
-            float4 vin[3], gout[3], gv[3];
-#pragma unroll
-            for (int s = 0; s < 3; s++) {
-                vin[s] = ld4(ws.V[k] + ((size_t)node * 3 + s) * D + col);
-                gout[s] = arr4(gvn[nd * 3 + s]);
-            }
-            vecln_backward(vin, gout, gv, lw.vln_w, lane);
-#pragma unroll
-            for (int s = 0; s < 3; s++) gvec[nd][s] = gvec[nd][s] + gv[s];
-            const float4 xin = ld4(ws.X[k] + (size_t)node * D + col);
-            gx[nd] = gx[nd] + ln_backward(xin, arr4(gxn[nd]), lw.ln_w, lane);
-        }
-    }
-    // clear the atomic targets of the next edge adjoint
-#pragma unroll
-    for (int nd = 0; nd < NPW; nd++) {
-        const int node = n0 + nd;
-        if (node >= ws.N) continue;
-        const float4 z4 = f4s(0.f);
-        float* gq = ws.GQKV + (size_t)node * 3 * D;
-        st4(gq + col, z4); st4(gq + D + col, z4); st4(gq + 2 * D + col, z4);
-#pragma unroll
-        for (int s = 0; s < 3; s++) {
-            const size_t r3 = (size_t)node * 3 + s;
-            st4(ws.GVNMSG + r3 * D + col, z4);
-            st4(ws.GTU + r3 * 2 * D + col, z4);
-            st4(ws.GTU + r3 * 2 * D + D + col, z4);
-        }
-    }
-    if (k >= 1) {
-        const LayerW& lw = a.mw.layer[k - 1];
-#pragma unroll
-        for (int nd = 0; nd < NPW; nd++) {
-            const int node = n0 + nd;
-            const bool ok = node < ws.N;
-            float4 go1 = f4s(0.f);
-#pragma unroll
-            for (int s = 0; s < 3; s++) {
-                const float4 v3 = ok ? ld4(ws.V123[k - 1] + ((size_t)node * 3 + s) * 3 * D + 2 * D + col) : f4s(0.f);
-                go1 = go1 + gvec[nd][s] * v3;
-            }
-            const float4 vd = ok ? ld4(ws.VDOT[k - 1] + (size_t)node * D + col) : f4s(0.f);
-            st4(gq_s + nd * LD3 + col, go1);
-            st4(gq_s + nd * LD3 + D + col, gx[nd] * vd);
-            st4(gq_s + nd * LD3 + 2 * D + col, gx[nd]);
-        }
-        __syncwarp();
-        float gxa[NPW][4];
-        acc_zero<NPW>(gxa);
-        warp_gemm<NPW, 3 * D, LD3>(gxa, gq_s, lw.WoN, D, lane);
-#pragma unroll
-        for (int nd = 0; nd < NPW; nd++)
-            if (n0 + nd < ws.N) st4(ws.GXA + (size_t)(n0 + nd) * D + col, arr4(gxa[nd]));
-    }
-#pragma unroll
-    for (int nd = 0; nd < NPW; nd++) {
-        const int node = n0 + nd;
-        if (node >= ws.N) continue;
-        st4(ws.GX + (size_t)node * D + col, gx[nd]);
-#pragma unroll
-        for (int s = 0; s < 3; s++) st4(ws.GVEC + ((size_t)node * 3 + s) * D + col, gvec[nd][s]);
-    }
-}
-
-template <int NPW>
-constexpr size_t node_bwd_smem_bytes() {
-    return (size_t)NODE_WARPS * (NPW * (3 * D + LDS_PAD) + 3 * NPW * (3 * D + LDS_PAD) + 3 * NPW * (2 * D + LDS_PAD)) *
-           sizeof(float);
 }
 
 }  // namespace vb

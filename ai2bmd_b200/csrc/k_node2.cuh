@@ -1,9 +1,12 @@
-// Per-node stages, CTA-cooperative version: a CTA of 8 warps (16 in the 4-node variant used for small systems) owns NB
-// consecutive nodes and spreads the (weight chunk x row block) GEMM units over its warps, so the critical path is
-// 1-3 units instead of the 11 chunk-GEMMs a single warp walked through in k_node.cuh; the 4-node variant also splits the
-// o_proj K dimension over warps and sums the partials in a fixed order.  Same math, same buffers, same references
-// (visnet_block.py:237-250, 271-273; utils.py:200-228).  Bound at small sizes by streaming ~720 KB of weights per CTA
-// from L2 (DESIGN.md section 5).
+// Per-node stages of a ViS_MP layer (forward and adjoint), SIMT version: a CTA of 8 warps (16 in the 4-node variant used
+// for small systems) owns NB consecutive nodes and spreads the (weight chunk x row block) GEMM units over its warps, so
+// the critical path is 1-3 units instead of the 11 chunk-GEMMs of one warp per node; the 4-node variant also splits the
+// o_proj K dimension over warps and sums the partials in a fixed order.
+//   reference: visnet_block.py:237-250 (LayerNorm, VecLayerNorm, q/k/v, vec_proj, vec_dot),
+//              :271-273 (o_proj, dx, dvec), :129-131,136-137 (residual updates),
+//              utils.py:200-228 (VecLayerNorm max_min), :290-292 (w_trg/w_src applied per node here:
+//              the reference applies them per edge after the gather; same per-row arithmetic).
+// Bound at small sizes by streaming ~720 KB of weights per CTA from L2 (DESIGN.md section 5).
 #pragma once
 #include "k_node.cuh"
 
@@ -12,14 +15,15 @@ namespace vb {
 // warps per CTA: 16 for the 4-node variant (small systems: more units in flight per node), 8 otherwise
 template <int NB> struct N2Cfg {
     static constexpr int WARPS = (NB <= 4) ? 16 : 8; static constexpr int THREADS = WARPS * 32;
-    static constexpr int KS = (NB <= 4) ? 2 : 1;       // K-split projection plan of the stand-alone kernels (see NodeFwd2Smem)
+    static constexpr int KS = (NB <= 4) ? 2 : 1;       // K-split projection plan (see NodeFwd2Smem)
 };
 template <int NB> struct N2Rows { static constexpr int RB = (NB < 8) ? NB : 8; };   // rows per GEMM unit
 
-// KS = 2 (stand-alone 4-node kernels): every projection unit covers ALL rows of the CTA (one pass over each weight
-// chunk instead of one per row block) and half of K; the second K-half leaves a partial row in shared memory.
-template <int NB, int KS = 1>
+// KS = 2 (4-node variant): every projection unit covers ALL rows of the CTA (one pass over each weight chunk instead of
+// one per row block) and half of K; the second K-half leaves a partial row in shared memory.
+template <int NB>
 struct NodeFwd2Smem {
+    static constexpr int KS = N2Cfg<NB>::KS;
     static constexpr int LDA = D + LDS_PAD;       // 132
     static constexpr int LDO = 3 * D + LDS_PAD;   // 388
     float xs[NB][LDA];                            // xa rows, later LayerNorm(x) rows
@@ -32,19 +36,25 @@ struct NodeFwd2Smem {
 };
 
 // ---------------------------------------------------------------------------------------------
-// forward node stage k (same contract as node_fwd_kernel)
+// Forward node stage k (k = 0..L), CTA b owns nodes [b*NB, b*NB + NB):
+//   if k >= 1: finish layer k-1:  o = xa Wo^T + bo ; x += vdot*o2 + o3 ; vec += v3*o1 + va
+//   if k <  L: start layer k:     xn = LN(x) ; vn = VecLN(vec) ; q,k,v ; [v1|v2|v3] = vn Wvec^T ; vdot ;
+//                                 [t|u] = vn [Wtrg|Wsrc]^T (k < L-1)
+//   zeroes XA / VA for the edge stage that follows.
 // ---------------------------------------------------------------------------------------------
-// Body shared by the stand-alone kernel below and by the fused per-layer kernel (k_fused.cuh): the N2Cfg<NB>::WARPS
-// warps with threadIdx.x < N2Cfg<NB>::THREADS run it for nodes [n0, n0 + NB); `sync` is a barrier among exactly those
-// threads (__syncthreads in the stand-alone kernel, a named barrier of the compute warps in the fused one).
-template <int NB, int NBUF = 4, int KS = 1, typename SyncF>
-__device__ __forceinline__ void node_fwd2_body(const ModelW& mw, const Workspace& ws, const int k, const int n0,
-                                               float* dyn_smem, SyncF sync, unsigned long long* tl = nullptr, const int krot = 0) {
+template <int NB>
+__global__ void __launch_bounds__(N2Cfg<NB>::THREADS) node_fwd2_kernel(NodeArgs a) {
+    pdl_entry();
+    extern __shared__ __align__(16) float dyn_smem[];
+    const ModelW& mw = a.mw;
+    const Workspace& ws = a.ws;
+    const int k = a.layer, n0 = (int)blockIdx.x * NB;
+    unsigned long long* const tl = a.tl;
+    const int krot = a.krot ? (int)blockIdx.x * 16 : 0;
 #define N2_TL(i) do { if (tl != nullptr && n0 == 0 && (threadIdx.x & 31) == 0) tl[(i) * 16 + (threadIdx.x >> 5)] = (unsigned long long)clock64(); } while (0)
     N2_TL(0);
-    constexpr int N2_WARPS = N2Cfg<NB>::WARPS, N2_THREADS = N2Cfg<NB>::THREADS;
-    static_assert(KS == 1 || (KS == 2 && NB <= 4 && N2_WARPS == 16), "the K-split projection plan is the 16-warp, <= 4-node one");
-    using S = NodeFwd2Smem<NB, KS>;
+    constexpr int N2_WARPS = N2Cfg<NB>::WARPS, N2_THREADS = N2Cfg<NB>::THREADS, KS = N2Cfg<NB>::KS;
+    using S = NodeFwd2Smem<NB>;
     constexpr int LDA = S::LDA;
     constexpr int N2_RB = N2Rows<NB>::RB;
     S& sm = *reinterpret_cast<S*>(dyn_smem);
@@ -61,7 +71,7 @@ __device__ __forceinline__ void node_fwd2_body(const ModelW& mw, const Workspace
         if constexpr (KS == 2) {
             if (warp < 12) go.prefetch(lw.WoT + (size_t)(warp / 3) * (D / 4) * 3 * D + (warp % 3) * D, 3 * D, lane, krot);
         }
-        sync();
+        __syncthreads();
         N2_TL(1);
         // o = xa Wo^T + bo : units = 3 chunks x NB/8 row blocks (x 4 K-quarters in the 16-warp variant)
         if constexpr (KS == 2) {
@@ -78,7 +88,7 @@ __device__ __forceinline__ void node_fwd2_body(const ModelW& mw, const Workspace
                 }
             }
             N2_TL(2);
-            sync();
+            __syncthreads();
             N2_TL(3);
             for (int idx = threadIdx.x; idx < NB * 96; idx += N2_THREADS) {      // fixed-order sum of the K-quarters
                 const int r = idx / 96, c4 = (idx % 96) * 4;
@@ -90,7 +100,7 @@ __device__ __forceinline__ void node_fwd2_body(const ModelW& mw, const Workspace
                 float acc[N2_RB][4];
                 if (kq == 0) acc_set_bias<N2_RB>(acc, lw.bo + ch * D, lane);
                 else acc_zero<N2_RB>(acc);
-                warp_gemm<N2_RB, D / 4, LDA, NBUF>(acc, &sm.xs[0][kq * (D / 4)], lw.WoT + (size_t)kq * (D / 4) * 3 * D + ch * D, 3 * D, lane, krot);
+                warp_gemm<N2_RB, D / 4, LDA, 4>(acc, &sm.xs[0][kq * (D / 4)], lw.WoT + (size_t)kq * (D / 4) * 3 * D + ch * D, 3 * D, lane, krot);
 #pragma unroll
                 for (int r = 0; r < N2_RB; r++) {
                     if (kq == 0) st4(&sm.os[r][ch * D + col], arr4(acc[r]));
@@ -98,7 +108,7 @@ __device__ __forceinline__ void node_fwd2_body(const ModelW& mw, const Workspace
                 }
             }
             N2_TL(2);
-            sync();
+            __syncthreads();
             N2_TL(3);
             for (int idx = threadIdx.x; idx < NB * 96; idx += N2_THREADS) {      // fixed-order sum of the K-quarters
                 const int r = idx / 96, c4 = (idx % 96) * 4;
@@ -109,12 +119,12 @@ __device__ __forceinline__ void node_fwd2_body(const ModelW& mw, const Workspace
                 const int ch = u % 3, rb = u / 3;
                 float acc[N2_RB][4];
                 acc_set_bias<N2_RB>(acc, lw.bo + ch * D, lane);
-                warp_gemm<N2_RB, D, LDA, (NB <= 8 ? NBUF : 2)>(acc, &sm.xs[rb * N2_RB][0], lw.WoT + ch * D, 3 * D, lane);
+                warp_gemm<N2_RB, D, LDA, (NB <= 8 ? 4 : 2)>(acc, &sm.xs[rb * N2_RB][0], lw.WoT + ch * D, 3 * D, lane);
 #pragma unroll
                 for (int r = 0; r < N2_RB; r++) st4(&sm.os[rb * N2_RB + r][ch * D + col], arr4(acc[r]));
             }
         }
-        sync();
+        __syncthreads();
         N2_TL(4);
     }
     // per-node phase: residual update, LayerNorm, VecLayerNorm (warp per node)
@@ -178,7 +188,7 @@ __device__ __forceinline__ void node_fwd2_body(const ModelW& mw, const Workspace
             gm.prefetch(W + (size_t)half * KH * ldw + ch2 * D, ldw, lane, krot);
         }
     }
-    sync();
+    __syncthreads();
     N2_TL(6);
     if constexpr (KS == 2) {
         const int ch = ch2;
@@ -206,7 +216,7 @@ __device__ __forceinline__ void node_fwd2_body(const ModelW& mw, const Workspace
             }
         }
         N2_TL(7);
-        sync();
+        __syncthreads();
         N2_TL(8);
         if (active && half == 0) {
             if (kind == 0) {
@@ -232,7 +242,7 @@ __device__ __forceinline__ void node_fwd2_body(const ModelW& mw, const Workspace
             if (u < UQ) {
                 const int ch = u % 3, rb = u / 3;
                 acc_set_bias<N2_RB>(acc, lw.bqkv + ch * D, lane);
-                warp_gemm<N2_RB, D, LDA, (NB <= 8 ? NBUF : 2)>(acc, &sm.xs[rb * N2_RB][0], lw.WqkvT + ch * D, 3 * D, lane);
+                warp_gemm<N2_RB, D, LDA, (NB <= 8 ? 4 : 2)>(acc, &sm.xs[rb * N2_RB][0], lw.WqkvT + ch * D, 3 * D, lane);
     #pragma unroll
                 for (int r = 0; r < N2_RB; r++) {
                     const int nd = rb * N2_RB + r;
@@ -241,7 +251,7 @@ __device__ __forceinline__ void node_fwd2_body(const ModelW& mw, const Workspace
             } else if (u < UQ + UV) {
                 const int v = u - UQ, ch = v % 3, rb = v / 3;
                 acc_zero<N2_RB>(acc);
-                warp_gemm<N2_RB, D, LDA, (NB <= 8 ? NBUF : 2)>(acc, &sm.vs[rb * N2_RB][0], lw.WvecT + ch * D, 3 * D, lane);
+                warp_gemm<N2_RB, D, LDA, (NB <= 8 ? 4 : 2)>(acc, &sm.vs[rb * N2_RB][0], lw.WvecT + ch * D, 3 * D, lane);
     #pragma unroll
                 for (int r = 0; r < N2_RB; r++) {
                     const int row = rb * N2_RB + r;                  // = nd*3 + s
@@ -250,7 +260,7 @@ __device__ __forceinline__ void node_fwd2_body(const ModelW& mw, const Workspace
             } else {
                 const int v = u - UQ - UV, ch = v % 2, rb = v / 2;
                 acc_zero<N2_RB>(acc);
-                warp_gemm<N2_RB, D, LDA, (NB <= 8 ? NBUF : 2)>(acc, &sm.vs[rb * N2_RB][0], lw.WtuT + ch * D, 2 * D, lane);
+                warp_gemm<N2_RB, D, LDA, (NB <= 8 ? 4 : 2)>(acc, &sm.vs[rb * N2_RB][0], lw.WtuT + ch * D, 2 * D, lane);
     #pragma unroll
                 for (int r = 0; r < N2_RB; r++) {
                     const int row = rb * N2_RB + r;
@@ -260,7 +270,7 @@ __device__ __forceinline__ void node_fwd2_body(const ModelW& mw, const Workspace
         }
     }
     N2_TL(9);
-    sync();     // V123 rows of this CTA are visible block-wide
+    __syncthreads();     // V123 rows of this CTA are visible block-wide
     N2_TL(10);
     for (int nd = warp; nd < nn; nd += N2_WARPS) {
         const size_t r3 = (size_t)(n0 + nd) * 3;
@@ -272,23 +282,11 @@ __device__ __forceinline__ void node_fwd2_body(const ModelW& mw, const Workspace
     N2_TL(11);
 }
 
+// KS = 2 (4-node variant): units of (all rows of the CTA) x (half a 128-deep K chunk): each weight element is read once
+// per CTA, 16 (12 in the last layer) units = one per warp; the o_proj adjoint is cut into 12 units of K = 32.
 template <int NB>
-__global__ void __launch_bounds__(N2Cfg<NB>::THREADS) node_fwd2_kernel(NodeArgs a) {
-    pdl_entry();
-    extern __shared__ __align__(16) float dyn_smem[];
-    node_fwd2_body<NB, 4, N2Cfg<NB>::KS>(a.mw, a.ws, a.layer, (int)blockIdx.x * NB, dyn_smem, [] { __syncthreads(); }, a.tl,
-                                         a.krot ? (int)blockIdx.x * 16 : 0);
-}
-
-// ---------------------------------------------------------------------------------------------
-// backward node stage k (same contract as node_bwd_kernel).  K-split units: every (row block, 128-wide K
-// chunk) is one unit writing a partial [8][128] product into its own shared slot; slots are summed in a
-// fixed order afterwards (deterministic).
-// ---------------------------------------------------------------------------------------------
-// KS = 2 (stand-alone 4-node kernels): units of (all rows of the CTA) x (half a 128-deep K chunk): each weight element is
-// read once per CTA, 16 (12 in the last layer) units = one per warp; the o_proj adjoint is cut into 12 units of K = 32.
-template <int NB, int KS = 1>
 struct NodeBwd2Smem {
+    static constexpr int KS = N2Cfg<NB>::KS;
     static constexpr int LD3 = 3 * D + LDS_PAD;   // 388
     static constexpr int LD2 = 2 * D + LDS_PAD;   // 260
     static constexpr int NVB = 3 * NB / N2Rows<NB>::RB;    // vector row blocks
@@ -301,16 +299,34 @@ struct NodeBwd2Smem {
                                                   // also the 12 K = 32 partials of the o_proj adjoint ([12][NB][D])
 };
 
-// Body (see node_fwd2_body).  GQKV / GVNMSG / GTU are the accumulators the edge adjoint of layer k added into; they are
-// consumed and re-zeroed here (the fused pipeline alternates between two sets, the stand-alone one uses ws.G*).
-template <int NB, int NBUF = 4, int KS = 1, typename SyncF>
-__device__ __forceinline__ void node_bwd2_body(const ModelW& mw, const Workspace& ws, const int k, const int n0,
-                                               float* __restrict__ GQKV, float* __restrict__ GVNMSG, float* __restrict__ GTU,
-                                               float* dyn_smem, SyncF sync, unsigned long long* tl = nullptr, const int krot = 0) {
-    constexpr int N2_WARPS = N2Cfg<NB>::WARPS;
-    static_assert(KS == 1 || (KS == 2 && NB <= 4 && N2_WARPS == 16), "the K-split plan is the 16-warp, <= 4-node one");
+// ---------------------------------------------------------------------------------------------
+// Backward node stage k (k = L..0), CTA b owns nodes [b*NB, b*NB + NB):
+//   if k <= L-1: adjoint of the first half of layer k (needs the edge adjoint of layer k):
+//        g_xn = [gq|gk|gv] Wqkv ; g_vn = g_vn_msg + [g_vdot*v2 | g_vdot*v1 | gvec*o1] Wvec + [gt|gu] Wtu
+//        gvec += VecLN'(vec_in, g_vn) ; gx += LN'(x_in, g_xn)
+//   if k >= 1:   adjoint of the second half of layer k-1:
+//        g_xa = [sum_s gvec*v3 | gx*vdot | gx] Wo          (feeds the edge adjoint of layer k-1)
+//   GQKV / GVNMSG / GTU are the accumulators the edge adjoint of layer k added into; they are consumed and re-zeroed
+//   here (atomic targets of the next edge adjoint).
+// K-split units: every (row block, 128-wide K chunk) is one unit writing a partial [8][128] product into its own shared
+// slot; slots are summed in a fixed order afterwards (deterministic).
+// ---------------------------------------------------------------------------------------------
+template <int NB>
+__global__ void __launch_bounds__(N2Cfg<NB>::THREADS) node_bwd2_kernel(NodeArgs a) {
+    pdl_entry();
+    extern __shared__ __align__(16) float dyn_smem[];
+    const ModelW& mw = a.mw;
+    const Workspace& ws = a.ws;
+    const int k = a.layer, n0 = (int)blockIdx.x * NB;
+    unsigned long long* const tl = a.tl;
+    const int krot = a.krot ? (int)blockIdx.x * 16 : 0;
+    // the accumulators alias nothing else this kernel accesses: __restrict__ lets their loads move ahead of other stores
+    float* __restrict__ const GQKV = ws.GQKV;
+    float* __restrict__ const GVNMSG = ws.GVNMSG;
+    float* __restrict__ const GTU = ws.GTU;
+    constexpr int N2_WARPS = N2Cfg<NB>::WARPS, KS = N2Cfg<NB>::KS;
     N2_TL(0);
-    using S = NodeBwd2Smem<NB, KS>;
+    using S = NodeBwd2Smem<NB>;
     constexpr int LD3 = S::LD3, LD2 = S::LD2;
     constexpr int N2_RB = N2Rows<NB>::RB;
     S& sm = *reinterpret_cast<S*>(dyn_smem);
@@ -363,7 +379,7 @@ __device__ __forceinline__ void node_bwd2_body(const ModelW& mw, const Workspace
             }
         }
         N2_TL(1);
-        sync();
+        __syncthreads();
         N2_TL(2);
         if constexpr (KS == 2) {
             const int u = warp;
@@ -393,20 +409,20 @@ __device__ __forceinline__ void node_bwd2_body(const ModelW& mw, const Workspace
                 acc_zero<N2_RB>(acc);
                 if (u < UX) {
                     const int kc = u % 3, rb = u / 3;
-                    warp_gemm<N2_RB, D, LD3, NBUF>(acc, &sm.gq[rb * N2_RB][kc * D], lw.WqkvN + (size_t)kc * D * D, D, lane);
+                    warp_gemm<N2_RB, D, LD3, 4>(acc, &sm.gq[rb * N2_RB][kc * D], lw.WqkvN + (size_t)kc * D * D, D, lane);
     #pragma unroll
                     for (int r = 0; r < N2_RB; r++) st4(&sm.part_x[kc][rb * N2_RB + r][col], arr4(acc[r]));
                 } else {
                     const int v = u - UX, kc = v % kv, rb = v / kv;
-                    if (kc < 3) warp_gemm<N2_RB, D, LD3, NBUF>(acc, &sm.gvp[rb * N2_RB][kc * D], lw.WvecN + (size_t)kc * D * D, D, lane);
-                    else        warp_gemm<N2_RB, D, LD2, NBUF>(acc, &sm.gtu[rb * N2_RB][(kc - 3) * D], lw.WtuN + (size_t)(kc - 3) * D * D, D, lane);
+                    if (kc < 3) warp_gemm<N2_RB, D, LD3, 4>(acc, &sm.gvp[rb * N2_RB][kc * D], lw.WvecN + (size_t)kc * D * D, D, lane);
+                    else        warp_gemm<N2_RB, D, LD2, 4>(acc, &sm.gtu[rb * N2_RB][(kc - 3) * D], lw.WtuN + (size_t)(kc - 3) * D * D, D, lane);
     #pragma unroll
                     for (int r = 0; r < N2_RB; r++) st4(&sm.part_v[kc][rb * N2_RB + r][col], arr4(acc[r]));
                 }
             }
         }
         N2_TL(3);
-        sync();
+        __syncthreads();
         N2_TL(4);
     }
     // per-node phase
@@ -478,7 +494,7 @@ __device__ __forceinline__ void node_bwd2_body(const ModelW& mw, const Workspace
     if constexpr (KS == 2) {
         if (warp < 12) go.prefetch(lwo.WoN + ((size_t)(warp >> 2) * D + (warp & 3) * (D / 4)) * D, D, lane, krot);
     }
-    sync();
+    __syncthreads();
     N2_TL(6);
     if constexpr (KS == 2) {
         // g_xa = g_o Wo: 12 units of K = 32 (3 chunks x 4 quarters), one per warp; partial rows in the (now free) part_v area
@@ -492,7 +508,7 @@ __device__ __forceinline__ void node_bwd2_body(const ModelW& mw, const Workspace
             for (int r = 0; r < NB; r++) st4(&po[warp][r][col], arr4(acc[r]));
         }
         N2_TL(7);
-        sync();
+        __syncthreads();
         N2_TL(8);
         for (int nd = warp; nd < nn; nd += N2_WARPS) {
             float4 t[3];
@@ -507,27 +523,16 @@ __device__ __forceinline__ void node_bwd2_body(const ModelW& mw, const Workspace
             const int kc = u % 3, rb = u / 3;
             float acc[N2_RB][4];
             acc_zero<N2_RB>(acc);
-            warp_gemm<N2_RB, D, LD3, NBUF>(acc, &sm.gq[rb * N2_RB][kc * D], lwo.WoN + (size_t)kc * D * D, D, lane);
+            warp_gemm<N2_RB, D, LD3, 4>(acc, &sm.gq[rb * N2_RB][kc * D], lwo.WoN + (size_t)kc * D * D, D, lane);
 #pragma unroll
             for (int r = 0; r < N2_RB; r++) st4(&sm.part_x[kc][rb * N2_RB + r][col], arr4(acc[r]));
         }
-        sync();
+        __syncthreads();
         for (int nd = warp; nd < nn; nd += N2_WARPS)
             st4(ws.GXA + (size_t)(n0 + nd) * D + col,
                 (ld4(&sm.part_x[0][nd][col]) + ld4(&sm.part_x[1][nd][col])) + ld4(&sm.part_x[2][nd][col]));
     }
 }
-
-template <int NB>
-__global__ void __launch_bounds__(N2Cfg<NB>::THREADS) node_bwd2_kernel(NodeArgs a) {
-    pdl_entry();
-    extern __shared__ __align__(16) float dyn_smem[];
-    node_bwd2_body<NB, 4, N2Cfg<NB>::KS>(a.mw, a.ws, a.layer, (int)blockIdx.x * NB, a.ws.GQKV, a.ws.GVNMSG, a.ws.GTU, dyn_smem, [] { __syncthreads(); }, a.tl,
-                                         a.krot ? (int)blockIdx.x * 16 : 0);
-}
 #undef N2_TL
-
-template <int NB> using NodeFwd2SmemK = NodeFwd2Smem<NB, N2Cfg<NB>::KS>;     // shared-memory blocks of the stand-alone kernels
-template <int NB> using NodeBwd2SmemK = NodeBwd2Smem<NB, N2Cfg<NB>::KS>;
 
 }  // namespace vb

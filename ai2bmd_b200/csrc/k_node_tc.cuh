@@ -15,7 +15,8 @@
 //                 bwdB    dE/dxa = [g_o1 | g_x vdot | g_x] Wo as three K-chunk partials (summed by the edge adjoint) (k >= 1)
 // Vector rows are the flat [3N][128] view of the [N][3][128] tensors (row = 3 * node + s): a 128-row tile is dense.
 #pragma once
-#include "k_fused.cuh"
+#include "k_edge_tc.cuh"
+#include "k_node.cuh"
 
 namespace vb {
 
@@ -143,7 +144,7 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) node_tc_kernel(const __grid_co
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// forward glue (warp per node): residual update, LayerNorm, VecLayerNorm   (the per-node phase of node_fwd2_body)
+// forward glue (warp per node): residual update, LayerNorm, VecLayerNorm   (the per-node phase of node_fwd2_kernel)
 // ---------------------------------------------------------------------------------------------------------
 constexpr int NN_WARPS = 8;
 __global__ void __launch_bounds__(NN_WARPS * 32) node_norm_fwd_kernel(int k, ModelW mw, Workspace ws) {
@@ -188,7 +189,7 @@ __global__ void __launch_bounds__(NN_WARPS * 32) node_norm_fwd_kernel(int k, Mod
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// backward glue (warp per node): the per-node phase of node_bwd2_body around the partial products
+// backward glue (warp per node): the per-node phase of node_bwd2_kernel around the partial products
 // ---------------------------------------------------------------------------------------------------------
 // `split`: the products arrive as one partial per K chunk (3 scalar, 3 + 2 vector) to be summed here; otherwise chunk 0
 // holds the complete product (the GEMM CTA accumulated its chunks).

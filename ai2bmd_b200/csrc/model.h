@@ -107,10 +107,6 @@ struct Workspace {
     float* GQKV;            // [N][384]
     float* GVNMSG;          // [N][3][128]
     float* GTU;             // [N][3][256]
-    // second accumulator set of the fused per-layer adjoint (k_fused.cuh): layer l adds into set l&1, consumes set (l+1)&1
-    float* GQKV2;           // [N][384]
-    float* GVNMSG2;         // [N][3][128]
-    float* GTU2;            // [N][3][256]
     float* eatom;           // [N]
     // tensor-core node stage (k_node_tc.cuh)
     float* XN;              // [N][128]      LayerNorm(x) of the current stage

@@ -180,12 +180,11 @@ int vb_get_edges(vb_handle* h, int32_t* slots_host, int32_t* deg_host);
 
 /* Number of kernel launches of one vb_forward(), and whether it replays a captured CUDA graph. */
 int vb_launches_per_forward(const vb_handle* h);
-/* Tuning knobs: "use_graph" 0/1, "use_pdl" 0/1 (programmatic dependent launch between the stages, default off), "npw" 1/2, "te_fwd" 32/64, "te_bwd" 32/64, "node_impl" 0/1,
+/* Tuning knobs: "use_graph" 0/1, "use_pdl" 0/1 (programmatic dependent launch between the stages, default off), "npw" 1/2, "te_fwd" 32/64, "te_bwd" 32/64,
  * "edge_tc" bit0 = forward / bit1 = adjoint edge stage on tensor cores (default 3: both), "tc_rows" 32/64/96/128 fixed edges per tensor-core tile
  * (0 = default: tile length planned so the tiles fill whole waves of CTAs, from an estimate of 17 edges per atom or,
  * after "calibrate" 1, from the edge count of the last evaluation -- synchronises), "timeline" 0/1 in-kernel phase stamps of the tensor-core edge kernels and the SIMT node kernels (vb_debug_read "TL" / "TLN"),
- * "fused" 0/1 one launch per layer and direction (edge stage + node stage of a 4-node block; default off), "node_tc" 0/1
- * node stage on tensor cores (default: from 600 atoms), "node_nb" 0/1/2/3/4/8 nodes per CTA of the SIMT node kernels (0 = the
+ * "node_tc" 0/1 node stage on tensor cores (default: from 600 atoms), "node_nb" 0/1/2/3/4/8 nodes per CTA of the SIMT node kernels (0 = the
  * fewest that fit one wave), "krot" 0/1 every CTA of the SIMT node kernels walks the K dimension of its weight chunks from a
  * different row (default 1: the CTAs of a wave otherwise ask the same L2 slices for the same rows at the same time),
  * "embed_batch" -1/0..3 batch variants of the embedding kernels, "comm_auto" 0/1.  vb_get_option also answers "edge_overflow" (1 after a step exceeded a trimmed max_edges),
@@ -208,7 +207,7 @@ int vb_tc_selftest(int device, const float* a_host, const float* img_host, float
  * three-stage weight ring of the small-tile edge kernels. */
 int vb_tc_selftest_rows(int device, int rows, const float* a_host, const float* img_host, float* d_host, int reps, float* ms_out);
 /* Copy an internal buffer to the host.  name: "X","V","F","VN","QKV","V123","VDOT","TU","O" (per layer),
- * "XA","VA","GX","GVEC","GF","GXA","GQKV","GVNMSG","GTU","GQKV2","GVNMSG2","GTU2","geom","rbf","eacc","grbf","esrc","edst","rowptr",
+ * "XA","VA","GX","GVEC","GF","GXA","GQKV","GVNMSG","GTU","geom","rbf","eacc","grbf","esrc","edst","rowptr",
  * "eatom","energy","forces".  Returns the number of bytes copied (<= cap_bytes) or a negative status. */
 int64_t vb_debug_read(vb_handle* h, const char* name, int layer, void* host_dst, int64_t cap_bytes);
 

@@ -3,7 +3,7 @@
 
     compute-sanitizer --tool memcheck python tools/sanitize_run.py [edge_tc] [n_fragments] [key=value ...]
 
-Extra ``key=value`` pairs are engine options (``node_tc=1``, ``fused=1``); ``caph=1`` also runs the hydrogen refinement
+Extra ``key=value`` pairs are engine options (``node_tc=1``, ``node_nb=4``); ``caph=1`` also runs the hydrogen refinement
 and the whole-protein reduction of the first n_fragments through the device MD entry points."""
 import os
 import sys

@@ -91,12 +91,12 @@ def stage_report(frags="chig", weights="real", max_frags=0, opts=""):
         if k >= 1:
             report(st, f"g_xa{k-1}", rd("GXA", 0, (N, D)), B[f"g_xa{k-1}"])
 
-    def edge_bwd_checks(st, l, suffix=""):
+    def edge_bwd_checks(st, l):
         report(st, f"gf_in{l}", rd("GF", 0, (N * 32, D))[:E], B[f"gf_in{l}"])
-        report(st, "g_qkv", rd("GQKV" + suffix, 0, (N, 3 * D)), cat(B[f"g_q{l}"], B[f"g_k{l}"], B[f"g_v{l}"]))
-        report(st, "g_vn_msg", rd("GVNMSG" + suffix, 0, (N, 3, D)), B[f"g_vn_msg{l}"])
+        report(st, "g_qkv", rd("GQKV", 0, (N, 3 * D)), cat(B[f"g_q{l}"], B[f"g_k{l}"], B[f"g_v{l}"]))
+        report(st, "g_vn_msg", rd("GVNMSG", 0, (N, 3, D)), B[f"g_vn_msg{l}"])
         if l < L - 1:
-            report(st, "g_tu", rd("GTU" + suffix, 0, (N, 3, 2 * D)), cat(B[f"g_t{l}"], B[f"g_u{l}"]))
+            report(st, "g_tu", rd("GTU", 0, (N, 3, 2 * D)), cat(B[f"g_t{l}"], B[f"g_u{l}"]))
 
     for si, st in enumerate(names):
         eng.debug_run(dpos.data_ptr(), si + 1)
@@ -151,11 +151,6 @@ def stage_report(frags="chig", weights="real", max_frags=0, opts=""):
             report(st, "va", rd("VA", 0, (N, 3, D)), S[f"va{l}"])
             if l < L - 1:
                 report(st, f"f_in{l+1}", rd("F", l + 1, (N * 32, D))[:E], S[f"f_in{l+1}"])
-        elif st.startswith("fwd"):              # fused: edge stage l + node stage l+1 (xa / va are consumed inside)
-            l = int(st[3:])
-            if l < L - 1:
-                report(st, f"f_in{l+1}", rd("F", l + 1, (N * 32, D))[:E], S[f"f_in{l+1}"])
-            node_fwd_checks(st, l + 1)
         elif st == "head":
             report(st, "e_atom", rd("eatom", 0, (N,)), S["e_atom"][:, 0])
             report(st, "gx_out", rd("GX", 0, (N, D)), B["gx_out"])
@@ -166,10 +161,6 @@ def stage_report(frags="chig", weights="real", max_frags=0, opts=""):
             node_bwd_checks(st, int(st[8:]))
         elif st.startswith("edge_bwd"):
             edge_bwd_checks(st, int(st[8:]))
-        elif st.startswith("bwd"):              # fused: node adjoint l+1 + edge adjoint l (accumulator set l & 1)
-            l = int(st[3:])
-            node_bwd_checks(st, l + 1)
-            edge_bwd_checks(st, l, "2" if l & 1 else "")
         elif st == "embed_edge_bwd":
             report(st, "gx_emb", rd("GX", 0, (N, D)), B["gx_emb"])
         elif st == "embed_node_bwd":

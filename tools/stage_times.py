@@ -2,7 +2,7 @@
 """Per-launch device times of one evaluation (CUDA events inside the library, eager launches) and the graph-replay time,
 for a workload and a set of engine options.  GPU box diagnostic:
 
-    python tools/stage_times.py --workload chig --opts fused=1 [--out stages.txt]
+    python tools/stage_times.py --workload chig --opts node_tc=1 [--out stages.txt]
 """
 import argparse
 import os
@@ -52,7 +52,7 @@ def main():
     b.record(st)
     torch.cuda.synchronize()
     lines = [f"workload {args.workload}: {desc}: G={len(fd)} N={len(fd.z)}  options: {args.opts or 'defaults'} "
-             f"(fused={eng.get_option('fused')}, edge_tc={eng.get_option('edge_tc')}, tc_rows={eng.get_option('tc_rows')}, tile_rows={eng.get_option('tile_rows')})"]
+             f"(node_tc={eng.get_option('node_tc')}, edge_tc={eng.get_option('edge_tc')}, tc_rows={eng.get_option('tc_rows')}, tile_rows={eng.get_option('tile_rows')})"]
     for name, ms in prof:
         lines.append(f"{name:24s} {ms * 1e3:8.1f} us")
     lines.append(f"{'sum (eager, per-launch events)':32s} {sum(ms for _, ms in prof) * 1e3:8.1f} us  ({len(prof)} launches)")

@@ -86,7 +86,7 @@ def main():
     tb = eng.debug_read("TL", nl + args.layer, (64,), dtype=np.uint64)
     show("edge_fwd_tc", tf, FWD, mhz)
     show("edge_bwd_tc", tb, BWD, mhz)
-    if eng.get_option("node_tc") == 0 and eng.get_option("fused") == 0:
+    if eng.get_option("node_tc") == 0:
         EMB = {0: "start", 1: "previous kernel complete (pdl)", 2: "loads issued, rows staged", 3: "aggregation done", 4: "combine done", 5: "x written"}
         for title, idx, names in ((f"node_fwd2 stage {args.layer}", args.layer, NFWD), (f"node_bwd2 stage {args.layer}", nl + 1 + args.layer, NBWD),
                                   ("embed_node_small", 2 * nl + 2, EMB)):
