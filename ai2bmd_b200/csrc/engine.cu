@@ -1,6 +1,7 @@
 // Host side of the ViSNet sm_90a engine: workspace, launch sequence, CUDA-graph replay, C ABI.
 // See include/visnet_b200.h for the boundary each entry point replaces in the reference.
 #include <cuda_runtime.h>
+#include <cxxabi.h>
 
 #include <algorithm>
 #include <cstdarg>
@@ -173,6 +174,7 @@ struct vb_handle {
     int launches = 0;
     bool accum_dirty = false;    // a truncated vb_debug_run left accumulators (XA, VA, GQKV, ...) un-consumed
     std::vector<std::string> stage_names;
+    std::vector<std::string> stage_kernels;   // per stage: "symbol(...) grid=N" of the launch it makes (dry run)
     // device-resident MD state (k_md.cuh)
     bool md_ready = false;
     MdParams md{};
@@ -340,6 +342,27 @@ void layout_workspace(vb_handle* h, char* base, ArenaPlan& plan, int*& z, int*& 
 }
 
 // ---- launch sequence --------------------------------------------------------------------------------
+// "vb::edge_fwd_tc_kernel<64>(...) grid=132": the demangled symbol of a kernel, parameter list elided, and its grid
+std::string kernel_label(const void* fn, unsigned grid) {
+    const char* sym = nullptr;
+    std::string s = "?";
+    if (cudaFuncGetName(&sym, fn) == cudaSuccess && sym) s = sym;
+    else (void)cudaGetLastError();
+    int status = 0;
+    if (char* dm = abi::__cxa_demangle(s.c_str(), nullptr, nullptr, &status)) { s = dm; std::free(dm); }
+    if (s.compare(0, 5, "void ") == 0) s.erase(0, 5);           // return type of a template instance
+    if (!s.empty() && s.back() == ')') {                        // the last balanced "(...)" is the parameter list
+        int depth = 0;
+        size_t i = s.size();
+        while (i-- > 0) {
+            if (s[i] == ')') depth++;
+            else if (s[i] == '(' && --depth == 0) break;
+        }
+        if (i < s.size()) s = s.substr(0, i) + "(...)";
+    }
+    return s + " grid=" + std::to_string(grid);
+}
+
 struct Launcher {
     vb_handle* h;
     cudaStream_t st;
@@ -348,6 +371,8 @@ struct Launcher {
     bool record_names;
     cudaError_t status = cudaSuccess;
     std::vector<cudaEvent_t>* events = nullptr;   // optional: one event recorded before every stage
+    // dry run: launch() appends the label of the kernel it would launch to the current stage's entry and enqueues nothing
+    std::vector<std::string>* kernels = nullptr;
 
     bool next(const char* name) {
         if (record_names) h->stage_names.push_back(name);
@@ -364,6 +389,12 @@ struct Launcher {
     // kernel) for its completion.  Off by default: measured neutral (exit-time trigger) to slower (entry-time trigger).
     template <typename... KArgs, typename... Args>
     void launch(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, Args&&... args) {
+        if (kernels) {
+            if ((int)kernels->size() < count) kernels->resize(count);
+            std::string& s = (*kernels)[count - 1];
+            s += (s.empty() ? "" : "; ") + kernel_label((const void*)kernel, grid.x);
+            return;
+        }
         cudaLaunchConfig_t cfg = {};
         cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
         cudaLaunchAttribute attr[1];
@@ -807,11 +838,15 @@ void set_gxa_parts(vb_handle* h) {
     }
 }
 
-// stage names / launch count of one evaluation under the current options (nothing is launched)
+// stage names, the kernel each stage launches and the launch count of one evaluation under the current options: a dry
+// run of the launch sequence (nothing is enqueued; the launch helpers only compute grids and arguments)
 void record_stages(vb_handle* h) {
     h->stage_names.clear();
-    Launcher Lc{h, nullptr, 0, 0, true};
+    h->stage_kernels.clear();
+    Launcher Lc{h, nullptr, -1, 0, true};
+    Lc.kernels = &h->stage_kernels;
     enqueue_all(Lc, internal_io(h, false));
+    h->stage_kernels.resize(h->stage_names.size());
     h->launches = (int)h->stage_names.size();
 }
 
@@ -1632,6 +1667,7 @@ int64_t vb_get_option(const vb_handle* h, const char* key) {
     if (k == "tc_rows") return h->tc_rows;
     if (k == "tile_rows") return h->tile_rows;
     if (k == "n_edges_capacity") return h->ws.Ecap;
+    if (k == "gxa_parts") return h->ws.gxa_parts;
     return VB_ERR_ARG;
 }
 
@@ -1639,6 +1675,10 @@ int vb_num_stages(const vb_handle* h) { return h ? (int)h->stage_names.size() : 
 const char* vb_stage_name(const vb_handle* h, int stage) {
     if (!h || stage < 0 || stage >= (int)h->stage_names.size()) return "";
     return h->stage_names[stage].c_str();
+}
+const char* vb_stage_kernel(const vb_handle* h, int stage) {
+    if (!h || stage < 0 || stage >= (int)h->stage_kernels.size()) return "";
+    return h->stage_kernels[stage].c_str();
 }
 
 int vb_debug_run(vb_handle* h, const float* pos_dev, int n_stages) {

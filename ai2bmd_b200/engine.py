@@ -38,7 +38,7 @@ class _CaphProblem(C.Structure):
 EXPORTED_SYMBOLS = [
     "vb_weight_manifest", "vb_create", "vb_destroy", "vb_last_error", "vb_set_topology", "vb_forward",
     "vb_forward_host", "vb_set_protein_map", "vb_forward_protein", "vb_get_edges", "vb_launches_per_forward",
-    "vb_set_option", "vb_get_option", "vb_num_stages", "vb_stage_name", "vb_debug_run", "vb_debug_read", "vb_profile_stages", "vb_tc_selftest", "vb_tc_selftest_rows",
+    "vb_set_option", "vb_get_option", "vb_num_stages", "vb_stage_name", "vb_stage_kernel", "vb_debug_run", "vb_debug_read", "vb_profile_stages", "vb_tc_selftest", "vb_tc_selftest_rows",
     "vb_md_setup", "vb_md_set_normals", "vb_md_set_state", "vb_md_kick1", "vb_md_eval", "vb_md_kick2", "vb_md_run", "vb_md_get_state",
     "vb_set_nonbonded", "vb_nonbonded",
     "vb_comm_init", "vb_comm_connect", "vb_comm_allreduce",
@@ -87,6 +87,8 @@ def load_library(path: Optional[str] = None):
     lib.vb_num_stages.argtypes = [vp]
     lib.vb_stage_name.restype = C.c_char_p
     lib.vb_stage_name.argtypes = [vp, C.c_int]
+    lib.vb_stage_kernel.restype = C.c_char_p
+    lib.vb_stage_kernel.argtypes = [vp, C.c_int]
     lib.vb_debug_run.restype = C.c_int
     lib.vb_debug_run.argtypes = [vp, vp, C.c_int]
     lib.vb_profile_stages.restype = C.c_int
@@ -334,6 +336,16 @@ class Engine:
     # ---- diagnostics ----
     def stage_names(self):
         return [self.lib.vb_stage_name(self.h, i).decode() for i in range(self.lib.vb_num_stages(self.h))]
+
+    def stage_kernels(self):
+        """[(stage name, kernel, grid)] of one evaluation under the current options, e.g.
+        ("edge_fwd0", "vb::edge_fwd_tc_kernel<64>(...)", 132); from a dry run of the launch sequence (nothing enqueued)."""
+        out = []
+        for i, name in enumerate(self.stage_names()):
+            label = self.lib.vb_stage_kernel(self.h, i).decode()
+            kernel, _, grid = label.rpartition(" grid=")
+            out.append((name, kernel, int(grid)))
+        return out
 
     def debug_run(self, pos_ptr: int, n_stages: int):
         self._check(self.lib.vb_debug_run(self.h, pos_ptr, int(n_stages)), "vb_debug_run")

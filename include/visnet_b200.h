@@ -188,13 +188,18 @@ int vb_launches_per_forward(const vb_handle* h);
  * fewest that fit one wave), "krot" 0/1 every CTA of the SIMT node kernels walks the K dimension of its weight chunks from a
  * different row (default 1: the CTAs of a wave otherwise ask the same L2 slices for the same rows at the same time),
  * "embed_batch" -1/0..3 batch variants of the embedding kernels, "comm_auto" 0/1.  vb_get_option also answers "edge_overflow" (1 after a step exceeded a trimmed max_edges),
- * "tile_rows" (planned edges per tile), "comm_ready", "caph_ready" and "caph_evals" (energy evaluations of the last hydrogen refinement). */
+ * "tile_rows" (planned edges per tile), "gxa_parts" (1: every tensor-core node CTA runs all column chunks of its row tile; 3: one
+ * chunk per CTA, dE/dxa arrives as three partials), "comm_ready", "caph_ready" and "caph_evals" (energy evaluations of the last
+ * hydrogen refinement). */
 int vb_set_option(vb_handle* h, const char* key, int64_t value);
 int64_t vb_get_option(const vb_handle* h, const char* key);   /* resolved value (after vb_set_topology) */
 
 /* ---- diagnostics (stage-by-stage parity checks; not part of the hot path) ---- */
 int vb_num_stages(const vb_handle* h);
 const char* vb_stage_name(const vb_handle* h, int stage);
+/* The kernel a stage launches under the current options, as "demangled symbol(...) grid=N" (e.g.
+ * "vb::edge_fwd_tc_kernel<64>(...) grid=132"), taken from a dry run of the launch sequence that enqueues nothing. */
+const char* vb_stage_kernel(const vb_handle* h, int stage);
 /* Run only the first n_stages launches of an evaluation, synchronously (no graph). */
 int vb_debug_run(vb_handle* h, const float* pos_dev, int n_stages);
 /* Per-launch device time (ms, CUDA events on the launching stream, average of n_iter eager evaluations after

@@ -193,8 +193,12 @@ def test_graph_replay_equals_eager_and_tile_variants(real_weights, chig):
     e0, f0 = eng.forward_host(fd.pos)
     e1, f1 = eng.forward_host(fd.pos)                 # graph replay
     assert np.abs(f0 - f1).max() <= 1e-5 and np.abs(e0 - e1).max() <= 2e-3
-    for key, val in (("use_graph", 0), ("te_fwd", 64), ("te_bwd", 64), ("npw", 2)):
+    # te_fwd / te_bwd choose the tile length of the SIMT edge kernels, so they follow edge_tc = 0
+    for key, val in (("use_graph", 0), ("edge_tc", 0), ("te_fwd", 64), ("te_bwd", 64), ("npw", 2)):
+        before = eng.stage_kernels()
         eng.set_option(key, val)
+        if key != "use_graph":                        # eager launches instead of a graph replay: the same kernels
+            assert eng.stage_kernels() != before, f"{key}={val} changed no kernel"
         e2, f2 = eng.forward_host(fd.pos)
         assert np.abs(f0 - f2).max() <= 2e-5 and (np.abs(e0 - e2) <= e_tol(e0)).all(), key
     assert 15 <= eng.launches_per_forward <= 40

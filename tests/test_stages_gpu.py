@@ -2,7 +2,9 @@
 (``vb_debug_run``) and every buffer a stage produces is compared with the fp64 hand-adjoint oracle
 (``oracle/adjoint_ref.py``, equal to autograd at 1e-14).  Covered: the default plan (SIMT node stage, both edge stages
 on tensor cores), every other combination of SIMT and tensor-core edge stages ("edge_tc" 0, 1, 2), the tensor-core node
-stage and every CTA size of the SIMT node kernels.
+stage and the SIMT node kernels of NB = 1, 2, 3, 4 and 8 nodes per CTA, all on the first four Chignolin fragments (one
+edge tile per CTA).  NB = 16 ("npw" 2), several tiles per CTA and the production-size variants are in
+test_kernel_variants_gpu.py.
 Tolerance: 2e-3 relative to the largest reference entry of the buffer (fp32 + 3xTF32 against fp64; measured
 1e-6 .. 3e-4, adjoint buffers deep in the reverse sweep being the largest)."""
 import os
