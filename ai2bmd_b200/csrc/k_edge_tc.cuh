@@ -16,6 +16,7 @@ constexpr int TC_SLABS = D / tc::SLAB_K;   // K-slabs (ring stages) per product
 static_assert((TC_SLABS & (TC_SLABS - 1)) == 0, "tc_slab rotates the slab order with a mask: TC_SLABS must be a power of two");
 constexpr int TC_MAXJOBS = 12;
 constexpr int TC_LT = D + LDS_PAD;   // padded row length of the staging tile and of the A operand (132 floats)
+typedef float TcRow[TC_LT];           // one padded row: a [rows][TC_LT] shared buffer is addressed through TcRow*
 
 struct TcJob {
     const float* img;   // weight image of this 128x128 chunk (4 slabs x 32 KB)
@@ -75,11 +76,14 @@ __device__ __forceinline__ void tc_issue(TcShared& sh, int k) {
 // Tensor-core edge stage, hybrid layout.
 //   * 16 compute warps keep the coalesced "lane owns 4 channels" layout of k_edge.cuh for every global
 //     gather / scatter / elementwise step (one 512 B request per node row per warp);
-//   * the five 128x128x128 contractions per tile run on wgmma: the A operand is copied from the padded shared
-//     staging tile into a second padded buffer, every warpgroup multiplies one part of the product (A fragments
-//     split into 3xTF32 hi / lo in registers, B = the weight ring) and the accumulator comes back into the staging
-//     tile: each warpgroup computes a 64 x 64 quarter (rows x columns halves), and a warpgroup whose 64 product rows are
-//     all past the tile's edges skips its MMAs;
+//   * the five 128x128x128 contractions per tile run on wgmma: every warpgroup multiplies one part of the product (A
+//     fragments split into 3xTF32 hi / lo in registers from a padded shared buffer, B = the weight ring): each
+//     warpgroup computes a 64 x 64 quarter (rows x columns halves), and a warpgroup whose 64 product rows are all past
+//     the tile's edges skips its MMAs;
+//   * buffers: a tile of 96 / 128 rows has two, the staging tile and the A operand (`tc2_tile_to_a` copies an operand
+//     that a phase wrote into the tile); a tile of <= 64 rows has three, `tile`, `abuf` and `tc_aux` (rows 64.. of
+//     `tile`), so every operand is read where it was written, a phase that produces two row sets writes both at once,
+//     and nothing is copied or gathered twice;
 //   * there is no producer warp: the ring is refilled by whichever compute warp releases a stage last (tc2_release),
 //     so the CTA is 512 threads with 128 registers each;
 //   * a tile holds ROWS = 32 / 64 / 96 / 128 edges (template parameter): compute warp w owns rows
@@ -150,17 +154,23 @@ __device__ __forceinline__ void tc2_tile_to_a(TcShared& sh, int rows) {
     }
 }
 
-// acc (+)= A * W^T for the next job of the ring (all warps).  Warpgroup q = warp / 4 computes rows 64 * (q & 1) .. +63
+// rows 64..127 of the staging tile, a third [64][TC_LT] buffer when the tile capacity is <= 64 rows (such a tile never
+// touches them): products read their A operand and leave their results wherever the next phase wants them, so the
+// small-tile kernels copy nothing between `tile` and `abuf`
+__device__ __forceinline__ TcRow* tc_aux(TcShared& sh) { return sh.tile + 64; }
+
+// acc (+)= A * W^T for the next job of the ring (all warps), A = a padded [rows][TC_LT] shared buffer: `abuf`, `tile`
+// or, for a tile capacity of <= 64 rows, `tc_aux(sh)`.  Warpgroup q = warp / 4 computes rows 64 * (q & 1) .. +63
 // and columns 64 * (q >> 1) .. +63 of the 128 x 128 product; each K-step is three tf32 MMAs, lo * hi + hi * lo + hi * hi
 // (~ fp32 accuracy).  A warpgroup whose rows all lie at or past `nvalid` only releases the ring stages (so a tile
-// capacity of <= 64 rows never reads rows 64.. of `abuf`, where its third ring stage lives).  Per K-slab the A
+// capacity of <= 64 rows never reads rows 64.. of its A buffer: the third ring stage, or `tc_aux`).  Per K-slab the A
 // fragments are split into tf32 hi / lo as they are loaded (before the slab's weights are waited for), one commit group
 // of 12 MMAs runs, and the stage is released as soon as that group retires: a product streams 128 KB of weights through
 // the ring, and an early release is worth more than MMAs kept in flight across slabs.  On return `acc` holds this
 // thread's part of the product (layout: tc_common.cuh).
 template <int ROWS>
-__device__ __forceinline__ void tc2_mma(TcShared& sh, TcRing<ROWS>& ring, float (&acc)[32], int accumulate, int warp, int lane,
-                                        int nvalid) {
+__device__ __forceinline__ void tc2_mma(TcShared& sh, TcRing<ROWS>& ring, const TcRow* A, float (&acc)[32], int accumulate,
+                                        int warp, int lane, int nvalid) {
     constexpr int NS = TcRing<ROWS>::NS;
     csync();                                                   // the A operand is complete
     const int q = warp >> 2, m0 = (q & 1) * 64 + (warp & 3) * 16, g = lane >> 2, t = lane & 3;
@@ -178,10 +188,10 @@ __device__ __forceinline__ void tc2_mma(TcShared& sh, TcRing<ROWS>& ring, float 
 #pragma unroll
             for (int kk = 0; kk < 4; kk++) {
                 const int kc = k0 + kk * 8;
-                tc::split_tf32(sh.abuf[m0 + g][kc], ahi[kk][0], alo[kk][0]);
-                tc::split_tf32(sh.abuf[m0 + g + 8][kc], ahi[kk][1], alo[kk][1]);
-                tc::split_tf32(sh.abuf[m0 + g][kc + 4], ahi[kk][2], alo[kk][2]);
-                tc::split_tf32(sh.abuf[m0 + g + 8][kc + 4], ahi[kk][3], alo[kk][3]);
+                tc::split_tf32(A[m0 + g][kc], ahi[kk][0], alo[kk][0]);
+                tc::split_tf32(A[m0 + g + 8][kc], ahi[kk][1], alo[kk][1]);
+                tc::split_tf32(A[m0 + g][kc + 4], ahi[kk][2], alo[kk][2]);
+                tc::split_tf32(A[m0 + g + 8][kc + 4], ahi[kk][3], alo[kk][3]);
             }
             tc::mbar_wait(&sh.b_full[stage], (uint32_t)(k / NS) & 1u);
             const uint32_t bhi = tc::smem_u32(tc_stage_ptr(sh, stage)) + (uint32_t)(q >> 1) * (64 * 128);
@@ -211,13 +221,13 @@ __device__ __forceinline__ void tc2_mma(TcShared& sh, TcRing<ROWS>& ring, float 
     ring.next += TC_SLABS;
 }
 
-// accumulator -> staging tile (rows below `nvalid`)
-__device__ __forceinline__ void tc2_acc_to_tile(TcShared& sh, const float (&acc)[32], int warp, int lane, int nvalid) {
+// accumulator -> a padded [rows][TC_LT] shared buffer (rows below `nvalid`)
+__device__ __forceinline__ void tc2_acc_to(TcRow* dst, const float (&acc)[32], int warp, int lane, int nvalid) {
     const int q = warp >> 2, r = (q & 1) * 64 + (warp & 3) * 16 + (lane >> 2), c = (q >> 1) * 64 + 2 * (lane & 3);
 #pragma unroll
     for (int i = 0; i < 8; i++) {
-        if (r < nvalid) *reinterpret_cast<float2*>(&sh.tile[r][c + 8 * i]) = make_float2(acc[4 * i], acc[4 * i + 1]);
-        if (r + 8 < nvalid) *reinterpret_cast<float2*>(&sh.tile[r + 8][c + 8 * i]) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
+        if (r < nvalid) *reinterpret_cast<float2*>(&dst[r][c + 8 * i]) = make_float2(acc[4 * i], acc[4 * i + 1]);
+        if (r + 8 < nvalid) *reinterpret_cast<float2*>(&dst[r + 8][c + 8 * i]) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
     }
 }
 
@@ -243,9 +253,9 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) tc_selftest_kernel(const float
             st4(&sh.tile[r][c], ld4(A + (size_t)r * D + c));
         }
         tc2_tile_to_a(sh, ROWS);
-        tc2_mma(sh, ring, acc, 0, warp, lane, ROWS);
+        tc2_mma(sh, ring, sh.abuf, acc, 0, warp, lane, ROWS);
         csync();
-        tc2_acc_to_tile(sh, acc, warp, lane, ROWS);
+        tc2_acc_to(sh.tile, acc, warp, lane, ROWS);
         csync();
         for (int idx = threadIdx.x; idx < ROWS * (D / 4); idx += TC2_CTHREADS) {
             const int r = idx >> 5, c = (idx & 31) * 4;
@@ -270,6 +280,7 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_fwd_tc_kernel(const __gri
     const bool upd = (l < L - 1);
     const int J_DK = 0, J_DV = 1, J_F = 2, J_S1 = upd ? 3 : 2, J_S2 = upd ? 4 : 3;
     constexpr int RPW = ROWS / TC2_CWARPS;      // rows per compute warp in the coalesced phases
+    constexpr bool SMALL = ROWS <= 64;          // tile_to_a-free schedule: m stays in `tile`, f rows in `abuf`, results in tc_aux
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, col = lane * 4;
     const int E = ws.rowptr[ws.N];
     const int trows = min(ROWS, max(16, a.tile_rows));          // edges per tile (<= ROWS, chosen on the host so the tiles fill whole waves)
@@ -298,7 +309,8 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_fwd_tc_kernel(const __gri
         // keeps every warp busy (slot s of a warp is row warp * rpw + s, valid while s < rpw and the row exists)
         const int rpw = (nvalid + TC2_CWARPS - 1) / TC2_CWARPS, r0 = warp * rpw;
         // ---- per-edge feature rows -> the A operand buffer by TMA bulk copies (one 512 B row each, padded rows in
-        //      shared memory), completion on an mbarrier: f is only ever read as the A operand (dk, dv, f products) ----
+        //      shared memory), completion on an mbarrier: f is the A operand of the dk, dv and f products (and, in a
+        //      tile of <= 64 rows, the edge update's residual) ----
         {
             constexpr int RW = ROWS / TC2_CWARPS;                 // rows a warp issues
             const int w0 = warp * RW, wn = max(0, min(RW, nvalid - w0));
@@ -315,9 +327,9 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_fwd_tc_kernel(const __gri
         TC_TL(2);
         // ---- dk -> attention weights ----
         float Areg[RPW];
-        tc2_mma(sh, ring, acc, a.jobs[J_DK].accumulate, warp, lane, nvalid);
+        tc2_mma(sh, ring, sh.abuf, acc, a.jobs[J_DK].accumulate, warp, lane, nvalid);
         TC_TL(4);
-        tc2_acc_to_tile(sh, acc, warp, lane, nvalid);         // (nothing reads the tile between the MMAs' barrier and here)
+        tc2_acc_to(sh.tile, acc, warp, lane, nvalid);         // (nothing reads the tile between the MMAs' barrier and here)
         csync();
         {
             TC_TL(5);
@@ -339,10 +351,10 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_fwd_tc_kernel(const __gri
         }
         TC_TL(6);
         // ---- dv -> message m (in place in the tile) ----
-        tc2_mma(sh, ring, acc, a.jobs[J_DV].accumulate, warp, lane, nvalid);
+        tc2_mma(sh, ring, sh.abuf, acc, a.jobs[J_DV].accumulate, warp, lane, nvalid);
         TC_TL(7);
         csync();
-        tc2_acc_to_tile(sh, acc, warp, lane, nvalid);
+        tc2_acc_to(sh.tile, acc, warp, lane, nvalid);
         csync();
         {
             TC_TL(8);
@@ -372,14 +384,16 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_fwd_tc_kernel(const __gri
             }
         }
         TC_TL(10);
-        // ---- A = m, start s1 (-> D1) ----
-        if (upd) tc2_mma(sh, ring, acc, a.jobs[J_F].accumulate, warp, lane, nvalid);
-        tc2_tile_to_a(sh, nvalid);
+        // ---- f product; A = m for s1 and s2: a tile of <= 64 rows leaves m in `tile` (the products read it there) and
+        //      keeps the f rows in `abuf` for the edge update, a longer one copies m into `abuf` ----
+        if (upd) tc2_mma(sh, ring, sh.abuf, acc, a.jobs[J_F].accumulate, warp, lane, nvalid);
+        if constexpr (!SMALL) tc2_tile_to_a(sh, nvalid);
         TC_TL(11);
         // ---- edge update from the f chunk (D0) ----
         if (upd) {
-            csync();                                          // m tile fully consumed (xa + A copy)
-            tc2_acc_to_tile(sh, acc, warp, lane, nvalid);
+            TcRow* const pfb = SMALL ? tc_aux(sh) : sh.tile;
+            if constexpr (!SMALL) csync();                   // m tile fully consumed (xa + A copy)
+            tc2_acc_to(pfb, acc, warp, lane, nvalid);
             csync();
             const float4 bb = ldg4(lw.b1 + 2 * D + col);
 #pragma unroll 1
@@ -390,7 +404,8 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_fwd_tc_kernel(const __gri
                 for (int u = 0; u < 2; u++) {
                     const int row = r0 + rb + u;
                     const size_t i3 = (size_t)sh.meta.dst[row] * 3, j3 = (size_t)sh.meta.src[row] * 3;
-                    fin[u] = (rb + u < rpw && row < nvalid) ? ldg4(Fin + (size_t)(e0 + row) * D + col) : f4s(0.f);
+                    if (rb + u < rpw && row < nvalid) fin[u] = SMALL ? ld4(&sh.abuf[row][col]) : ldg4(Fin + (size_t)(e0 + row) * D + col);
+                    else fin[u] = f4s(0.f);
 #pragma unroll
                     for (int s = 0; s < 3; s++) {
                         tir[u][s] = ldg4(TU + (i3 + s) * 2 * D + col);
@@ -401,7 +416,7 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_fwd_tc_kernel(const __gri
                 for (int u = 0; u < 2; u++) {
                     const int row = r0 + rb + u;
                     const float4 dd = sh.meta.d[row];
-                    const float4 Pf = ld4(&sh.tile[row][col]) + bb;
+                    const float4 Pf = ld4(&pfb[row][col]) + bb;
                     const float4 fp = silu4(Pf);
                     const float4 a1 = tir[u][0] * dd.x + tir[u][1] * dd.y + tir[u][2] * dd.z;
                     const float4 a2 = ujr[u][0] * dd.x + ujr[u][1] * dd.y + ujr[u][2] * dd.z;
@@ -417,10 +432,11 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_fwd_tc_kernel(const __gri
         TC_TL(12);
         // ---- s1 (D1): va_i += sum_e vn_j * s1 ----
         float bnd[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
-        tc2_mma(sh, ring, acc, a.jobs[J_S1].accumulate, warp, lane, nvalid);
+        TcRow* const s1b = SMALL ? tc_aux(sh) : sh.tile;
+        tc2_mma(sh, ring, SMALL ? sh.tile : sh.abuf, acc, a.jobs[J_S1].accumulate, warp, lane, nvalid);
         TC_TL(13);
-        csync();
-        tc2_acc_to_tile(sh, acc, warp, lane, nvalid);
+        if constexpr (!SMALL) csync();
+        tc2_acc_to(s1b, acc, warp, lane, nvalid);
         csync();
         {
             TC_TL(14);
@@ -438,7 +454,7 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_fwd_tc_kernel(const __gri
                     for (int u = 0; u < 4; u++) {
                         const size_t j3 = (size_t)sh.meta.src[r + u] * 3;
                         g[u][0] = __ldg(VN + (j3 + 0) * D + cch); g[u][1] = __ldg(VN + (j3 + 1) * D + cch); g[u][2] = __ldg(VN + (j3 + 2) * D + cch);
-                        const float sp = sh.tile[r + u][cch] + b;
+                        const float sp = s1b[r + u][cch] + b;
                         SP[(size_t)(e0 + r + u) * 2 * D + cch] = sp;
                         s1[u] = silu_(sp);
                     }
@@ -447,7 +463,7 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_fwd_tc_kernel(const __gri
                 }
                 for (; r < hi; r++) {
                     const size_t j3 = (size_t)sh.meta.src[r] * 3;
-                    const float sp = sh.tile[r][cch] + b;
+                    const float sp = s1b[r][cch] + b;
                     SP[(size_t)(e0 + r) * 2 * D + cch] = sp;
                     const float s1 = silu_(sp);
                     v0 += __ldg(VN + (j3 + 0) * D + cch) * s1;
@@ -470,10 +486,11 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_fwd_tc_kernel(const __gri
             tc::tma_prefetch_l2(Fin + (size_t)en * D, (uint32_t)min(trows, E - en) * D * 4);
         }
         // ---- s2 (D0): va_i += sum_e s2 * d ----
-        tc2_mma(sh, ring, acc, a.jobs[J_S2].accumulate, warp, lane, nvalid);
+        TcRow* const s2b = SMALL ? sh.abuf : sh.tile;
+        tc2_mma(sh, ring, SMALL ? sh.tile : sh.abuf, acc, a.jobs[J_S2].accumulate, warp, lane, nvalid);
         TC_TL(16);
-        csync();
-        tc2_acc_to_tile(sh, acc, warp, lane, nvalid);
+        if constexpr (!SMALL) csync();
+        tc2_acc_to(s2b, acc, warp, lane, nvalid);
         csync();
         {
             TC_TL(17);
@@ -486,7 +503,7 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_fwd_tc_kernel(const __gri
                 float v0 = 0.f, v1 = 0.f, v2 = 0.f;
                 for (int r = lo; r < hi; r++) {
                     const float4 de = sh.meta.d[r];
-                    const float sp = sh.tile[r][cch] + b;
+                    const float sp = s2b[r][cch] + b;
                     SP[(size_t)(e0 + r) * 2 * D + D + cch] = sp;
                     const float s2 = silu_(sp);
                     v0 += s2 * de.x; v1 += s2 * de.y; v2 += s2 * de.z;
@@ -530,6 +547,9 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_bwd_tc_kernel(const __gri
     const int J_LAST = upd ? J_G4F : J_G4DK;
     constexpr int RPW = ROWS / TC2_CWARPS;
     constexpr int RB4 = (RPW % 4 == 0) ? 4 : 2;     // rows whose loads are issued together
+    constexpr bool SMALL = ROWS <= 64;              // tile_to_a-free schedule: products read A where it was written, side
+                                                    // results go to tc_aux, and no row set is gathered twice
+    constexpr int RBM = SMALL ? 2 : RB4;            // g_m phase: its merged neighbours leave fewer registers (0 spills)
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, col = lane * 4, hd = lane >> 2;
     const int E = ws.rowptr[ws.N];
     const int trows = min(ROWS, max(16, a.tile_rows));          // edges per tile (<= ROWS, chosen on the host so the tiles fill whole waves)
@@ -557,74 +577,118 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_bwd_tc_kernel(const __gri
         load_edge_meta<TC_TE, TC2_CTHREADS>(sh.meta, ws, e0, nvalid);
         csync();
         TC_TL(2);
-        // ---- s1 half: g_Spre[:, 0:128] -> A (written in place: the previous tile's products are done) ; source-side g_vn ----
-        // (loads of 4 rows are issued together: the atomics below are compiler barriers for load hoisting)
+        if constexpr (SMALL) {
+            // ---- both halves in one pass (a target's GVEC rows are gathered once): g_Spre[:, 0:128] -> abuf (A of g3a),
+            //      g_Spre[:, 128:256] -> tile (A of g3b), written in place (the previous tile's products are done) ;
+            //      source-side g_vn, dE/dd ----
 #pragma unroll 1
-        for (int rb = 0; rb < RPW; rb += RB4) {
-            if (rb >= rpw) break;
-            float4 sp[RB4], gM[RB4][3], vn[RB4][3];
+            for (int rb = 0; rb < RPW; rb += RB4) {
+                if (rb >= rpw) break;
+                float4 sp[RB4][2], gM[RB4][3], vn[RB4][3];
 #pragma unroll
-            for (int u = 0; u < RB4; u++) {
-                const int row = r0 + rb + u;
-                const size_t e = (size_t)(e0 + ((rb + u < rpw && row < nvalid) ? row : 0));
-                const size_t i3 = (size_t)sh.meta.dst[row] * 3, j3 = (size_t)sh.meta.src[row] * 3;
-                sp[u] = ldg4(SP + e * 2 * D + col);
+                for (int u = 0; u < RB4; u++) {
+                    const int row = r0 + rb + u;
+                    const size_t e = (size_t)(e0 + ((rb + u < rpw && row < nvalid) ? row : 0));
+                    const size_t i3 = (size_t)sh.meta.dst[row] * 3, j3 = (size_t)sh.meta.src[row] * 3;
+                    sp[u][0] = ldg4(SP + e * 2 * D + col);
+                    sp[u][1] = ldg4(SP + e * 2 * D + D + col);
 #pragma unroll
-                for (int s = 0; s < 3; s++) { gM[u][s] = ldg4(ws.GVEC + (i3 + s) * D + col); vn[u][s] = ldg4(VN + (j3 + s) * D + col); }
-            }
+                    for (int s = 0; s < 3; s++) { gM[u][s] = ldg4(ws.GVEC + (i3 + s) * D + col); vn[u][s] = ldg4(VN + (j3 + s) * D + col); }
+                }
 #pragma unroll
-            for (int u = 0; u < RB4; u++) {
-                const int row = r0 + rb + u;
-                const bool ok = (rb + u < rpw && row < nvalid);
-                const size_t j3 = (size_t)sh.meta.src[row] * 3;
-                const float4 s1 = silu4(sp[u]);
-                const float4 gs1 = gM[u][0] * vn[u][0] + gM[u][1] * vn[u][1] + gM[u][2] * vn[u][2];
-                if (rb + u < rpw) st4(&sh.abuf[row][col], ok ? gs1 * dsilu4(sp[u]) : f4s(0.f));   // (a slot past the run is the next warp's row)
-                if (ok) {
-                    red4(ws.GVNMSG + (j3 + 0) * D + col, gM[u][0] * s1);
-                    red4(ws.GVNMSG + (j3 + 1) * D + col, gM[u][1] * s1);
-                    red4(ws.GVNMSG + (j3 + 2) * D + col, gM[u][2] * s1);
+                for (int u = 0; u < RB4; u++) {
+                    const int row = r0 + rb + u;
+                    const bool mine = rb + u < rpw, ok = (mine && row < nvalid);   // (a slot past the run is the next warp's row)
+                    const size_t j3 = (size_t)sh.meta.src[row] * 3;
+                    const float4 dd = sh.meta.d[row];
+                    const float4 s1 = silu4(sp[u][0]), s2 = silu4(sp[u][1]);
+                    const float4 gs1 = gM[u][0] * vn[u][0] + gM[u][1] * vn[u][1] + gM[u][2] * vn[u][2];
+                    const float gx_ = warp_sum(hsum4(gM[u][0] * s2)), gy_ = warp_sum(hsum4(gM[u][1] * s2)), gz_ = warp_sum(hsum4(gM[u][2] * s2));
+                    if (mine) {
+                        st4(&sh.abuf[row][col], ok ? gs1 * dsilu4(sp[u][0]) : f4s(0.f));
+                        st4(&sh.tile[row][col], ok ? (gM[u][0] * dd.x + gM[u][1] * dd.y + gM[u][2] * dd.z) * dsilu4(sp[u][1]) : f4s(0.f));
+                        if (lane == 0) { sh.eacc[row][1] = gx_; sh.eacc[row][2] = gy_; sh.eacc[row][3] = gz_; }
+                    }
+                    if (ok) {
+                        red4(ws.GVNMSG + (j3 + 0) * D + col, gM[u][0] * s1);
+                        red4(ws.GVNMSG + (j3 + 1) * D + col, gM[u][1] * s1);
+                        red4(ws.GVNMSG + (j3 + 2) * D + col, gM[u][2] * s1);
+                    }
                 }
             }
-        }
-        TC_TL(3);
-        // ---- s2 half (into the tile; the g3a product's barrier publishes the A rows above) ----
+            TC_TL(3);
+        } else {
+            // ---- s1 half: g_Spre[:, 0:128] -> A (written in place: the previous tile's products are done) ; source-side g_vn ----
+            // (loads of 4 rows are issued together: the atomics below are compiler barriers for load hoisting)
+#pragma unroll 1
+            for (int rb = 0; rb < RPW; rb += RB4) {
+                if (rb >= rpw) break;
+                float4 sp[RB4], gM[RB4][3], vn[RB4][3];
+#pragma unroll
+                for (int u = 0; u < RB4; u++) {
+                    const int row = r0 + rb + u;
+                    const size_t e = (size_t)(e0 + ((rb + u < rpw && row < nvalid) ? row : 0));
+                    const size_t i3 = (size_t)sh.meta.dst[row] * 3, j3 = (size_t)sh.meta.src[row] * 3;
+                    sp[u] = ldg4(SP + e * 2 * D + col);
+#pragma unroll
+                    for (int s = 0; s < 3; s++) { gM[u][s] = ldg4(ws.GVEC + (i3 + s) * D + col); vn[u][s] = ldg4(VN + (j3 + s) * D + col); }
+                }
+#pragma unroll
+                for (int u = 0; u < RB4; u++) {
+                    const int row = r0 + rb + u;
+                    const bool ok = (rb + u < rpw && row < nvalid);
+                    const size_t j3 = (size_t)sh.meta.src[row] * 3;
+                    const float4 s1 = silu4(sp[u]);
+                    const float4 gs1 = gM[u][0] * vn[u][0] + gM[u][1] * vn[u][1] + gM[u][2] * vn[u][2];
+                    if (rb + u < rpw) st4(&sh.abuf[row][col], ok ? gs1 * dsilu4(sp[u]) : f4s(0.f));   // (a slot past the run is the next warp's row)
+                    if (ok) {
+                        red4(ws.GVNMSG + (j3 + 0) * D + col, gM[u][0] * s1);
+                        red4(ws.GVNMSG + (j3 + 1) * D + col, gM[u][1] * s1);
+                        red4(ws.GVNMSG + (j3 + 2) * D + col, gM[u][2] * s1);
+                    }
+                }
+            }
+            TC_TL(3);
+            // ---- s2 half (into the tile; the g3a product's barrier publishes the A rows above) ----
 #pragma unroll 4
-        for (int r = 0; r < RPW; r++) {
-            if (r >= rpw) break;
-            const int row = r0 + r;
-            const bool ok = (r < rpw && row < nvalid);
-            const size_t e = (size_t)(e0 + (ok ? row : 0));
-            const size_t i3 = (size_t)sh.meta.dst[row] * 3;
-            const float4 dd = sh.meta.d[row];
-            const float4 sp = ldg4(SP + e * 2 * D + D + col);
-            const float4 s2 = silu4(sp);
-            const float4 gM0 = ldg4(ws.GVEC + (i3 + 0) * D + col), gM1 = ldg4(ws.GVEC + (i3 + 1) * D + col),
-                         gM2 = ldg4(ws.GVEC + (i3 + 2) * D + col);
-            const float gx_ = warp_sum(hsum4(gM0 * s2)), gy_ = warp_sum(hsum4(gM1 * s2)), gz_ = warp_sum(hsum4(gM2 * s2));
-            if (lane == 0) { sh.eacc[row][1] = gx_; sh.eacc[row][2] = gy_; sh.eacc[row][3] = gz_; }
-            st4(&sh.tile[row][col], ok ? (gM0 * dd.x + gM1 * dd.y + gM2 * dd.z) * dsilu4(sp) : f4s(0.f));
+            for (int r = 0; r < RPW; r++) {
+                if (r >= rpw) break;
+                const int row = r0 + r;
+                const bool ok = (r < rpw && row < nvalid);
+                const size_t e = (size_t)(e0 + (ok ? row : 0));
+                const size_t i3 = (size_t)sh.meta.dst[row] * 3;
+                const float4 dd = sh.meta.d[row];
+                const float4 sp = ldg4(SP + e * 2 * D + D + col);
+                const float4 s2 = silu4(sp);
+                const float4 gM0 = ldg4(ws.GVEC + (i3 + 0) * D + col), gM1 = ldg4(ws.GVEC + (i3 + 1) * D + col),
+                             gM2 = ldg4(ws.GVEC + (i3 + 2) * D + col);
+                const float gx_ = warp_sum(hsum4(gM0 * s2)), gy_ = warp_sum(hsum4(gM1 * s2)), gz_ = warp_sum(hsum4(gM2 * s2));
+                if (lane == 0) { sh.eacc[row][1] = gx_; sh.eacc[row][2] = gy_; sh.eacc[row][3] = gz_; }
+                st4(&sh.tile[row][col], ok ? (gM0 * dd.x + gM1 * dd.y + gM2 * dd.z) * dsilu4(sp) : f4s(0.f));
+            }
+            TC_TL(5);
         }
-        TC_TL(5);
         csync();
-        tc2_mma(sh, ring, acc, a.jobs[J_G3A].accumulate, warp, lane, nvalid);
+        tc2_mma(sh, ring, sh.abuf, acc, a.jobs[J_G3A].accumulate, warp, lane, nvalid);
         TC_TL(6);
-        tc2_tile_to_a(sh, nvalid);
-        TC_TL(7);
+        if constexpr (!SMALL) {
+            tc2_tile_to_a(sh, nvalid);
+            TC_TL(7);
+        }
         // ---- g_m = g_xa_i + g_Spre Ws ; adjoint of m = v_j dv A ----
-        tc2_mma(sh, ring, acc, a.jobs[J_G3B].accumulate, warp, lane, nvalid);
+        tc2_mma(sh, ring, SMALL ? sh.tile : sh.abuf, acc, a.jobs[J_G3B].accumulate, warp, lane, nvalid);
         TC_TL(8);
-        csync();
-        tc2_acc_to_tile(sh, acc, warp, lane, nvalid);
+        csync();                                 // (a tile of <= 64 rows: every warp is done with the tile as g3b's A)
+        tc2_acc_to(sh.tile, acc, warp, lane, nvalid);
         csync();
         TC_TL(9);
 #pragma unroll 1
-        for (int rb = 0; rb < RPW; rb += RB4) {
+        for (int rb = 0; rb < RPW; rb += RBM) {
             if (rb >= rpw) break;
-            float4 gxa[RB4], vjr[RB4], pdvr[RB4];
-            float avr[RB4];
+            float4 gxa[RBM], vjr[RBM], pdvr[RBM];
+            float avr[RBM];
 #pragma unroll
-            for (int u = 0; u < RB4; u++) {
+            for (int u = 0; u < RBM; u++) {
                 const int row = r0 + rb + u;
                 const size_t e = (size_t)(e0 + ((rb + u < rpw && row < nvalid) ? row : 0));
                 gxa[u] = load_gxa(ws, (size_t)sh.meta.dst[row], col);
@@ -633,7 +697,7 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_bwd_tc_kernel(const __gri
                 avr[u] = (rb + u < rpw && row < nvalid) ? __ldg(ATT + e * H + hd) : 0.f;
             }
 #pragma unroll
-            for (int u = 0; u < RB4; u++) {
+            for (int u = 0; u < RBM; u++) {
                 const int row = r0 + rb + u;
                 const bool ok = (rb + u < rpw && row < nvalid);
                 const size_t j = sh.meta.src[row];
@@ -642,7 +706,7 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_bwd_tc_kernel(const __gri
                 const bool mine = rb + u < rpw;                 // a slot past the run is the next warp's row: no shared accesses
                 const float4 gm = mine ? ld4(&sh.tile[row][col]) + gxa[u] : f4s(0.f);   // (its owner rewrites it in this phase)
                 const float4 dv = silu4(pdvr[u]);
-                if (mine) st4(&sh.abuf[row][col], ok ? gm * vjr[u] * A * dsilu4(pdvr[u]) : f4s(0.f));      // g_Pdv -> A (g3b done)
+                if (mine) st4(&sh.abuf[row][col], ok ? gm * vjr[u] * A * dsilu4(pdvr[u]) : f4s(0.f));      // g_Pdv -> A (g3a, g3b done)
                 const float gA = quad_sum(hsum4(gm * vjr[u] * dv));
                 if (mine && (lane & 3) == 0) sh.gattn[row][hd] = gA * Ce * dsilu_(av);
                 const float gc = warp_sum((lane & 3) == 0 ? gA * sa : 0.f);
@@ -652,7 +716,8 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_bwd_tc_kernel(const __gri
         }
         TC_TL(10);
         csync();                                 // gattn / A = g_Pdv complete
-        // ---- adjoint of a_h = sum q_i k_j dk : first g_Pdk (next A operand), then the g_q tile ----
+        // ---- adjoint of a_h = sum q_i k_j dk : g_Pdk (next A operand) ; in a tile of <= 64 rows also the per-edge g_q
+        //      rows (-> tc_aux), a longer tile gathers them again below once g_Pdk is copied into abuf ----
 #pragma unroll 1
         for (int rb = 0; rb < RPW; rb += RB4) {
             if (rb >= rpw) break;
@@ -673,40 +738,47 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_bwd_tc_kernel(const __gri
                 const float4 dk = silu4(pdkr[u]);
                 const float gav = sh.gattn[row][hd];
                 if (rb + u < rpw) st4(&sh.tile[row][col], ok ? qir[u] * kjr[u] * gav * dsilu4(pdkr[u]) : f4s(0.f));   // g_Pdk
+                if (SMALL && rb + u < rpw) st4(&tc_aux(sh)[row][col], kjr[u] * dk * gav);                            // g_q
                 if (ok) red4(ws.GQKV + j * 3 * D + D + col, qir[u] * dk * gav);
             }
         }
         TC_TL(12);
         csync();
-        tc2_mma(sh, ring, acc, a.jobs[J_G4DV].accumulate, warp, lane, nvalid);
+        tc2_mma(sh, ring, sh.abuf, acc, a.jobs[J_G4DV].accumulate, warp, lane, nvalid);
         TC_TL(13);
-        tc2_tile_to_a(sh, nvalid);               // A = g_Pdk
-        TC_TL(14);
-        csync();
+        if constexpr (!SMALL) {
+            tc2_tile_to_a(sh, nvalid);           // A = g_Pdk
+            TC_TL(14);
+            csync();
 #pragma unroll 4
-        for (int r = 0; r < RPW; r++) {
-            if (r >= rpw) break;
-            const int row = r0 + r;
-            const size_t e = (size_t)(e0 + ((r < rpw && row < nvalid) ? row : 0));
-            const float4 dk = silu4(ldg4(P1 + e * 3 * D + col));
-            const float4 kj = ldg4(QKV + (size_t)sh.meta.src[row] * 3 * D + D + col);
-            st4(&sh.tile[row][col], kj * dk * sh.gattn[row][hd]);                    // per-edge g_q contribution
+            for (int r = 0; r < RPW; r++) {
+                if (r >= rpw) break;
+                const int row = r0 + r;
+                const size_t e = (size_t)(e0 + ((r < rpw && row < nvalid) ? row : 0));
+                const float4 dk = silu4(ldg4(P1 + e * 3 * D + col));
+                const float4 kj = ldg4(QKV + (size_t)sh.meta.src[row] * 3 * D + D + col);
+                st4(&sh.tile[row][col], kj * dk * sh.gattn[row][hd]);                // per-edge g_q contribution
+            }
+            csync();
         }
-        csync();
         {
+            const TcRow* const gqb = SMALL ? tc_aux(sh) : sh.tile;
             const int i_first = sh.meta.dst[0], i_last = sh.meta.dst[nvalid - 1];
             for (int i = i_first + grp; i <= i_last; i += TC2_NGRP) {
                 const int q0 = ws.rowptr[i], q1 = ws.rowptr[i + 1];
                 const int lo = max(q0, e0) - e0, hi = min(q1, e0 + nvalid) - e0;
                 float gq = 0.f;
-                for (int r = lo; r < hi; r++) gq += sh.tile[r][cch];
+                for (int r = lo; r < hi; r++) gq += gqb[r][cch];
                 if (q0 >= e0 && q1 <= e0 + nvalid) ws.GQKV[(size_t)i * 3 * D + cch] = gq;
                 else atomicAdd(ws.GQKV + (size_t)i * 3 * D + cch, gq);
             }
         }
         TC_TL(15);
-        // ---- adjoint of the edge update: first g_Pf (A operand), then the g_wdot tile ----
+        // ---- adjoint of the edge update: g_Pf (A operand: abuf in a tile of <= 64 rows, free once g4dv has retired,
+        //      while `tile` still holds g_Pdk for g4dk) ; in a tile of <= 64 rows also the g_wdot rows (-> tc_aux, free once
+        //      the g_q sums are done), a longer tile gathers them again below once g_Pf is copied into abuf ----
         if (upd) {
+            TcRow* const gpfb = SMALL ? sh.abuf : sh.tile;
             csync();
 #pragma unroll 1
             for (int rb = 0; rb < RPW; rb += 2) {
@@ -743,7 +815,10 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_bwd_tc_kernel(const __gri
                     for (int s = 0; s < 3; s++) { w1[s] = tir[u][s] - a1 * dv3[s]; w2[s] = ujr[u][s] - a2 * dv3[s]; }
                     const float4 wdot = w1[0] * w2[0] + w1[1] * w2[1] + w1[2] * w2[2];
                     const float4 gwd = gfn * fp;
-                    if (rb + u < rpw) st4(&sh.tile[row][col], gfn * wdot * dsilu4(pf));                    // g_Pf
+                    if (rb + u < rpw) {
+                        st4(&gpfb[row][col], gfn * wdot * dsilu4(pf));                                     // g_Pf
+                        if (SMALL) st4(&tc_aux(sh)[row][col], gwd);                                        // g_wdot
+                    }
                     const float4 c1 = gwd * (w2[0] * dd.x + w2[1] * dd.y + w2[2] * dd.z);
                     const float4 c2 = gwd * (w1[0] * dd.x + w1[1] * dd.y + w1[2] * dd.z);
                     float gdl[3];
@@ -765,22 +840,25 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_bwd_tc_kernel(const __gri
             }
             TC_TL(16);
             csync();
-            tc2_mma(sh, ring, acc, a.jobs[J_G4DK].accumulate, warp, lane, nvalid);
+            tc2_mma(sh, ring, SMALL ? sh.tile : sh.abuf, acc, a.jobs[J_G4DK].accumulate, warp, lane, nvalid);
             TC_TL(17);
-            tc2_tile_to_a(sh, nvalid);           // A = g_Pf
-            TC_TL(18);
-            csync();
+            if constexpr (!SMALL) {
+                tc2_tile_to_a(sh, nvalid);       // A = g_Pf
+                TC_TL(18);
+                csync();
 #pragma unroll 4
-            for (int r = 0; r < RPW; r++) {
-                if (r >= rpw) break;
-                const int row = r0 + r;
-                const bool ok = (r < rpw && row < nvalid);
-                const size_t e = (size_t)(e0 + (ok ? row : 0));
-                const float4 gfn = ok ? ld4(ws.GF + e * D + col) : f4s(0.f);
-                st4(&sh.tile[row][col], gfn * silu4(ldg4(P1 + e * 3 * D + 2 * D + col)));   // g_wdot
+                for (int r = 0; r < RPW; r++) {
+                    if (r >= rpw) break;
+                    const int row = r0 + r;
+                    const bool ok = (r < rpw && row < nvalid);
+                    const size_t e = (size_t)(e0 + (ok ? row : 0));
+                    const float4 gfn = ok ? ld4(ws.GF + e * D + col) : f4s(0.f);
+                    st4(&sh.tile[row][col], gfn * silu4(ldg4(P1 + e * 3 * D + 2 * D + col)));   // g_wdot
+                }
+                csync();
             }
-            csync();
             {
+                const TcRow* const gwb = SMALL ? tc_aux(sh) : sh.tile;
                 const int i_first = sh.meta.dst[0], i_last = sh.meta.dst[nvalid - 1];
                 for (int i = i_first + grp; i <= i_last; i += TC2_NGRP) {
                     const int q0 = ws.rowptr[i], q1 = ws.rowptr[i + 1];
@@ -788,7 +866,7 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_bwd_tc_kernel(const __gri
                     float gt0 = 0.f, gt1 = 0.f, gt2 = 0.f;
                     auto term = [&](int r, float u0, float u1, float u2) {
                         const float4 dd = sh.meta.d[r];
-                        const float gw = sh.tile[r][cch];
+                        const float gw = gwb[r][cch];
                         const float a2 = u0 * dd.x + u1 * dd.y + u2 * dd.z;
                         const float w20 = u0 - a2 * dd.x, w21 = u1 - a2 * dd.y, w22 = u2 - a2 * dd.z;
                         const float wd = w20 * dd.x + w21 * dd.y + w22 * dd.z;
@@ -837,10 +915,10 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_bwd_tc_kernel(const __gri
             else tc::tma_prefetch_l2(ATT + (size_t)en * H, nn * H * 4);
         }
         // ---- g_f = g_f_next + [g_Pdk|g_Pdv|g_Pf] W1 ----
-        tc2_mma(sh, ring, acc, a.jobs[J_LAST].accumulate, warp, lane, nvalid);
+        tc2_mma(sh, ring, (SMALL && !upd) ? sh.tile : sh.abuf, acc, a.jobs[J_LAST].accumulate, warp, lane, nvalid);
         TC_TL(20);
-        csync();
-        tc2_acc_to_tile(sh, acc, warp, lane, nvalid);
+        if (!SMALL || !upd) csync();             // (the tile is free unless it was this product's A)
+        tc2_acc_to(sh.tile, acc, warp, lane, nvalid);
         csync();
         TC_TL(21);
 #pragma unroll 4

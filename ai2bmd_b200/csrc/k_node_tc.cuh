@@ -102,9 +102,9 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) node_tc_kernel(const __grid_co
         load_a(0);
         tc2_tile_to_a(sh, nvalid);
         for (int j = 0; j < nj; j++) {
-            tc2_mma(sh, ring, acc, jl[j].accumulate, warp, lane, nvalid);
+            tc2_mma(sh, ring, sh.abuf, acc, jl[j].accumulate, warp, lane, nvalid);
             csync();                                          // the tile is free (A copied / previous chunk stored)
-            tc2_acc_to_tile(sh, acc, warp, lane, nvalid);
+            tc2_acc_to(sh.tile, acc, warp, lane, nvalid);
             csync();
             const int jj = j0 + j;
             for (int r = warp; r < nvalid; r += TC2_CWARPS) {
@@ -125,10 +125,10 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) node_tc_kernel(const __grid_co
         for (int j = 0; j < nj; j++) {
             load_a(j0 + j);                                   // (the previous chunk's MMAs began with a barrier: tile free)
             tc2_tile_to_a(sh, nvalid);
-            tc2_mma(sh, ring, acc, jl[j].accumulate, warp, lane, nvalid);
+            tc2_mma(sh, ring, sh.abuf, acc, jl[j].accumulate, warp, lane, nvalid);
         }
         csync();
-        tc2_acc_to_tile(sh, acc, warp, lane, nvalid);
+        tc2_acc_to(sh.tile, acc, warp, lane, nvalid);
         csync();
         for (int r = warp; r < nvalid; r += TC2_CWARPS) {
             const size_t row = (size_t)(row0 + r);

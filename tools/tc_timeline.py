@@ -21,17 +21,19 @@ from ai2bmd_b200.fixtures import WEIGHTS, load_fragments   # noqa: E402
 from ai2bmd_b200.synth import synthetic_batch    # noqa: E402
 from ai2bmd_b200.weights import load_state_dict  # noqa: E402
 
+# Slots marked "96/128 rows" are stamped only by the two-buffer schedule of 96- and 128-row tiles; a tile of <= 64 rows
+# copies no A operand and gathers no row set twice (its s1/s2, g_Pdk/g_q and g_Pf/g_wdot rows are written in one pass).
 FWD = {0: "kernel start", 1: "setup done (barriers)", 2: "f rows (= A) + meta loaded",
        4: "dk MMAs done", 5: "dk -> tile", 6: "attention weights done", 7: "dv MMAs done", 8: "dv -> tile",
-       9: "messages m done", 10: "xa aggregation done", 11: "A=m copied", 12: "edge update (f) done",
-       13: "s1 MMAs done", 14: "s1 -> tile", 15: "s1 aggregation done", 16: "s2 MMAs done", 17: "s2 -> tile",
-       18: "s2 aggregation done", 31: "teardown done"}
-BWD = {0: "kernel start", 1: "setup done", 2: "meta loaded", 3: "s1-half SIMT done (= A of g3a)",
-       5: "s2-half SIMT done", 6: "g3a MMAs done", 7: "A copied (g3b)", 8: "g3b MMAs done", 9: "g_m -> tile",
-       10: "g_m / g_Pdv SIMT done (= A of g4dv)", 12: "g_Pdk SIMT done", 13: "g4dv MMAs done",
-       14: "A copied (g4dk)", 15: "g_q tile + aggregation done", 16: "g_Pf SIMT done", 17: "g4dk MMAs done",
-       18: "A copied (g4f)", 19: "g_wdot tile + aggregation done", 20: "last job MMAs done", 21: "g_f -> tile",
-       22: "g_f written", 31: "teardown done"}
+       9: "messages m done", 10: "xa aggregation done", 11: "f MMAs done (96/128 rows: + A=m copy)",
+       12: "edge update (f) done", 13: "s1 MMAs done", 14: "s1 -> buffer", 15: "s1 aggregation done",
+       16: "s2 MMAs done", 17: "s2 -> buffer", 18: "s2 aggregation done", 31: "teardown done"}
+BWD = {0: "kernel start", 1: "setup done", 2: "meta loaded", 3: "s1-half SIMT done (<=64 rows: s1+s2)",
+       5: "s2-half SIMT done (96/128 rows)", 6: "g3a MMAs done", 7: "A copied for g3b (96/128 rows)", 8: "g3b MMAs done",
+       9: "g_m -> tile", 10: "g_m / g_Pdv SIMT done (= A of g4dv)", 12: "g_Pdk SIMT done (<=64 rows: + g_q)",
+       13: "g4dv MMAs done", 14: "A copied for g4dk (96/128 rows)", 15: "g_q aggregation done",
+       16: "g_Pf SIMT done (<=64 rows: + g_wdot)", 17: "g4dk MMAs done", 18: "A copied for g4f (96/128 rows)",
+       19: "g_wdot aggregation done", 20: "last job MMAs done", 21: "g_f -> tile", 22: "g_f written", 31: "teardown done"}
 
 
 NFWD = {0: "start", 1: "xa rows staged", 2: "o_proj unit done", 4: "K-quarters summed", 5: "per-node phase done",
