@@ -4,6 +4,7 @@
 #include <cxxabi.h>
 
 #include <algorithm>
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -184,6 +185,10 @@ struct vb_handle {
     long long* d_step = nullptr;
     long long ehist_cap = 1 << 16;
     float* md_ef = nullptr;              // caller-owned [3*n_protein + 1]
+    // Hookean restraints (k_md.cuh MdRestraints): term CSR + rf [3*n_protein + 1] in one allocation
+    bool rs_ready = false;
+    MdRestraints rs{};
+    void* rs_mem = nullptr;
     // non-bonded MM term (k_nonbonded.cuh)
     bool nb_ready = false;
     NbParams nb{};
@@ -225,7 +230,12 @@ struct vb_handle {
         d_nb_q = d_nb_sigma = d_nb_eps = nullptr; d_nb_rowptr = d_nb_col = nullptr; d_nb_eatom = nullptr;
         nb_ready = false;
     }
+    void free_rs() {
+        cudaFree(rs_mem);
+        rs_mem = nullptr; rs = MdRestraints{}; rs_ready = false;
+    }
     void free_md() {
+        free_rs();                       // the restraints index the MD state
         cudaFree(d_mx); cudaFree(d_mv); cudaFree(d_mmass); cudaFree(d_ehist);
         cudaFree(d_real); cudaFree(d_acc); cudaFree(d_rem); cudaFree(d_blen); cudaFree(d_step);
         d_mx = d_mv = d_mmass = d_ehist = nullptr; d_real = d_acc = d_rem = nullptr; d_blen = nullptr; d_step = nullptr;
@@ -1163,10 +1173,13 @@ StepIO md_io(vb_handle* h) {
     io.ef = h->md_ef;
     return io;
 }
-// fragment placement -> evaluation + signed whole-protein reduction [-> non-bonded term], all on st
+// fragment placement [+ restraints into rf, one more CTA] -> evaluation + signed whole-protein reduction
+// [-> non-bonded term], all on st.  Every rank of a sharded run holds the same state and the whole term set, so each
+// computes the same rf; only ef goes through the all-reduce.
 int md_eval_enqueue(vb_handle* h, cudaStream_t st) {
     const int N = h->ws.N;
-    md_place_kernel<<<(N + 255) / 256, 256, 0, st>>>(N, h->d_real, h->d_acc, h->d_rem, h->d_blen, h->d_mx, h->d_pos);
+    md_place_kernel<<<(N + 255) / 256 + (h->rs_ready ? 1 : 0), 256, 0, st>>>(N, h->d_real, h->d_acc, h->d_rem, h->d_blen,
+                                                                            h->d_mx, h->d_pos, h->rs);
     if (h->caph_ready) caph_relax_kernel<<<1, CAPH_THREADS, 0, st>>>(h->caph, h->d_pos);   // hydrogen refinement, in place
     if (int rc = enqueue_eval(h, st, md_io(h))) return rc;
     if (h->nb_ready && h->nb.hi > h->nb.lo) {      // non-bonded MM term on the same protein coordinates
@@ -1178,10 +1191,11 @@ int md_eval_enqueue(vb_handle* h, cudaStream_t st) {
     return VB_OK;
 }
 void md_kick1_enqueue(vb_handle* h, cudaStream_t st) {
-    md_kick1_kernel<<<1, MD_K1_THREADS, 0, st>>>(h->md, h->d_step, h->d_mmass, h->md_ef, h->d_mx, h->d_mv);
+    md_kick1_kernel<<<1, MD_K1_THREADS, 0, st>>>(h->md, h->d_step, h->d_mmass, h->md_ef, h->rs.rf, h->d_mx, h->d_mv);
 }
 void md_kick2_enqueue(vb_handle* h, cudaStream_t st) {
-    md_kick2_kernel<<<1, MD_K2_THREADS, 0, st>>>(h->md, h->d_step, h->d_mmass, h->md_ef, h->d_mv, h->d_ehist, h->ehist_cap);
+    md_kick2_kernel<<<1, MD_K2_THREADS, 0, st>>>(h->md, h->d_step, h->d_mmass, h->md_ef, h->rs.rf, h->d_mv, h->d_ehist,
+                                                 h->ehist_cap);
 }
 int md_check(vb_handle* h, const char* who) {
     if (!h->md_ready) { h->set_error("%s: call vb_md_setup first", who); return VB_ERR_STATE; }
@@ -1260,6 +1274,86 @@ int vb_md_set_state(vb_handle* h, const double* x_host, const double* v_host, in
     CUDA_TRY(h, cudaMemcpy(h->d_mx, x_host, sizeof(double) * 3 * h->n_protein, cudaMemcpyHostToDevice));
     CUDA_TRY(h, cudaMemcpy(h->d_mv, v_host, sizeof(double) * 3 * h->n_protein, cudaMemcpyHostToDevice));
     CUDA_TRY(h, cudaMemcpy(h->d_step, &s, sizeof(long long), cudaMemcpyHostToDevice));
+    return VB_OK;
+}
+
+int vb_md_set_restraints(vb_handle* h, int64_t n_tether, const int32_t* tether_atom, double tether_k,
+                         int64_t n_spring, const int32_t* spring_ij, const double* spring_k, const double* spring_rt) {
+    if (!h) return VB_ERR_ARG;
+    std::lock_guard<std::mutex> lk(h->mu);
+    if (int rc = md_check(h, "vb_md_set_restraints")) return rc;
+    const int P = h->n_protein;
+    auto bad = [&](const char* what, long long i) {
+        h->set_error("vb_md_set_restraints: %s (term %lld)", what, i);
+        return VB_ERR_ARG;
+    };
+    if (n_tether < 0 || n_spring < 0 || n_tether > P || n_spring > (1 << 26)) return bad("bad term count", -1);
+    if (n_tether > 0 && (!tether_atom || !std::isfinite(tether_k) || tether_k < 0.0)) return bad("tether k must be finite and >= 0", -1);
+    if (n_spring > 0 && (!spring_ij || !spring_k || !spring_rt)) return bad("null spring array", -1);
+    std::vector<char> tethered(P, 0);
+    for (int64_t i = 0; i < n_tether; i++) {
+        const int a = tether_atom[i];
+        if (a < 0 || a >= P) return bad("tether atom out of range", i);
+        if (tethered[a]) return bad("atom tethered twice", i);
+        tethered[a] = 1;
+    }
+    for (int64_t s = 0; s < n_spring; s++) {
+        const int i = spring_ij[2 * s], j = spring_ij[2 * s + 1];
+        if (i < 0 || i >= P || j < 0 || j >= P) return bad("spring atom out of range", s);
+        if (i == j) return bad("spring between an atom and itself", s);
+        if (!std::isfinite(spring_k[s]) || spring_k[s] < 0.0 || !std::isfinite(spring_rt[s]) || spring_rt[s] < 0.0)
+            return bad("spring k and rt must be finite and >= 0", s);
+    }
+    CUDA_TRY(h, cudaSetDevice(h->device));
+    CUDA_TRY(h, cudaDeviceSynchronize());
+    h->drop_graph();              // the kick and placement launches hold rf / the term arrays
+    h->free_rs();
+    if (n_tether == 0 && n_spring == 0) return VB_OK;
+    // tethers are anchored where the atoms stand now (the reference re-anchors at the start of every stage)
+    std::vector<double> x(3 * (size_t)P);
+    CUDA_TRY(h, cudaMemcpy(x.data(), h->d_mx, sizeof(double) * 3 * P, cudaMemcpyDeviceToHost));
+    // CSR over atoms; an atom's terms in order: its tether, then its springs in the caller's order
+    const int64_t T = n_tether + 2 * n_spring;
+    std::vector<int> rowptr(P + 1, 0), partner(T);
+    std::vector<double> kk(T), rt(T), p0(3 * T, 0.0);
+    for (int64_t i = 0; i < n_tether; i++) rowptr[tether_atom[i] + 1]++;
+    for (int64_t s = 0; s < n_spring; s++) { rowptr[spring_ij[2 * s] + 1]++; rowptr[spring_ij[2 * s + 1] + 1]++; }
+    for (int p = 0; p < P; p++) rowptr[p + 1] += rowptr[p];
+    std::vector<int> fill(rowptr.begin(), rowptr.end() - 1);
+    for (int64_t i = 0; i < n_tether; i++) {
+        const int a = tether_atom[i], t = fill[a]++;
+        partner[t] = -1; kk[t] = tether_k; rt[t] = 0.0;
+        for (int c = 0; c < 3; c++) p0[3 * t + c] = x[3 * a + c];
+    }
+    for (int64_t s = 0; s < n_spring; s++) {
+        const int i = spring_ij[2 * s], j = spring_ij[2 * s + 1];
+        const int ti = fill[i]++, tj = fill[j]++;
+        partner[ti] = j; partner[tj] = i;
+        kk[ti] = kk[tj] = spring_k[s];
+        rt[ti] = rt[tj] = spring_rt[s];
+    }
+    // one allocation, carved in 256-byte steps
+    size_t total = 0;
+    auto carve = [&](size_t bytes) { const size_t o = total; total += (bytes + 255) & ~(size_t)255; return o; };
+    const size_t o_rf = carve(sizeof(double) * (3 * (size_t)P + 1)), o_k = carve(sizeof(double) * T),
+                 o_rt = carve(sizeof(double) * T), o_p0 = carve(sizeof(double) * 3 * T),
+                 o_row = carve(sizeof(int) * (P + 1)), o_par = carve(sizeof(int) * T);
+    CUDA_TRY(h, cudaMalloc(&h->rs_mem, total));
+    char* base = static_cast<char*>(h->rs_mem);
+    CUDA_TRY(h, cudaMemset(base + o_rf, 0, sizeof(double) * (3 * (size_t)P + 1)));
+    CUDA_TRY(h, cudaMemcpy(base + o_k, kk.data(), sizeof(double) * T, cudaMemcpyHostToDevice));
+    CUDA_TRY(h, cudaMemcpy(base + o_rt, rt.data(), sizeof(double) * T, cudaMemcpyHostToDevice));
+    CUDA_TRY(h, cudaMemcpy(base + o_p0, p0.data(), sizeof(double) * 3 * T, cudaMemcpyHostToDevice));
+    CUDA_TRY(h, cudaMemcpy(base + o_row, rowptr.data(), sizeof(int) * (P + 1), cudaMemcpyHostToDevice));
+    CUDA_TRY(h, cudaMemcpy(base + o_par, partner.data(), sizeof(int) * T, cudaMemcpyHostToDevice));
+    h->rs = MdRestraints{P, reinterpret_cast<int*>(base + o_row), reinterpret_cast<int*>(base + o_par),
+                         reinterpret_cast<double*>(base + o_k), reinterpret_cast<double*>(base + o_rt),
+                         reinterpret_cast<double*>(base + o_p0), reinterpret_cast<double*>(base + o_rf)};
+    h->rs_ready = true;
+    // rf at the current positions, so the next kick1 already sees this set: the restraint CTA alone (no atom to place)
+    md_place_kernel<<<1, 256, 0, h->own_stream>>>(0, nullptr, nullptr, nullptr, nullptr, h->d_mx, nullptr, h->rs);
+    CUDA_TRY(h, cudaGetLastError());
+    CUDA_TRY(h, cudaStreamSynchronize(h->own_stream));
     return VB_OK;
 }
 
@@ -1809,6 +1903,7 @@ int64_t vb_debug_read(vb_handle* h, const char* name, int layer, void* host_dst,
     else BUF("eatom", ws.eatom, N, 4)
     else BUF("energy", h->d_energy, G, 4)
     else BUF("forces", h->d_forces, N * 3, 4)
+    else if (k == "RF" && h->rs_ready) { src = h->rs.rf; bytes = (3 * (size_t)h->n_protein + 1) * 8; }
 #undef BUF
     if (!src) { h->set_error("vb_debug_read: unknown buffer %s[%d]", name, layer); return VB_ERR_ARG; }
     if ((int64_t)bytes > cap_bytes) bytes = (size_t)cap_bytes;

@@ -4,6 +4,7 @@
 //     recalled, restated on the host in ai2bmd_b200/md.py which is this file's checker);
 //   * placement of every packed fragment atom from the protein coordinates, cap hydrogens on the acceptor->removed ray
 //     (src/Fragmentation/distancefrag.py:34-54; host restatement ai2bmd_b200/pdbfrag.py FragmentRecipe.positions).
+//   * optional Hookean position / bond restraints on top of the calculator forces (see MdRestraints below).
 // State (positions, velocities) is fp64 like ASE's numpy arrays; forces arrive as the fp32 whole-protein buffer
 // [3*n_protein + 1] the signed fragment reduction writes.  Normals come from a counter-based Philox4x32-10 stream
 // keyed by (seed; step, component), so every rank of a sharded run draws identical numbers without communication.
@@ -71,6 +72,7 @@ __device__ inline MdCoef md_coef(const MdParams& p, double mass) {
 constexpr int MD_K1_THREADS = 1024;
 __global__ void __launch_bounds__(MD_K1_THREADS) md_kick1_kernel(MdParams p, const long long* __restrict__ step_ctr,
                                                                  const double* __restrict__ mass, const float* __restrict__ ef,
+                                                                 const double* __restrict__ rf,
                                                                  double* __restrict__ x, double* __restrict__ v) {
     __shared__ double shift[3];
     const int n3 = 3 * p.n_protein;
@@ -85,7 +87,8 @@ __global__ void __launch_bounds__(MD_K1_THREADS) md_kick1_kernel(MdParams p, con
             const MdCoef c = md_coef(p, m);
             double xi = 0.0, eta = 0.0;
             if (p.fr > 0.0) md_normals(p, step, comp, xi, eta);
-            const double f = (double)ef[comp];
+            double f = (double)ef[comp];
+            if (rf != nullptr) f += rf[comp];
             double vv = v[comp];
             vv = vv + (c.c1 * f / m - c.c2 * vv + c.c3 * xi - c.c4 * eta);
             const double x_old = x[comp];
@@ -127,10 +130,68 @@ __global__ void __launch_bounds__(MD_K1_THREADS) md_kick1_kernel(MdParams p, con
     }
 }
 
-// fragment atoms follow the protein: real atoms copy, cap hydrogens sit at P[acc] + unit(P[rem] - P[acc]) * blen
+// ---- Hookean restraints (ASE 3.22 ase/constraints.py Hookean, recalled; host checker oracle/hookean_ref.py) -----------
+// The reference's pre-equilibration tethers every protein atom to where it stood at the start of a stage
+// (src/AIMD/simulator.py:139-166, ASE type 'point', rt = 0) and --constraints adds a spring between every hydrogen and its
+// bonded partner (simulator.py:168-180, ASE type 'two atoms').  For one term, with d the vector from the atom to the
+// anchor (tether) or to the partner (spring) and L = |d|: if L > rt, F += k (L - rt) d / L and E += k (L - rt)^2 / 2 (at
+// L = 0 nothing is added).  ASE applies find_mic with the cell; here there is no minimum image: a tether moves far less
+// than half a box length and a bond is about 1 A, so the minimum image is the displacement itself.
+// Terms are a CSR over protein atoms built on the host: a spring appears once at each of its two atoms (the partner's
+// entry sees -d, i.e. the opposite force), a tether once.  One thread sums an atom's terms in CSR order, no atomics; the
+// energy of a spring is counted at its lower-indexed atom and reduced in a fixed order, so rf is bit-reproducible.
+// The output rf[3*n_protein + 1] (forces, then the energy) is the engine's own fp64 buffer: the caller's ef stays the
+// calculator output and the kicks add the two, as ASE's Atoms.get_forces() adds the constraint on top of the calculator.
+struct MdRestraints {
+    int n_protein;
+    const int* rowptr;      // [n_protein + 1]
+    const int* partner;     // per term: the other atom of a spring, or -1 for a tether
+    const double* k;        // per term, eV/A^2
+    const double* rt;       // per term, A
+    const double* p0;       // [3 * terms]: the anchor of a tether (unused for springs)
+    double* rf;             // [3 * n_protein + 1]
+};
+
+// evaluated by one CTA of blockDim.x threads (a multiple of 32, at most 1024)
+__device__ inline void md_restraint_cta(const MdRestraints& r, const double* __restrict__ x) {
+    __shared__ double red[32];
+    double e = 0.0;
+    for (int a = threadIdx.x; a < r.n_protein; a += blockDim.x) {
+        const double xa = x[3 * a], ya = x[3 * a + 1], za = x[3 * a + 2];
+        double fx = 0.0, fy = 0.0, fz = 0.0;
+        for (int t = r.rowptr[a]; t < r.rowptr[a + 1]; t++) {
+            const int j = r.partner[t];
+            double dx, dy, dz;
+            if (j < 0) { dx = r.p0[3 * t] - xa; dy = r.p0[3 * t + 1] - ya; dz = r.p0[3 * t + 2] - za; }
+            else       { dx = x[3 * j] - xa;    dy = x[3 * j + 1] - ya;    dz = x[3 * j + 2] - za; }
+            const double L = sqrt(dx * dx + dy * dy + dz * dz), rt = r.rt[t];
+            if (L > rt) {
+                const double mag = r.k[t] * (L - rt);
+                fx += dx / L * mag; fy += dy / L * mag; fz += dz / L * mag;
+                if (j < a) e += 0.5 * r.k[t] * ((L - rt) * (L - rt));    // tethers (j = -1) and each spring once
+            }
+        }
+        r.rf[3 * a] = fx; r.rf[3 * a + 1] = fy; r.rf[3 * a + 2] = fz;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) e += __shfl_xor_sync(0xffffffffu, e, o);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = e;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double t = 0.0;
+        for (int w = 0; w < (int)(blockDim.x >> 5); w++) t += red[w];
+        r.rf[3 * r.n_protein] = t;
+    }
+}
+
+// fragment atoms follow the protein: real atoms copy, cap hydrogens sit at P[acc] + unit(P[rem] - P[acc]) * blen.
+// With restraints the launch has one CTA more than the placement needs, and that last CTA evaluates them into rf at the
+// same protein coordinates: the restraints cost no launch of their own in the step (a grid of one CTA with n_atoms = 0
+// evaluates only the restraints).
 __global__ void md_place_kernel(int n_atoms, const int* __restrict__ real, const int* __restrict__ acc,
                                 const int* __restrict__ rem, const float* __restrict__ blen,
-                                const double* __restrict__ x, float* __restrict__ pos) {
+                                const double* __restrict__ x, float* __restrict__ pos, MdRestraints rs) {
+    if ((int)blockIdx.x == (n_atoms + (int)blockDim.x - 1) / (int)blockDim.x) { md_restraint_cta(rs, x); return; }
     const int a = blockIdx.x * blockDim.x + threadIdx.x;
     if (a >= n_atoms) return;
     const int r = real[a];
@@ -154,6 +215,7 @@ __global__ void md_place_kernel(int n_atoms, const int* __restrict__ real, const
 constexpr int MD_K2_THREADS = 1024;
 __global__ void __launch_bounds__(MD_K2_THREADS) md_kick2_kernel(MdParams p, long long* __restrict__ step_ctr,
                                                                  const double* __restrict__ mass, const float* __restrict__ ef,
+                                                                 const double* __restrict__ rf,
                                                                  double* __restrict__ v, double* __restrict__ epot_hist,
                                                                  long long hist_cap) {
     __shared__ double red[3][MD_K2_THREADS / 32];
@@ -165,8 +227,10 @@ __global__ void __launch_bounds__(MD_K2_THREADS) md_kick2_kernel(MdParams p, lon
         const MdCoef c = md_coef(p, m);
         double xi = 0.0, eta = 0.0;
         if (p.fr > 0.0) md_normals(p, step, comp, xi, eta);
+        double f = (double)ef[comp];
+        if (rf != nullptr) f += rf[comp];
         double vv = v[comp];
-        vv = vv + (c.c1 * (double)ef[comp] / m - c.c2 * vv + c.c3 * xi - c.c4 * eta);
+        vv = vv + (c.c1 * f / m - c.c2 * vv + c.c3 * xi - c.c4 * eta);
         v[comp] = vv;
     }
     if (p.fr > 0.0) {
@@ -199,7 +263,8 @@ __global__ void __launch_bounds__(MD_K2_THREADS) md_kick2_kernel(MdParams p, lon
         for (int comp = threadIdx.x; comp < n3; comp += MD_K2_THREADS) v[comp] -= com[comp % 3] / mtot;
     }
     if (threadIdx.x == 0) {
-        if (epot_hist != nullptr && hist_cap > 0) epot_hist[step % hist_cap] = (double)ef[n3];
+        // with restraints, the restrained potential energy (ASE get_potential_energy(apply_constraint=True))
+        if (epot_hist != nullptr && hist_cap > 0) epot_hist[step % hist_cap] = (double)ef[n3] + (rf != nullptr ? rf[n3] : 0.0);
         *step_ctr = step + 1;
     }
 }

@@ -40,6 +40,7 @@ EXPORTED_SYMBOLS = [
     "vb_forward_host", "vb_set_protein_map", "vb_forward_protein", "vb_get_edges", "vb_launches_per_forward",
     "vb_set_option", "vb_get_option", "vb_num_stages", "vb_stage_name", "vb_stage_kernel", "vb_debug_run", "vb_debug_read", "vb_profile_stages", "vb_tc_selftest", "vb_tc_selftest_rows",
     "vb_md_setup", "vb_md_set_normals", "vb_md_set_state", "vb_md_kick1", "vb_md_eval", "vb_md_kick2", "vb_md_run", "vb_md_get_state",
+    "vb_md_set_restraints",
     "vb_set_nonbonded", "vb_nonbonded",
     "vb_comm_init", "vb_comm_connect", "vb_comm_allreduce",
     "vb_set_caph", "vb_caph_relax",
@@ -110,6 +111,8 @@ def load_library(path: Optional[str] = None):
         getattr(lib, name).argtypes = [vp, vp]
     lib.vb_md_run.restype = C.c_int
     lib.vb_md_run.argtypes = [vp, i64, vp]
+    lib.vb_md_set_restraints.restype = C.c_int
+    lib.vb_md_set_restraints.argtypes = [vp, i64, vp, C.c_double, i64, vp, vp, vp]
     lib.vb_set_nonbonded.restype = C.c_int
     lib.vb_set_nonbonded.argtypes = [vp, i64, vp, vp, vp, vp, vp, i64, i64]
     lib.vb_nonbonded.restype = C.c_int
@@ -312,6 +315,24 @@ class Engine:
 
     def md_run(self, n_steps: int, stream_ptr: int = 0):
         self._check(self.lib.vb_md_run(self.h, int(n_steps), stream_ptr), "vb_md_run")
+
+    def md_set_restraints(self, tether_atoms=(), tether_k: float = 0.0, spring_ij=None, spring_k=(), spring_rt=()):
+        """Hookean restraints in eV/A^2 and A (vb_md_set_restraints): tethers anchored at the current device positions,
+        springs ``spring_ij [n,2]`` pulling beyond ``spring_rt``.  Replaces the previous set; no terms removes it."""
+        ta = np.ascontiguousarray(tether_atoms, dtype=np.int32).reshape(-1)
+        ij = np.ascontiguousarray(np.zeros((0, 2)) if spring_ij is None else spring_ij, dtype=np.int32).reshape(-1, 2)
+        sk = np.ascontiguousarray(spring_k, dtype=np.float64).reshape(-1)
+        sr = np.ascontiguousarray(spring_rt, dtype=np.float64).reshape(-1)
+        if not (len(ij) == len(sk) == len(sr)):
+            raise ValueError("spring_ij, spring_k and spring_rt must have one entry per spring")
+        self._check(self.lib.vb_md_set_restraints(self.h, ta.size, ta.ctypes.data if ta.size else None, float(tether_k),
+                                                  len(ij), ij.ctypes.data if len(ij) else None,
+                                                  sk.ctypes.data if len(sk) else None, sr.ctypes.data if len(sr) else None),
+                    "vb_md_set_restraints")
+
+    def md_restraint_forces(self) -> np.ndarray:
+        """The restraint buffer rf [3*n_protein + 1] (fp64 forces, then the energy) of the last evaluation; synchronises."""
+        return self.debug_read("RF", 0, (3 * self._md_n + 1,), np.float64)
 
     def md_get_state(self, n_hist: int = 0):
         """(x [n,3], v [n,3], step, epot history of the last n_hist steps) -- synchronises the device."""

@@ -19,6 +19,7 @@ import numpy as np
 from .engine import Engine
 from .fragment_data import FragmentData
 from .pdbfrag import FragmentRecipe, ProteinMap
+from .restraints import KCALMOL_EV, PREEQ_SCHEDULE
 
 FS = 0.09822694788464063        # 1 fs in ASE time units
 KB = 8.617330337217213e-05      # eV / K
@@ -239,3 +240,53 @@ class DeviceLangevin:
 
     def temperature(self):
         return 2.0 * self.kinetic_energy() / (3 * self.n) / KB
+
+    # ---- restraints and the reference's run protocol (simulator.py:139-180) ----
+    def set_restraints(self, tether_atoms=None, tether_k_kcal=0.0, springs=None):
+        """Hookean restraints inside the device step, replacing any set before: ``tether_atoms`` tied to where they stand
+        now with ``tether_k_kcal`` kcal/mol/A^2, and ``springs = (ij [n,2], k [n] eV/A^2, rt [n] A)`` (e.g.
+        :func:`ai2bmd_b200.restraints.hydrogen_bond_springs`).  No argument removes them.  Every rank of a sharded run
+        makes the same call."""
+        ij, k, rt = springs if springs is not None else (None, (), ())
+        self.engine.md_set_restraints(() if tether_atoms is None else tether_atoms, tether_k_kcal * KCALMOL_EV, ij, k, rt)
+
+    def run_observed(self, n_steps: int, record_per_steps=None, observer=None):
+        """``run(n_steps)`` in blocks that end at every step number divisible by ``record_per_steps``; there, like the
+        reference's ``MDObserver.printenergy`` (utils.py:143-159), the temperature is checked -- above 1.5 T0 raises
+        :class:`TemperatureRunawayError` -- and ``observer(step, x, v, epot, ekin)`` is called with the restrained
+        potential energy of that step."""
+        if not record_per_steps:
+            self.run(n_steps)
+            return
+        _, _, step, _ = self.state()
+        end = step + n_steps
+        while step < end:
+            nxt = min(end, (step // record_per_steps + 1) * record_per_steps)
+            self.run(nxt - step)
+            step = nxt
+            if step % record_per_steps:
+                continue
+            x, v, _, hist = self.state(n_hist=1)
+            ekin = 0.5 * float((self.masses[:, None] * v * v).sum())
+            temp = 2.0 * ekin / (3 * self.n) / KB
+            if temp > 1.5 * self.kT / KB:
+                raise TemperatureRunawayError(f"temperature runaway at step {step}: {temp:.1f} K")
+            if observer is not None:
+                observer(step, x, v, float(hist[0]), ekin)
+
+    def preequilibrate(self, steps_per_stage: int, schedule=PREEQ_SCHEDULE, atoms=None, record_per_steps=None, observer=None):
+        """The reference's pre-equilibration: for each force constant of ``schedule`` (kcal/mol/A^2, the reference's
+        :data:`ai2bmd_b200.restraints.PREEQ_SCHEDULE`) tether ``atoms`` (default: every protein atom) to where they stand
+        at the start of the stage, run ``steps_per_stage`` steps (``run_observed``), and remove the restraints.  The
+        step counter, and with it the random stream, runs on through the stages."""
+        atoms = np.arange(self.n) if atoms is None else atoms
+        for k in schedule:
+            self.set_restraints(tether_atoms=atoms, tether_k_kcal=k)
+            try:
+                self.run_observed(steps_per_stage, record_per_steps, observer)
+            finally:
+                self.set_restraints()
+
+
+class TemperatureRunawayError(RuntimeError):
+    """The temperature left 1.5 x the thermostat's target (the reference's guard, ``src/utils/utils.py:153-155``)."""

@@ -109,6 +109,20 @@ int vb_md_set_state(vb_handle* h, const double* x_host, const double* v_host, in
 int vb_md_kick1(vb_handle* h, void* stream);
 int vb_md_eval(vb_handle* h, void* stream);
 int vb_md_kick2(vb_handle* h, void* stream);
+/* Hookean restraints on top of the forces of ef_prot_dev (ASE 3.22 Hookean, the kicks use ef + rf; the energy history
+ * records ASE's restrained potential energy ef[3n] + rf[3n]).  Units eV/Angstrom^2 and Angstrom.
+ *   tethers: atom tether_atom[t] to the point where it stands NOW (the device positions at this call), spring tether_k,
+ *            rt = 0 -- the reference's pre-equilibration stage (src/AIMD/simulator.py:139-166, re-anchored per stage);
+ *   springs: atoms spring_ij[s][0..1], spring_k[s], spring_rt[s], pulling only when the pair is farther apart than rt --
+ *            the hydrogen bond constraints of --constraints (simulator.py:168-180, pairs from
+ *            PDBAnalyzer.find_bonded_atoms, src/utils/utils.py:201-221).
+ * Host arrays, copied; replaces the whole previous set; (0, ..., 0, ...) removes all restraints and the step is the
+ * unrestrained one again.  Synchronises, then evaluates rf at the current positions so the next kick1 sees the new set
+ * (vb_md_eval re-evaluates it, e.g. after vb_md_set_state).  VB_ERR_ARG: atom out of range, an atom tethered twice, a
+ * spring with i == j, negative or non-finite k or rt.  Requires vb_md_setup. */
+int vb_md_set_restraints(vb_handle* h, int64_t n_tether, const int32_t* tether_atom, double tether_k,
+                         int64_t n_spring, const int32_t* spring_ij /* [n][2] */, const double* spring_k,
+                         const double* spring_rt);
 /* Single GPU: n_steps whole steps, each one replay of a captured CUDA graph, no host synchronisation. */
 int vb_md_run(vb_handle* h, int64_t n_steps, void* stream);
 /* Synchronises; any of x_host / v_host / step_out may be NULL.  epot_hist_host[n_hist] receives the potential
@@ -213,7 +227,8 @@ int vb_tc_selftest(int device, const float* a_host, const float* img_host, float
 int vb_tc_selftest_rows(int device, int rows, const float* a_host, const float* img_host, float* d_host, int reps, float* ms_out);
 /* Copy an internal buffer to the host.  name: "X","V","F","VN","QKV","V123","VDOT","TU","O" (per layer),
  * "XA","VA","GX","GVEC","GF","GXA","GQKV","GVNMSG","GTU","geom","rbf","eacc","grbf","esrc","edst","rowptr",
- * "eatom","energy","forces".  Returns the number of bytes copied (<= cap_bytes) or a negative status. */
+ * "eatom","energy","forces", and "RF" (fp64 restraint forces then energy [3*n_protein + 1], while restraints are set).
+ * Returns the number of bytes copied (<= cap_bytes) or a negative status. */
 int64_t vb_debug_read(vb_handle* h, const char* name, int layer, void* host_dst, int64_t cap_bytes);
 
 #ifdef __cplusplus
