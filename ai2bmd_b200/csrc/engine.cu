@@ -809,6 +809,22 @@ int run_cached(vb_handle* h, cudaStream_t st, int kind, const StepIO& io, F&& en
     return VB_OK;
 }
 
+// Flag waits of the all-reduce that ran past their deadline so far (k_comm.cuh counters[3]), read on the handle's own
+// stream without waiting for the caller's.  After one the ranks' windows are out of step for good, so every later
+// all-reduce and MD call fails instead of running on stale sums.
+int comm_check(vb_handle* h, const char* who) {
+    if (!h->comm_ready) return VB_OK;
+    unsigned int n = 0;
+    CUDA_TRY(h, cudaSetDevice(h->device));
+    CUDA_TRY(h, cudaMemcpyAsync(&n, h->comm.counters + 3, sizeof(n), cudaMemcpyDeviceToHost, h->own_stream));
+    CUDA_TRY(h, cudaStreamSynchronize(h->own_stream));
+    if (n) {
+        h->set_error("%s: %u all-reduce flag wait(s) timed out: a peer never signalled; re-run vb_comm_init / vb_comm_connect", who, n);
+        return VB_ERR_STATE;
+    }
+    return VB_OK;
+}
+
 // all-reduce of buf[n] over the connected ranks (k_comm.cuh), one launch on st
 int enqueue_allreduce(vb_handle* h, cudaStream_t st, float* buf, long long n) {
     if (n > h->comm.max_floats) { h->set_error("all-reduce of %lld floats exceeds the window (%lld)", n, h->comm.max_floats); return VB_ERR_ARG; }
@@ -1197,9 +1213,11 @@ void md_kick2_enqueue(vb_handle* h, cudaStream_t st) {
     md_kick2_kernel<<<1, MD_K2_THREADS, 0, st>>>(h->md, h->d_step, h->d_mmass, h->md_ef, h->rs.rf, h->d_mv, h->d_ehist,
                                                  h->ehist_cap);
 }
-int md_check(vb_handle* h, const char* who) {
+// `stepping`: the call enqueues or changes MD work, which a broken all-reduce would corrupt; reading the state stays
+// allowed, so a failed run can still be inspected
+int md_check(vb_handle* h, const char* who, bool stepping = true) {
     if (!h->md_ready) { h->set_error("%s: call vb_md_setup first", who); return VB_ERR_STATE; }
-    return VB_OK;
+    return stepping ? comm_check(h, who) : VB_OK;
 }
 }  // namespace
 
@@ -1410,7 +1428,7 @@ int vb_md_run(vb_handle* h, int64_t n_steps, void* stream) {
 int vb_md_get_state(vb_handle* h, double* x_host, double* v_host, int64_t* step_out, double* epot_hist_host, int64_t n_hist) {
     if (!h) return VB_ERR_ARG;
     std::lock_guard<std::mutex> lk(h->mu);
-    if (int rc = md_check(h, "vb_md_get_state")) return rc;
+    if (int rc = md_check(h, "vb_md_get_state", false)) return rc;
     if (n_hist < 0 || n_hist > h->ehist_cap || (n_hist > 0 && !epot_hist_host)) { h->set_error("vb_md_get_state: bad history request"); return VB_ERR_ARG; }
     CUDA_TRY(h, cudaSetDevice(h->device));
     CUDA_TRY(h, cudaDeviceSynchronize());
@@ -1669,7 +1687,7 @@ int vb_comm_allreduce(vb_handle* h, float* buf_dev, int64_t n, void* stream) {
     std::lock_guard<std::mutex> lk(h->mu);
     if (!h->comm_ready) { h->set_error("vb_comm_allreduce: call vb_comm_init / vb_comm_connect first"); return VB_ERR_STATE; }
     if (!buf_dev || n <= 0) { h->set_error("vb_comm_allreduce: bad arguments"); return VB_ERR_ARG; }
-    CUDA_TRY(h, cudaSetDevice(h->device));
+    if (int rc = comm_check(h, "vb_comm_allreduce")) return rc;
     return enqueue_allreduce(h, (cudaStream_t)stream, buf_dev, n);
 }
 
@@ -1752,6 +1770,14 @@ int64_t vb_get_option(const vb_handle* h, const char* key) {
         return v;
     }
     if (k == "comm_ready") return h->comm_ready ? 1 : 0;
+    if (k == "comm_timeouts" || k == "comm_seq") {
+        // all-reduce flag waits that ran past their deadline / all-reduces completed since vb_comm_init (synchronises)
+        unsigned int v = 0;
+        if (!h->comm_ready || cudaSetDevice(h->device) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess ||
+            cudaMemcpy(&v, h->comm.counters + (k == "comm_seq" ? 2 : 3), sizeof(v), cudaMemcpyDeviceToHost) != cudaSuccess)
+            return VB_ERR_STATE;
+        return v;
+    }
     if (k == "edge_overflow") {
         int flag = 0;
         if (h->d_flags && cudaMemcpy(&flag, h->d_flags, sizeof(int), cudaMemcpyDeviceToHost) != cudaSuccess) return VB_ERR_CUDA;
@@ -1903,6 +1929,7 @@ int64_t vb_debug_read(vb_handle* h, const char* name, int layer, void* host_dst,
     else BUF("eatom", ws.eatom, N, 4)
     else BUF("energy", h->d_energy, G, 4)
     else BUF("forces", h->d_forces, N * 3, 4)
+    else BUF("pos", h->d_pos, N * 3, 4)
     else if (k == "RF" && h->rs_ready) { src = h->rs.rf; bytes = (3 * (size_t)h->n_protein + 1) * 8; }
 #undef BUF
     if (!src) { h->set_error("vb_debug_read: unknown buffer %s[%d]", name, layer); return VB_ERR_ARG; }

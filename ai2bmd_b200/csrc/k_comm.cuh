@@ -16,6 +16,14 @@
 // Two parities suffice: a rank can run at most one step ahead of the slowest one, because finishing step s+1 needs the
 // slowest rank's push for s+1, which that rank issues only after it has summed step s.
 // All CTAs of the kernel must be co-resident (they wait for each other): the grid is capped at COMM_MAX_CTAS.
+// The wait has a deadline: a flag that does not arrive within COMM_WAIT_NS (a peer that died, a broken protocol) is
+// counted in counters[3] and the kernel finishes with whatever the slots hold, so the stream never hangs.  Once the count
+// is nonzero the ranks are out of step for good, and every later launch of the kernel (the rest of an md_run's replays)
+// skips the wait, so one failure costs one deadline, not one per enqueued step.  The host reports the count
+// (vb_get_option "comm_timeouts") and fails every later all-reduce and MD call of the handle but vb_md_get_state.
+// The deadline bounds the skew between ranks, host side included: one rank stalled for more than 10 s between steps
+// (I/O, a checkpoint) while its peers already wait in the next all-reduce also trips it.
+// The sum starts at +0.0f, so an element that is -0.0 on every rank comes out as +0.0 (also with world = 1).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -25,14 +33,22 @@ namespace vb {
 constexpr int COMM_MAX_WORLD = 16;
 constexpr int COMM_THREADS = 512;
 constexpr int COMM_MAX_CTAS = 32;
+constexpr unsigned long long COMM_WAIT_NS = 10ull * 1000 * 1000 * 1000;
 
 struct CommParams {
     int rank, world;
     long long max_floats;                 // capacity of one slot
     float* slots[COMM_MAX_WORLD];         // slots[r]: base of rank r's slot array [2][world][max_floats] (peer-mapped)
     int* flags[COMM_MAX_WORLD];           // flags[r]: base of rank r's flag array [2][world]
-    unsigned int* counters;               // local: [0] CTAs done pushing, [1] CTAs done summing, [2] sequence number
+    unsigned int* counters;               // local: [0] CTAs done pushing, [1] CTAs done summing, [2] sequence number,
+                                          //        [3] flag waits that ran past COMM_WAIT_NS
 };
+
+__device__ __forceinline__ unsigned long long globaltimer_ns() {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
 
 __device__ __forceinline__ void st_release_sys(int* p, int v) {
     asm volatile("st.release.sys.global.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
@@ -49,10 +65,13 @@ __device__ __forceinline__ float ld_relaxed_sys(const float* p) {
 }
 
 __global__ void __launch_bounds__(COMM_THREADS) comm_allreduce_kernel(CommParams c, float* __restrict__ buf, long long n) {
-    __shared__ unsigned int s_seq;
+    __shared__ unsigned int s_seq, s_broken;
     __shared__ int s_last;
     const int rank = c.rank, world = c.world;
-    if (threadIdx.x == 0) s_seq = *reinterpret_cast<volatile unsigned int*>(c.counters + 2);
+    if (threadIdx.x == 0) {
+        s_seq = *reinterpret_cast<volatile unsigned int*>(c.counters + 2);
+        s_broken = *reinterpret_cast<volatile unsigned int*>(c.counters + 3);
+    }
     __syncthreads();
     const unsigned int seq = s_seq + 1u;                    // this step's sequence number (starts at 1)
     const int par = (int)(seq & 1u);
@@ -72,9 +91,13 @@ __global__ void __launch_bounds__(COMM_THREADS) comm_allreduce_kernel(CommParams
         if ((int)threadIdx.x < world) st_release_sys(c.flags[threadIdx.x] + par * world + rank, (int)seq);
     }
     // 3. wait for every rank's flag of this parity in my own memory
-    if ((int)threadIdx.x < world) {
+    if ((int)threadIdx.x < world && s_broken == 0u) {
         const int* f = c.flags[rank] + par * world + threadIdx.x;
-        while (ld_acquire_sys(f) != (int)seq) { __nanosleep(64); }
+        const unsigned long long t0 = globaltimer_ns();
+        while (ld_acquire_sys(f) != (int)seq) {
+            if (globaltimer_ns() - t0 > COMM_WAIT_NS) { atomicAdd(c.counters + 3, 1u); break; }
+            __nanosleep(64);
+        }
     }
     __syncthreads();
     // 4. fixed-order sum of the slots (same order on every rank)

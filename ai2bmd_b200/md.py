@@ -101,12 +101,17 @@ class Langevin:
     def temperature(self):
         return 2.0 * self.kinetic_energy() / (3 * len(self.x)) / KB
 
-    def step(self):
+    def normals(self):
+        """(xi, eta) of the current step: from ``normal_source``, else two draws of the numpy generator (0 at friction 0)."""
         if self.fr > 0 and self.normal_source is not None:
-            xi, eta = self.normal_source(self.nsteps)
-        else:
-            xi = self.rng.standard_normal(self.x.shape) if self.fr > 0 else 0.0
-            eta = self.rng.standard_normal(self.x.shape) if self.fr > 0 else 0.0
+            return self.normal_source(self.nsteps)
+        xi = self.rng.standard_normal(self.x.shape) if self.fr > 0 else 0.0
+        eta = self.rng.standard_normal(self.x.shape) if self.fr > 0 else 0.0
+        return xi, eta
+
+    def first_half(self, xi, eta):
+        """Half-kick with the current forces, drift, centre of mass put back, velocities from the positions
+        (the device's ``md_kick1_kernel``)."""
         self.v = self.v + (self.c1 * self.f / self.m - self.c2 * self.v + self.c3 * xi - self.c4 * eta)
         x_old = self.x
         self.x = self.x + self.dt * self.v + self.c5 * eta
@@ -114,11 +119,20 @@ class Langevin:
             msum = self.m.sum()
             self.x = self.x + ((self.m * x_old).sum(0) / msum - (self.m * self.x).sum(0) / msum)
         self.v = (self.x - x_old - self.c5 * eta) / self.dt
-        self.energy, self.f = self.force_fn(self.x)
+
+    def second_half(self, xi, eta):
+        """Half-kick with the forces of the new positions, centre-of-mass velocity removed, step counter advanced
+        (the device's ``md_kick2_kernel``)."""
         self.v = self.v + (self.c1 * self.f / self.m - self.c2 * self.v + self.c3 * xi - self.c4 * eta)
         if self.fr > 0:
             self.v -= (self.v * self.m).sum(0) / self.m.sum()
         self.nsteps += 1
+
+    def step(self):
+        xi, eta = self.normals()
+        self.first_half(xi, eta)
+        self.energy, self.f = self.force_fn(self.x)
+        self.second_half(xi, eta)
         return self.energy
 
     def run(self, n_steps):

@@ -203,8 +203,11 @@ int vb_launches_per_forward(const vb_handle* h);
  * different row (default 1: the CTAs of a wave otherwise ask the same L2 slices for the same rows at the same time),
  * "embed_batch" -1/0..3 batch variants of the embedding kernels, "comm_auto" 0/1.  vb_get_option also answers "edge_overflow" (1 after a step exceeded a trimmed max_edges),
  * "tile_rows" (planned edges per tile), "gxa_parts" (1: every tensor-core node CTA runs all column chunks of its row tile; 3: one
- * chunk per CTA, dE/dxa arrives as three partials), "comm_ready", "caph_ready" and "caph_evals" (energy evaluations of the last
- * hydrogen refinement). */
+ * chunk per CTA, dE/dxa arrives as three partials), "comm_ready", "comm_timeouts" (all-reduce flag waits that gave up after
+ * their 10 s deadline; once nonzero, vb_comm_allreduce and every vb_md_* call but vb_md_setup and vb_md_get_state fail
+ * with VB_ERR_STATE), "comm_seq" (all-reduces completed since vb_comm_init: the window parity of the next one is its
+ * parity plus one),
+ * "caph_ready" and "caph_evals" (energy evaluations of the last hydrogen refinement). */
 int vb_set_option(vb_handle* h, const char* key, int64_t value);
 int64_t vb_get_option(const vb_handle* h, const char* key);   /* resolved value (after vb_set_topology) */
 
@@ -227,7 +230,8 @@ int vb_tc_selftest(int device, const float* a_host, const float* img_host, float
 int vb_tc_selftest_rows(int device, int rows, const float* a_host, const float* img_host, float* d_host, int reps, float* ms_out);
 /* Copy an internal buffer to the host.  name: "X","V","F","VN","QKV","V123","VDOT","TU","O" (per layer),
  * "XA","VA","GX","GVEC","GF","GXA","GQKV","GVNMSG","GTU","geom","rbf","eacc","grbf","esrc","edst","rowptr",
- * "eatom","energy","forces", and "RF" (fp64 restraint forces then energy [3*n_protein + 1], while restraints are set).
+ * "eatom","energy","forces","pos" (the packed fragment positions [N*3] the MD placement and hydrogen refinement write),
+ * and "RF" (fp64 restraint forces then energy [3*n_protein + 1], while restraints are set).
  * Returns the number of bytes copied (<= cap_bytes) or a negative status. */
 int64_t vb_debug_read(vb_handle* h, const char* name, int layer, void* host_dst, int64_t cap_bytes);
 

@@ -95,3 +95,16 @@ def relax(f, max_iter=10, lr=0.1, tolerance_grad=0.1, tolerance_change=0.01):
     x = f["pos"].copy()
     evals = _load().caph_relax(C.byref(_struct(f)), x.ctypes.data, int(max_iter), lr, tolerance_grad, tolerance_change)
     return x, int(evals)
+
+
+def relax_problem(pr, pos, **lbfgs):
+    """``relax`` on the flat arrays of an :class:`ai2bmd_b200.caph.CapHProblem` at packed positions ``pos``, with the
+    ACE-NME mirror copies re-applied afterwards as the device kernel does: (positions, energy evaluations)."""
+    flat = {"pos": np.ascontiguousarray(pos, dtype=np.float32).copy(), "h_idx": pr.h_idx.astype(np.int64)}
+    for key in ("bond_ij", "angle_ijk", "dih_ijkl", "pair_ij"):
+        flat[key] = np.ascontiguousarray(getattr(pr, key), dtype=np.int64)
+    for key in ("bond_k", "bond_r0", "angle_k", "angle_t0", "dih_k", "dih_n", "dih_p", "pair_a", "pair_b", "pair_qq"):
+        flat[key] = np.ascontiguousarray(getattr(pr, key), dtype=np.float32)
+    x, evals = relax(flat, **lbfgs)
+    x[pr.mirror_dst] = x[pr.mirror_src]
+    return x, evals

@@ -85,13 +85,13 @@ KERNELS = {
     "tc_selftest_kernel<32>": "test_tc_selftest_gpu.py",
     "tc_selftest_kernel<64>": "test_tc_selftest_gpu.py",
     "tc_selftest_kernel<TC_TE>": "test_tc_selftest_gpu.py",
-    "md_kick1_kernel": "test_md_gpu.py",
-    "md_place_kernel": "test_md_gpu.py",
-    "md_kick2_kernel": "test_md_gpu.py",
-    "caph_relax_kernel": "test_caph_gpu.py",
-    "nonbonded_kernel": "test_nonbonded.py",
-    "nonbonded_energy_kernel": "test_nonbonded.py",
-    "comm_allreduce_kernel": "test_multigpu.py",          # runs where the machine has two or more GPUs
+    "md_kick1_kernel": "test_md_kernels_gpu.py",
+    "md_place_kernel": "test_md_kernels_gpu.py",
+    "md_kick2_kernel": "test_md_kernels_gpu.py",
+    "caph_relax_kernel": "test_md_kernels_gpu.py",
+    "nonbonded_kernel": "test_md_kernels_gpu.py",
+    "nonbonded_energy_kernel": "test_md_kernels_gpu.py",
+    "comm_allreduce_kernel": "test_md_kernels_gpu.py",    # world = 1 here; test_multigpu.py runs world > 1
 }
 _NT = {"NT_OPROJ": "0", "NT_PROJ": "1", "NT_BWDA": "2", "NT_BWDB": "3"}
 
