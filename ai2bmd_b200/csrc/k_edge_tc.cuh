@@ -84,6 +84,8 @@ __device__ __forceinline__ void tc_issue(TcShared& sh, int k) {
 //     that a phase wrote into the tile); a tile of <= 64 rows has three, `tile`, `abuf` and `tc_aux` (rows 64.. of
 //     `tile`), so every operand is read where it was written, a phase that produces two row sets writes both at once,
 //     and nothing is copied or gathered twice;
+//   * the forward of a tile of <= 64 rows is warp-specialised: warpgroups 0 and 2 run the products, 1 and 3 the
+//     gathers and SIMT phases (see tc2_is_mma_warp);
 //   * there is no producer warp: the ring is refilled by whichever compute warp releases a stage last (tc2_release),
 //     so the CTA is 512 threads with 128 registers each;
 //   * a tile holds ROWS = 32 / 64 / 96 / 128 edges (template parameter): compute warp w owns rows
@@ -105,10 +107,23 @@ struct EdgeTcArgs {
     int tile_rows;              // edges per tile, <= the kernel's ROWS
     unsigned long long* tl;     // optional timeline (SM clock stamps of CTA 0, first tile); nullptr = off
 };
-constexpr int TC_TL_SLOTS = 64;  // [0,32): compute thread 0 phase stamps
+constexpr int TC_TL_SLOTS = 64;  // [0,32): compute thread 0 phase stamps, [32,64): thread 128 (a gather warp of a warp-specialised tile)
 #define TC_TL(k) do { if (a.tl != nullptr && blockIdx.x == 0 && it == 0 && threadIdx.x == 0) a.tl[k] = (unsigned long long)clock64(); } while (0)
 
 __device__ __forceinline__ void csync() { asm volatile("bar.sync 1, %0;" ::"n"(TC2_CTHREADS) : "memory"); }
+
+// Warp-specialised tiles of <= 64 rows.  Such a tile has product rows for warpgroups 0 and 2 only (tc2_mma: rows
+// 64 * (q & 1)), so those two warpgroups (the MMA warps) run the tile's products back to back and the other two (the
+// gather warps, 256 threads) run the SIMT phases: each phase issues its loads and computes what needs no product
+// result before it waits for the product.  A hand-off between the roles is a named barrier of all 512 threads: the
+// producing role arrives (bar.arrive, no wait), the consuming role waits (bar.sync).  Every id is used once per tile,
+// and the tile ends with a CTA barrier, so an arrival can never complete a later phase of the same id.
+constexpr int TC2_WS_THREADS = TC2_CTHREADS / 2;    // threads per role
+__device__ __forceinline__ bool tc2_is_mma_warp(int warp) { return ((warp >> 2) & 1) == 0; }
+// named barrier ids: 0 = __syncthreads, 1 = csync, 2 = the gather warps among themselves, 3..15 = a kernel's hand-offs
+__device__ __forceinline__ void gather_sync() { asm volatile("bar.sync 2, %0;" ::"n"(TC2_WS_THREADS) : "memory"); }
+__device__ __forceinline__ void handoff_arrive(int id) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "n"(TC2_CTHREADS) : "memory"); }
+__device__ __forceinline__ void handoff_wait(int id) { asm volatile("bar.sync %0, %1;" ::"r"(id), "n"(TC2_CTHREADS) : "memory"); }
 
 // position of a thread in the ring's slab sequence (every thread walks the same sequence), for a tile capacity of ROWS
 template <int ROWS>
@@ -134,13 +149,14 @@ __device__ __forceinline__ void tc2_setup(TcShared& sh, const TcRing<ROWS>&, con
 }
 
 // a warp is done with slab k (every MMA that read it has retired): the warp that releases it last refills the stage
-// with slab k + NS.  No warp waits for a refill, so none can wait on one that only it would issue.
-template <int NS>
+// with slab k + NS.  No warp waits for a refill, so none can wait on one that only it would issue.  NW: the warps that
+// walk the ring (all 16, or the 8 MMA warps of a warp-specialised tile)
+template <int NS, int NW>
 __device__ __forceinline__ void tc2_release(TcShared& sh, int k, int lane) {
     __syncwarp();
     if (lane == 0) {
         const uint32_t before = tc::atom_add_acq_rel(&sh.released[k % NS], 1u);
-        if (before % TC2_CWARPS == TC2_CWARPS - 1) tc_issue<NS>(sh, k + NS);
+        if (before % NW == NW - 1) tc_issue<NS>(sh, k + NS);
     }
 }
 
@@ -167,14 +183,16 @@ __device__ __forceinline__ TcRow* tc_aux(TcShared& sh) { return sh.tile + 64; }
 // fragments are split into tf32 hi / lo as they are loaded (before the slab's weights are waited for), one commit group
 // of 12 MMAs runs, and the stage is released as soon as that group retires: a product streams 128 KB of weights through
 // the ring, and an early release is worth more than MMAs kept in flight across slabs.  On return `acc` holds this
-// thread's part of the product (layout: tc_common.cuh).
-template <int ROWS>
+// thread's part of the product (layout: tc_common.cuh).  WS: a warp-specialised tile, where only the MMA warps call this
+// (after a hand-off that publishes A) and they alone release the ring stages.
+template <int ROWS, bool WS = false>
 __device__ __forceinline__ void tc2_mma(TcShared& sh, TcRing<ROWS>& ring, const TcRow* A, float (&acc)[32], int accumulate,
                                         int warp, int lane, int nvalid) {
     constexpr int NS = TcRing<ROWS>::NS;
-    csync();                                                   // the A operand is complete
+    static_assert(!WS || ROWS <= 64, "only tiles of <= 64 rows leave two warpgroups without product rows");
+    if constexpr (!WS) csync();                                // the A operand is complete
     const int q = warp >> 2, m0 = (q & 1) * 64 + (warp & 3) * 16, g = lane >> 2, t = lane & 3;
-    const bool active = (q & 1) * 64 < nvalid;                 // warpgroup-uniform
+    const bool active = WS || (q & 1) * 64 < nvalid;           // warpgroup-uniform
     if (!accumulate) {
 #pragma unroll
         for (int i = 0; i < 32; i++) acc[i] = 0.f;
@@ -216,7 +234,7 @@ __device__ __forceinline__ void tc2_mma(TcShared& sh, TcRing<ROWS>& ring, const 
         } else {
             tc::mbar_wait(&sh.b_full[stage], (uint32_t)(k / NS) & 1u);
         }
-        tc2_release<NS>(sh, k, lane);
+        tc2_release<NS, WS ? TC2_CWARPS / 2 : TC2_CWARPS>(sh, k, lane);
     }
     ring.next += TC_SLABS;
 }
@@ -269,6 +287,99 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) tc_selftest_kernel(const float
 // forward (math and reference lines: see edge_fwd_kernel in k_edge.cuh)
 // job order: dk, dv, [f], s1, s2
 // ---------------------------------------------------------------------------------------------
+// Per-target sums of the forward over a tile's targets.  Thread (channel c, group grp of ngrp) sums targets
+// i_first + grp, + ngrp, ..; a target whose edges all lie in the tile is stored, a target cut by a tile boundary is added
+// atomically.
+// xa_i = sum_e m_e
+__device__ __forceinline__ void tc_fwd_xa(const TcShared& sh, const Workspace& ws, const TcRow* mb, int e0, int nvalid,
+                                          int c, int grp, int ngrp) {
+    const int i_first = sh.meta.dst[0], i_last = sh.meta.dst[nvalid - 1];
+    for (int i = i_first + grp; i <= i_last; i += ngrp) {
+        const int q0 = ws.rowptr[i], q1 = ws.rowptr[i + 1];
+        const int lo = max(q0, e0) - e0, hi = min(q1, e0 + nvalid) - e0;
+        float xa = 0.f;
+        for (int r = lo; r < hi; r++) xa += mb[r][c];
+        if (q0 >= e0 && q1 <= e0 + nvalid) ws.XA[(size_t)i * D + c] = xa;
+        else atomicAdd(ws.XA + (size_t)i * D + c, xa);
+    }
+}
+// s1 (D1): va_i = sum_e vn_j * silu(s1 + bs); the sums of cut targets (at most two per thread) stay in `bnd` for tc_fwd_s2
+__device__ __forceinline__ void tc_fwd_s1(const TcShared& sh, const Workspace& ws, const LayerW& lw, const float* __restrict__ VN,
+                                          float* __restrict__ SP, const TcRow* s1b, int e0, int nvalid, int c, int grp, int ngrp,
+                                          float (&bnd)[2][3]) {
+    const float b = __ldg(lw.bs + c);
+    const int i_first = sh.meta.dst[0], i_last = sh.meta.dst[nvalid - 1];
+    int nb = 0;
+    for (int i = i_first + grp; i <= i_last; i += ngrp) {
+        const int q0 = ws.rowptr[i], q1 = ws.rowptr[i + 1];
+        const int lo = max(q0, e0) - e0, hi = min(q1, e0 + nvalid) - e0;
+        float v0 = 0.f, v1 = 0.f, v2 = 0.f;
+        int r = lo;
+        for (; r + 4 <= hi; r += 4) {              // 12 independent gathers in flight
+            float g[4][3], s1[4];
+#pragma unroll
+            for (int u = 0; u < 4; u++) {
+                const size_t j3 = (size_t)sh.meta.src[r + u] * 3;
+                g[u][0] = __ldg(VN + (j3 + 0) * D + c); g[u][1] = __ldg(VN + (j3 + 1) * D + c); g[u][2] = __ldg(VN + (j3 + 2) * D + c);
+                const float sp = s1b[r + u][c] + b;
+                SP[(size_t)(e0 + r + u) * 2 * D + c] = sp;
+                s1[u] = silu_(sp);
+            }
+#pragma unroll
+            for (int u = 0; u < 4; u++) { v0 += g[u][0] * s1[u]; v1 += g[u][1] * s1[u]; v2 += g[u][2] * s1[u]; }
+        }
+        for (; r < hi; r++) {
+            const size_t j3 = (size_t)sh.meta.src[r] * 3;
+            const float sp = s1b[r][c] + b;
+            SP[(size_t)(e0 + r) * 2 * D + c] = sp;
+            const float s1 = silu_(sp);
+            v0 += __ldg(VN + (j3 + 0) * D + c) * s1;
+            v1 += __ldg(VN + (j3 + 1) * D + c) * s1;
+            v2 += __ldg(VN + (j3 + 2) * D + c) * s1;
+        }
+        if (q0 >= e0 && q1 <= e0 + nvalid) {
+            ws.VA[((size_t)i * 3 + 0) * D + c] = v0;
+            ws.VA[((size_t)i * 3 + 1) * D + c] = v1;
+            ws.VA[((size_t)i * 3 + 2) * D + c] = v2;
+        } else if (nb < 2) {
+            bnd[nb][0] = v0; bnd[nb][1] = v1; bnd[nb][2] = v2;
+            nb++;
+        }
+    }
+}
+// s2 (D0): va_i += sum_e silu(s2 + bs) * d (the same threads and targets as tc_fwd_s1)
+__device__ __forceinline__ void tc_fwd_s2(const TcShared& sh, const Workspace& ws, const LayerW& lw, float* __restrict__ SP,
+                                          const TcRow* s2b, int e0, int nvalid, int c, int grp, int ngrp, const float (&bnd)[2][3]) {
+    const float b = __ldg(lw.bs + D + c);
+    const int i_first = sh.meta.dst[0], i_last = sh.meta.dst[nvalid - 1];
+    int nb = 0;
+    for (int i = i_first + grp; i <= i_last; i += ngrp) {
+        const int q0 = ws.rowptr[i], q1 = ws.rowptr[i + 1];
+        const int lo = max(q0, e0) - e0, hi = min(q1, e0 + nvalid) - e0;
+        float v0 = 0.f, v1 = 0.f, v2 = 0.f;
+        for (int r = lo; r < hi; r++) {
+            const float4 de = sh.meta.d[r];
+            const float sp = s2b[r][c] + b;
+            SP[(size_t)(e0 + r) * 2 * D + D + c] = sp;
+            const float s2 = silu_(sp);
+            v0 += s2 * de.x; v1 += s2 * de.y; v2 += s2 * de.z;
+        }
+        if (q0 >= e0 && q1 <= e0 + nvalid) {
+            ws.VA[((size_t)i * 3 + 0) * D + c] += v0;
+            ws.VA[((size_t)i * 3 + 1) * D + c] += v1;
+            ws.VA[((size_t)i * 3 + 2) * D + c] += v2;
+        } else if (nb < 2) {
+            atomicAdd(ws.VA + ((size_t)i * 3 + 0) * D + c, bnd[nb][0] + v0);
+            atomicAdd(ws.VA + ((size_t)i * 3 + 1) * D + c, bnd[nb][1] + v1);
+            atomicAdd(ws.VA + ((size_t)i * 3 + 2) * D + c, bnd[nb][2] + v2);
+            nb++;
+        }
+    }
+}
+
+// gather-warp stamps of the timeline (thread 128 = lane 0 of warp 4, the first gather warp): slots [32, 64)
+#define TC_TLG(k) do { if (a.tl != nullptr && blockIdx.x == 0 && it == 0 && threadIdx.x == 128) a.tl[32 + (k)] = (unsigned long long)clock64(); } while (0)
+
 template <int ROWS>
 __global__ void __launch_bounds__(TC2_THREADS, 1) edge_fwd_tc_kernel(const __grid_constant__ EdgeTcArgs a) {
     pdl_entry();
@@ -280,7 +391,7 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_fwd_tc_kernel(const __gri
     const bool upd = (l < L - 1);
     const int J_DK = 0, J_DV = 1, J_F = 2, J_S1 = upd ? 3 : 2, J_S2 = upd ? 4 : 3;
     constexpr int RPW = ROWS / TC2_CWARPS;      // rows per compute warp in the coalesced phases
-    constexpr bool SMALL = ROWS <= 64;          // tile_to_a-free schedule: m stays in `tile`, f rows in `abuf`, results in tc_aux
+    constexpr bool SMALL = ROWS <= 64;          // warp-specialised schedule, three buffers: see below
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, col = lane * 4;
     const int E = ws.rowptr[ws.N];
     const int trows = min(ROWS, max(16, a.tile_rows));          // edges per tile (<= ROWS, chosen on the host so the tiles fill whole waves)
@@ -300,17 +411,12 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_fwd_tc_kernel(const __gri
     float* __restrict__ P1 = ws.P1[l];
     float* __restrict__ SP = ws.SP[l];
     float* __restrict__ ATT = ws.ATT[l];
-    const int cch = threadIdx.x & (D - 1), grp = threadIdx.x >> 7;      // aggregation role: channel, target parity
     for (int it = 0; it < my_tiles; it++) {
         const uint32_t tpar = (uint32_t)(it & 1);
         const int e0 = ((int)blockIdx.x + it * (int)gridDim.x) * trows;
         const int nvalid = min(trows, E - e0);
-        // rows are dealt to the compute warps in contiguous runs of rpw = ceil(nvalid / 16): a tile shorter than ROWS
-        // keeps every warp busy (slot s of a warp is row warp * rpw + s, valid while s < rpw and the row exists)
-        const int rpw = (nvalid + TC2_CWARPS - 1) / TC2_CWARPS, r0 = warp * rpw;
         // ---- per-edge feature rows -> the A operand buffer by TMA bulk copies (one 512 B row each, padded rows in
-        //      shared memory), completion on an mbarrier: f is the A operand of the dk, dv and f products (and, in a
-        //      tile of <= 64 rows, the edge update's residual) ----
+        //      shared memory), completion on an mbarrier: f is the A operand of the dk, dv and f products ----
         {
             constexpr int RW = ROWS / TC2_CWARPS;                 // rows a warp issues
             const int w0 = warp * RW, wn = max(0, min(RW, nvalid - w0));
@@ -322,205 +428,280 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) edge_fwd_tc_kernel(const __gri
             if (lane < wn) tc::tma_load_1d(&sh.abuf[w0 + lane][0], Fin + (size_t)(e0 + w0 + lane) * D, D * 4, &sh.b_tile);
         }
         load_edge_meta<TC_TE, TC2_CTHREADS>(sh.meta, ws, e0, nvalid);
-        tc::mbar_wait(&sh.b_tile, tpar);
-        csync();
-        TC_TL(2);
-        // ---- dk -> attention weights ----
-        float Areg[RPW];
-        tc2_mma(sh, ring, sh.abuf, acc, a.jobs[J_DK].accumulate, warp, lane, nvalid);
-        TC_TL(4);
-        tc2_acc_to(sh.tile, acc, warp, lane, nvalid);         // (nothing reads the tile between the MMAs' barrier and here)
-        csync();
-        {
-            TC_TL(5);
-            const float4 bb = ldg4(lw.b1 + col);
-#pragma unroll
-            for (int r = 0; r < RPW; r++) {
-                if (r >= rpw) break;
-                const int row = r0 + r;
-                const float4 qi = ldg4(QKV + (size_t)sh.meta.dst[row] * 3 * D + col);
-                const float4 kj = ldg4(QKV + (size_t)sh.meta.src[row] * 3 * D + D + col);
-                const float4 P = ld4(&sh.tile[row][col]) + bb;
-                const float av = quad_sum(hsum4(qi * kj * silu4(P)));
-                Areg[r] = silu_(av) * sh.meta.C[row];
-                if ((r < rpw && row < nvalid)) {
-                    st4(P1 + (size_t)(e0 + row) * 3 * D + col, P);
-                    if ((lane & 3) == 0) ATT[(size_t)(e0 + row) * H + (lane >> 2)] = av;
+        if constexpr (SMALL) {
+            // ---- warp-specialised tile.  Buffers: abuf = the f rows (A of dk, dv, f), then s1; tile = dk, then f, then
+            //      s2; tc_aux = q_i * k_j, then dv, turned into m in place (A of s1 and s2).  The MMA warps run dk, dv
+            //      and f back to back and s1, s2 as soon as m is complete; a result is stored once the phase that read
+            //      the buffer before it is done.  The edge update reads f from global memory (the rows the TMA just
+            //      brought into L2), so abuf is free for s1 once the f product has retired. ----
+            enum : int { H_DK = 3, H_ATT, H_DV, H_F, H_M, H_EU };     // hand-offs (named barrier ids)
+            TcRow* const xb = tc_aux(sh);
+            csync();                                                  // meta
+            if (tc2_is_mma_warp(warp)) {
+                tc::mbar_wait(&sh.b_tile, tpar);
+                TC_TL(2);
+                tc2_mma<ROWS, true>(sh, ring, sh.abuf, acc, a.jobs[J_DK].accumulate, warp, lane, nvalid);
+                tc2_acc_to(sh.tile, acc, warp, lane, nvalid);
+                handoff_arrive(H_DK);
+                TC_TL(4);
+                tc2_mma<ROWS, true>(sh, ring, sh.abuf, acc, a.jobs[J_DV].accumulate, warp, lane, nvalid);
+                TC_TL(7);
+                handoff_wait(H_ATT);                                  // the attention phase is done with dk and q_i * k_j
+                tc2_acc_to(xb, acc, warp, lane, nvalid);
+                handoff_arrive(H_DV);
+                TC_TL(8);
+                if (upd) {
+                    tc2_mma<ROWS, true>(sh, ring, sh.abuf, acc, a.jobs[J_F].accumulate, warp, lane, nvalid);
+                    tc2_acc_to(sh.tile, acc, warp, lane, nvalid);
+                    handoff_arrive(H_F);
+                    TC_TL(11);
                 }
-            }
-        }
-        TC_TL(6);
-        // ---- dv -> message m (in place in the tile) ----
-        tc2_mma(sh, ring, sh.abuf, acc, a.jobs[J_DV].accumulate, warp, lane, nvalid);
-        TC_TL(7);
-        csync();
-        tc2_acc_to(sh.tile, acc, warp, lane, nvalid);
-        csync();
-        {
-            TC_TL(8);
-            const float4 bb = ldg4(lw.b1 + D + col);
+                handoff_wait(H_M);                                    // m complete (and every MMA warp is past the f rows)
+                TC_TL(3);
+                tc2_mma<ROWS, true>(sh, ring, xb, acc, a.jobs[J_S1].accumulate, warp, lane, nvalid);
+                tc2_acc_to(sh.abuf, acc, warp, lane, nvalid);
+                TC_TL(13);
+                if (threadIdx.x == 0 && it + 1 < my_tiles) {         // next tile's feature rows -> L2 (bulk prefetch), shortly before use
+                    const int en = ((int)blockIdx.x + (it + 1) * (int)gridDim.x) * trows;
+                    tc::tma_prefetch_l2(Fin + (size_t)en * D, (uint32_t)min(trows, E - en) * D * 4);
+                }
+                tc2_mma<ROWS, true>(sh, ring, xb, acc, a.jobs[J_S2].accumulate, warp, lane, nvalid);
+                TC_TL(16);
+                if (upd) handoff_wait(H_EU);                          // the edge update is done with the tile
+                tc2_acc_to(sh.tile, acc, warp, lane, nvalid);
+                TC_TL(17);
+            } else {
+                // gather warps: gw = 0..7 owns rows [gw * grpw, (gw + 1) * grpw), grpw = ceil(nvalid / 8)
+                constexpr int GRPW = ROWS / (TC2_CWARPS / 2);
+                const int gw = (warp >> 3) * 4 + (warp & 3), gt = gw * 32 + lane;
+                const int grpw = (nvalid + 7) / 8, g0 = gw * grpw;
+                const int gch = gt & (D - 1), ggrp = gt >> 7;          // per-target sums: channel, target parity
+                // ---- attention weights: q_i * k_j (-> tc_aux) before dk lands ----
+#pragma unroll 4
+                for (int r = 0; r < GRPW; r++) {
+                    if (r >= grpw) break;
+                    const int row = g0 + r;
+                    st4(&xb[row][col], ldg4(QKV + (size_t)sh.meta.dst[row] * 3 * D + col) * ldg4(QKV + (size_t)sh.meta.src[row] * 3 * D + D + col));
+                }
+                TC_TLG(0);
+                float Areg[GRPW];
+                {
+                    const float4 bb = ldg4(lw.b1 + col);
+                    handoff_wait(H_DK);
+                    TC_TLG(1);
 #pragma unroll
-            for (int r = 0; r < RPW; r++) {
-                if (r >= rpw) break;
-                const int row = r0 + r;
-                const float4 vj = ldg4(QKV + (size_t)sh.meta.src[row] * 3 * D + 2 * D + col);
-                const float4 P = ld4(&sh.tile[row][col]) + bb;
-                st4(&sh.tile[row][col], vj * silu4(P) * Areg[r]);
-                if ((r < rpw && row < nvalid)) st4(P1 + (size_t)(e0 + row) * 3 * D + D + col, P);
-            }
-        }
-        csync();
-        TC_TL(9);
-        // ---- xa_i = sum_e m_e ----
-        {
-            const int i_first = sh.meta.dst[0], i_last = sh.meta.dst[nvalid - 1];
-            for (int i = i_first + grp; i <= i_last; i += TC2_NGRP) {
-                const int q0 = ws.rowptr[i], q1 = ws.rowptr[i + 1];
-                const int lo = max(q0, e0) - e0, hi = min(q1, e0 + nvalid) - e0;
-                float xa = 0.f;
-                for (int r = lo; r < hi; r++) xa += sh.tile[r][cch];
-                if (q0 >= e0 && q1 <= e0 + nvalid) ws.XA[(size_t)i * D + cch] = xa;
-                else atomicAdd(ws.XA + (size_t)i * D + cch, xa);
-            }
-        }
-        TC_TL(10);
-        // ---- f product; A = m for s1 and s2: a tile of <= 64 rows leaves m in `tile` (the products read it there) and
-        //      keeps the f rows in `abuf` for the edge update, a longer one copies m into `abuf` ----
-        if (upd) tc2_mma(sh, ring, sh.abuf, acc, a.jobs[J_F].accumulate, warp, lane, nvalid);
-        if constexpr (!SMALL) tc2_tile_to_a(sh, nvalid);
-        TC_TL(11);
-        // ---- edge update from the f chunk (D0) ----
-        if (upd) {
-            TcRow* const pfb = SMALL ? tc_aux(sh) : sh.tile;
-            if constexpr (!SMALL) csync();                   // m tile fully consumed (xa + A copy)
-            tc2_acc_to(pfb, acc, warp, lane, nvalid);
-            csync();
-            const float4 bb = ldg4(lw.b1 + 2 * D + col);
+                    for (int r = 0; r < GRPW; r++) {
+                        if (r >= grpw) break;
+                        const int row = g0 + r;
+                        const float4 P = ld4(&sh.tile[row][col]) + bb;
+                        const float av = quad_sum(hsum4(ld4(&xb[row][col]) * silu4(P)));
+                        Areg[r] = silu_(av) * sh.meta.C[row];
+                        if (row < nvalid) {
+                            st4(P1 + (size_t)(e0 + row) * 3 * D + col, P);
+                            if ((lane & 3) == 0) ATT[(size_t)(e0 + row) * H + (lane >> 2)] = av;
+                        }
+                    }
+                    handoff_arrive(H_ATT);
+                }
+                TC_TLG(2);
+                // ---- message m = v_j * silu(dv) * A (in place in tc_aux): v_j before dv lands ----
+                {
+                    float4 vj[GRPW];
+#pragma unroll
+                    for (int r = 0; r < GRPW; r++) {
+                        if (r >= grpw) break;
+                        vj[r] = ldg4(QKV + (size_t)sh.meta.src[g0 + r] * 3 * D + 2 * D + col);
+                    }
+                    const float4 bb = ldg4(lw.b1 + D + col);
+                    handoff_wait(H_DV);
+                    TC_TLG(3);
+#pragma unroll
+                    for (int r = 0; r < GRPW; r++) {
+                        if (r >= grpw) break;
+                        const int row = g0 + r;
+                        const float4 P = ld4(&xb[row][col]) + bb;
+                        st4(&xb[row][col], vj[r] * silu4(P) * Areg[r]);
+                        if (row < nvalid) st4(P1 + (size_t)(e0 + row) * 3 * D + D + col, P);
+                    }
+                }
+                gather_sync();
+                handoff_arrive(H_M);
+                TC_TLG(4);
+                tc_fwd_xa(sh, ws, xb, e0, nvalid, gch, ggrp, 2);
+                TC_TLG(5);
+                // ---- edge update f' = f + silu(Pf) * wdot (f from global memory: abuf is s1's by now) ----
+                if (upd) {
+                    const float4 bb = ldg4(lw.b1 + 2 * D + col);
+                    handoff_wait(H_F);
+                    TC_TLG(6);
 #pragma unroll 1
-            for (int rb = 0; rb < RPW; rb += 2) {       // gathers of 2 rows in flight before the first global store
-                if (rb >= rpw) break;
-                float4 tir[2][3], ujr[2][3], fin[2];
+                    for (int rb = 0; rb < GRPW; rb += 2) {             // gathers of 2 rows in flight before the first global store
+                        if (rb >= grpw) break;
+                        float4 tir[2][3], ujr[2][3], fin[2];
 #pragma unroll
-                for (int u = 0; u < 2; u++) {
-                    const int row = r0 + rb + u;
-                    const size_t i3 = (size_t)sh.meta.dst[row] * 3, j3 = (size_t)sh.meta.src[row] * 3;
-                    if (rb + u < rpw && row < nvalid) fin[u] = SMALL ? ld4(&sh.abuf[row][col]) : ldg4(Fin + (size_t)(e0 + row) * D + col);
-                    else fin[u] = f4s(0.f);
+                        for (int u = 0; u < 2; u++) {
+                            const int row = g0 + rb + u;
+                            const size_t i3 = (size_t)sh.meta.dst[row] * 3, j3 = (size_t)sh.meta.src[row] * 3;
+                            fin[u] = (rb + u < grpw && row < nvalid) ? ldg4(Fin + (size_t)(e0 + row) * D + col) : f4s(0.f);
 #pragma unroll
-                    for (int s = 0; s < 3; s++) {
-                        tir[u][s] = ldg4(TU + (i3 + s) * 2 * D + col);
-                        ujr[u][s] = ldg4(TU + (j3 + s) * 2 * D + D + col);
+                            for (int s = 0; s < 3; s++) {
+                                tir[u][s] = ldg4(TU + (i3 + s) * 2 * D + col);
+                                ujr[u][s] = ldg4(TU + (j3 + s) * 2 * D + D + col);
+                            }
+                        }
+#pragma unroll
+                        for (int u = 0; u < 2; u++) {
+                            const int row = g0 + rb + u;
+                            const float4 dd = sh.meta.d[row];
+                            const float4 Pf = ld4(&sh.tile[row][col]) + bb;
+                            const float4 fp = silu4(Pf);
+                            const float4 a1 = tir[u][0] * dd.x + tir[u][1] * dd.y + tir[u][2] * dd.z;
+                            const float4 a2 = ujr[u][0] * dd.x + ujr[u][1] * dd.y + ujr[u][2] * dd.z;
+                            const float4 wdot = (tir[u][0] - a1 * dd.x) * (ujr[u][0] - a2 * dd.x) + (tir[u][1] - a1 * dd.y) * (ujr[u][1] - a2 * dd.y) +
+                                                (tir[u][2] - a1 * dd.z) * (ujr[u][2] - a2 * dd.z);
+                            if (rb + u < grpw && row < nvalid) {
+                                st4(P1 + (size_t)(e0 + row) * 3 * D + 2 * D + col, Pf);
+                                st4(Fout + (size_t)(e0 + row) * D + col, fin[u] + fp * wdot);
+                            }
+                        }
                     }
+                    handoff_arrive(H_EU);
                 }
+                TC_TLG(7);
+            }
+            // ---- s1 (abuf), s2 (tile): va_i, by the whole CTA (the MMA warps have no product left) ----
+            csync();
+            TC_TL(18);
+            const int cch = threadIdx.x & (D - 1), grp = threadIdx.x >> 7;
+            float bnd[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+            tc_fwd_s1(sh, ws, lw, VN, SP, sh.abuf, e0, nvalid, cch, grp, TC2_NGRP, bnd);
+            TC_TL(19);
+            tc_fwd_s2(sh, ws, lw, SP, sh.tile, e0, nvalid, cch, grp, TC2_NGRP, bnd);
+            TC_TL(20);
+        } else {
+            const int cch = threadIdx.x & (D - 1), grp = threadIdx.x >> 7;      // per-target sums: channel, target parity
+            // rows are dealt to the compute warps in contiguous runs of rpw = ceil(nvalid / 16): a tile shorter than ROWS
+            // keeps every warp busy (slot s of a warp is row warp * rpw + s, valid while s < rpw and the row exists)
+            const int rpw = (nvalid + TC2_CWARPS - 1) / TC2_CWARPS, r0 = warp * rpw;
+            tc::mbar_wait(&sh.b_tile, tpar);
+            csync();
+            TC_TL(2);
+            // ---- dk -> attention weights ----
+            float Areg[RPW];
+            tc2_mma(sh, ring, sh.abuf, acc, a.jobs[J_DK].accumulate, warp, lane, nvalid);
+            TC_TL(4);
+            tc2_acc_to(sh.tile, acc, warp, lane, nvalid);         // (nothing reads the tile between the MMAs' barrier and here)
+            csync();
+            {
+                TC_TL(5);
+                const float4 bb = ldg4(lw.b1 + col);
 #pragma unroll
-                for (int u = 0; u < 2; u++) {
-                    const int row = r0 + rb + u;
-                    const float4 dd = sh.meta.d[row];
-                    const float4 Pf = ld4(&pfb[row][col]) + bb;
-                    const float4 fp = silu4(Pf);
-                    const float4 a1 = tir[u][0] * dd.x + tir[u][1] * dd.y + tir[u][2] * dd.z;
-                    const float4 a2 = ujr[u][0] * dd.x + ujr[u][1] * dd.y + ujr[u][2] * dd.z;
-                    const float4 wdot = (tir[u][0] - a1 * dd.x) * (ujr[u][0] - a2 * dd.x) + (tir[u][1] - a1 * dd.y) * (ujr[u][1] - a2 * dd.y) +
-                                        (tir[u][2] - a1 * dd.z) * (ujr[u][2] - a2 * dd.z);
-                    if ((rb + u < rpw && row < nvalid)) {
-                        st4(P1 + (size_t)(e0 + row) * 3 * D + 2 * D + col, Pf);
-                        st4(Fout + (size_t)(e0 + row) * D + col, fin[u] + fp * wdot);
+                for (int r = 0; r < RPW; r++) {
+                    if (r >= rpw) break;
+                    const int row = r0 + r;
+                    const float4 qi = ldg4(QKV + (size_t)sh.meta.dst[row] * 3 * D + col);
+                    const float4 kj = ldg4(QKV + (size_t)sh.meta.src[row] * 3 * D + D + col);
+                    const float4 P = ld4(&sh.tile[row][col]) + bb;
+                    const float av = quad_sum(hsum4(qi * kj * silu4(P)));
+                    Areg[r] = silu_(av) * sh.meta.C[row];
+                    if ((r < rpw && row < nvalid)) {
+                        st4(P1 + (size_t)(e0 + row) * 3 * D + col, P);
+                        if ((lane & 3) == 0) ATT[(size_t)(e0 + row) * H + (lane >> 2)] = av;
                     }
                 }
             }
-        }
-        TC_TL(12);
-        // ---- s1 (D1): va_i += sum_e vn_j * s1 ----
-        float bnd[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
-        TcRow* const s1b = SMALL ? tc_aux(sh) : sh.tile;
-        tc2_mma(sh, ring, SMALL ? sh.tile : sh.abuf, acc, a.jobs[J_S1].accumulate, warp, lane, nvalid);
-        TC_TL(13);
-        if constexpr (!SMALL) csync();
-        tc2_acc_to(s1b, acc, warp, lane, nvalid);
-        csync();
-        {
+            TC_TL(6);
+            // ---- dv -> message m (in place in the tile) ----
+            tc2_mma(sh, ring, sh.abuf, acc, a.jobs[J_DV].accumulate, warp, lane, nvalid);
+            TC_TL(7);
+            csync();
+            tc2_acc_to(sh.tile, acc, warp, lane, nvalid);
+            csync();
+            {
+                TC_TL(8);
+                const float4 bb = ldg4(lw.b1 + D + col);
+#pragma unroll
+                for (int r = 0; r < RPW; r++) {
+                    if (r >= rpw) break;
+                    const int row = r0 + r;
+                    const float4 vj = ldg4(QKV + (size_t)sh.meta.src[row] * 3 * D + 2 * D + col);
+                    const float4 P = ld4(&sh.tile[row][col]) + bb;
+                    st4(&sh.tile[row][col], vj * silu4(P) * Areg[r]);
+                    if ((r < rpw && row < nvalid)) st4(P1 + (size_t)(e0 + row) * 3 * D + D + col, P);
+                }
+            }
+            csync();
+            TC_TL(9);
+            tc_fwd_xa(sh, ws, sh.tile, e0, nvalid, cch, grp, TC2_NGRP);
+            TC_TL(10);
+            // ---- f product; A = m for s1 and s2: m is copied into abuf ----
+            if (upd) tc2_mma(sh, ring, sh.abuf, acc, a.jobs[J_F].accumulate, warp, lane, nvalid);
+            tc2_tile_to_a(sh, nvalid);
+            TC_TL(11);
+            // ---- edge update from the f chunk (D0) ----
+            if (upd) {
+                csync();                                         // m tile fully consumed (xa + A copy)
+                tc2_acc_to(sh.tile, acc, warp, lane, nvalid);
+                csync();
+                const float4 bb = ldg4(lw.b1 + 2 * D + col);
+#pragma unroll 1
+                for (int rb = 0; rb < RPW; rb += 2) {       // gathers of 2 rows in flight before the first global store
+                    if (rb >= rpw) break;
+                    float4 tir[2][3], ujr[2][3], fin[2];
+#pragma unroll
+                    for (int u = 0; u < 2; u++) {
+                        const int row = r0 + rb + u;
+                        const size_t i3 = (size_t)sh.meta.dst[row] * 3, j3 = (size_t)sh.meta.src[row] * 3;
+                        if (rb + u < rpw && row < nvalid) fin[u] = ldg4(Fin + (size_t)(e0 + row) * D + col);
+                        else fin[u] = f4s(0.f);
+#pragma unroll
+                        for (int s = 0; s < 3; s++) {
+                            tir[u][s] = ldg4(TU + (i3 + s) * 2 * D + col);
+                            ujr[u][s] = ldg4(TU + (j3 + s) * 2 * D + D + col);
+                        }
+                    }
+#pragma unroll
+                    for (int u = 0; u < 2; u++) {
+                        const int row = r0 + rb + u;
+                        const float4 dd = sh.meta.d[row];
+                        const float4 Pf = ld4(&sh.tile[row][col]) + bb;
+                        const float4 fp = silu4(Pf);
+                        const float4 a1 = tir[u][0] * dd.x + tir[u][1] * dd.y + tir[u][2] * dd.z;
+                        const float4 a2 = ujr[u][0] * dd.x + ujr[u][1] * dd.y + ujr[u][2] * dd.z;
+                        const float4 wdot = (tir[u][0] - a1 * dd.x) * (ujr[u][0] - a2 * dd.x) + (tir[u][1] - a1 * dd.y) * (ujr[u][1] - a2 * dd.y) +
+                                            (tir[u][2] - a1 * dd.z) * (ujr[u][2] - a2 * dd.z);
+                        if ((rb + u < rpw && row < nvalid)) {
+                            st4(P1 + (size_t)(e0 + row) * 3 * D + 2 * D + col, Pf);
+                            st4(Fout + (size_t)(e0 + row) * D + col, fin[u] + fp * wdot);
+                        }
+                    }
+                }
+            }
+            TC_TL(12);
+            // ---- s1 (D1): va_i += sum_e vn_j * s1 ----
+            float bnd[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+            tc2_mma(sh, ring, sh.abuf, acc, a.jobs[J_S1].accumulate, warp, lane, nvalid);
+            TC_TL(13);
+            csync();
+            tc2_acc_to(sh.tile, acc, warp, lane, nvalid);
+            csync();
             TC_TL(14);
-            const float b = __ldg(lw.bs + cch);
-            const int i_first = sh.meta.dst[0], i_last = sh.meta.dst[nvalid - 1];
-            int nb = 0;
-            for (int i = i_first + grp; i <= i_last; i += TC2_NGRP) {
-                const int q0 = ws.rowptr[i], q1 = ws.rowptr[i + 1];
-                const int lo = max(q0, e0) - e0, hi = min(q1, e0 + nvalid) - e0;
-                float v0 = 0.f, v1 = 0.f, v2 = 0.f;
-                int r = lo;
-                for (; r + 4 <= hi; r += 4) {              // 12 independent gathers in flight
-                    float g[4][3], s1[4];
-#pragma unroll
-                    for (int u = 0; u < 4; u++) {
-                        const size_t j3 = (size_t)sh.meta.src[r + u] * 3;
-                        g[u][0] = __ldg(VN + (j3 + 0) * D + cch); g[u][1] = __ldg(VN + (j3 + 1) * D + cch); g[u][2] = __ldg(VN + (j3 + 2) * D + cch);
-                        const float sp = s1b[r + u][cch] + b;
-                        SP[(size_t)(e0 + r + u) * 2 * D + cch] = sp;
-                        s1[u] = silu_(sp);
-                    }
-#pragma unroll
-                    for (int u = 0; u < 4; u++) { v0 += g[u][0] * s1[u]; v1 += g[u][1] * s1[u]; v2 += g[u][2] * s1[u]; }
-                }
-                for (; r < hi; r++) {
-                    const size_t j3 = (size_t)sh.meta.src[r] * 3;
-                    const float sp = s1b[r][cch] + b;
-                    SP[(size_t)(e0 + r) * 2 * D + cch] = sp;
-                    const float s1 = silu_(sp);
-                    v0 += __ldg(VN + (j3 + 0) * D + cch) * s1;
-                    v1 += __ldg(VN + (j3 + 1) * D + cch) * s1;
-                    v2 += __ldg(VN + (j3 + 2) * D + cch) * s1;
-                }
-                if (q0 >= e0 && q1 <= e0 + nvalid) {
-                    ws.VA[((size_t)i * 3 + 0) * D + cch] = v0;
-                    ws.VA[((size_t)i * 3 + 1) * D + cch] = v1;
-                    ws.VA[((size_t)i * 3 + 2) * D + cch] = v2;
-                } else if (nb < 2) {
-                    bnd[nb][0] = v0; bnd[nb][1] = v1; bnd[nb][2] = v2;
-                    nb++;
-                }
+            tc_fwd_s1(sh, ws, lw, VN, SP, sh.tile, e0, nvalid, cch, grp, TC2_NGRP, bnd);
+            TC_TL(15);
+            if (threadIdx.x == 0 && it + 1 < my_tiles) {             // next tile's feature rows -> L2 (bulk prefetch), shortly before use
+                const int en = ((int)blockIdx.x + (it + 1) * (int)gridDim.x) * trows;
+                tc::tma_prefetch_l2(Fin + (size_t)en * D, (uint32_t)min(trows, E - en) * D * 4);
             }
-        }
-        TC_TL(15);
-        if (threadIdx.x == 0 && it + 1 < my_tiles) {             // next tile's feature rows -> L2 (bulk prefetch), shortly before use
-            const int en = ((int)blockIdx.x + (it + 1) * (int)gridDim.x) * trows;
-            tc::tma_prefetch_l2(Fin + (size_t)en * D, (uint32_t)min(trows, E - en) * D * 4);
-        }
-        // ---- s2 (D0): va_i += sum_e s2 * d ----
-        TcRow* const s2b = SMALL ? sh.abuf : sh.tile;
-        tc2_mma(sh, ring, SMALL ? sh.tile : sh.abuf, acc, a.jobs[J_S2].accumulate, warp, lane, nvalid);
-        TC_TL(16);
-        if constexpr (!SMALL) csync();
-        tc2_acc_to(s2b, acc, warp, lane, nvalid);
-        csync();
-        {
+            // ---- s2 (D0): va_i += sum_e s2 * d ----
+            tc2_mma(sh, ring, sh.abuf, acc, a.jobs[J_S2].accumulate, warp, lane, nvalid);
+            TC_TL(16);
+            csync();
+            tc2_acc_to(sh.tile, acc, warp, lane, nvalid);
+            csync();
             TC_TL(17);
-            const float b = __ldg(lw.bs + D + cch);
-            const int i_first = sh.meta.dst[0], i_last = sh.meta.dst[nvalid - 1];
-            int nb = 0;
-            for (int i = i_first + grp; i <= i_last; i += TC2_NGRP) {
-                const int q0 = ws.rowptr[i], q1 = ws.rowptr[i + 1];
-                const int lo = max(q0, e0) - e0, hi = min(q1, e0 + nvalid) - e0;
-                float v0 = 0.f, v1 = 0.f, v2 = 0.f;
-                for (int r = lo; r < hi; r++) {
-                    const float4 de = sh.meta.d[r];
-                    const float sp = s2b[r][cch] + b;
-                    SP[(size_t)(e0 + r) * 2 * D + D + cch] = sp;
-                    const float s2 = silu_(sp);
-                    v0 += s2 * de.x; v1 += s2 * de.y; v2 += s2 * de.z;
-                }
-                if (q0 >= e0 && q1 <= e0 + nvalid) {
-                    ws.VA[((size_t)i * 3 + 0) * D + cch] += v0;
-                    ws.VA[((size_t)i * 3 + 1) * D + cch] += v1;
-                    ws.VA[((size_t)i * 3 + 2) * D + cch] += v2;
-                } else if (nb < 2) {
-                    atomicAdd(ws.VA + ((size_t)i * 3 + 0) * D + cch, bnd[nb][0] + v0);
-                    atomicAdd(ws.VA + ((size_t)i * 3 + 1) * D + cch, bnd[nb][1] + v1);
-                    atomicAdd(ws.VA + ((size_t)i * 3 + 2) * D + cch, bnd[nb][2] + v2);
-                    nb++;
-                }
-            }
+            tc_fwd_s2(sh, ws, lw, SP, sh.tile, e0, nvalid, cch, grp, TC2_NGRP, bnd);
+            TC_TL(18);
         }
-        TC_TL(18);
         csync();                                              // tile / meta free for the next tile
     }
     if (a.tl != nullptr && blockIdx.x == 0 && threadIdx.x == 0) a.tl[31] = (unsigned long long)clock64();

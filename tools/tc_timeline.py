@@ -23,6 +23,14 @@ from ai2bmd_b200.weights import load_state_dict  # noqa: E402
 
 # Slots marked "96/128 rows" are stamped only by the two-buffer schedule of 96- and 128-row tiles; a tile of <= 64 rows
 # copies no A operand and gathers no row set twice (its s1/s2, g_Pdk/g_q and g_Pf/g_wdot rows are written in one pass).
+# The forward of a tile of <= 64 rows is warp-specialised: FWD_WS are the stamps of the MMA warps (thread 0), slots
+# 32.. those of the gather warps (thread 128); both are printed in time order.
+FWD_WS = {0: "kernel start", 1: "setup done (barriers)", 2: "f rows (= A) landed", 4: "dk -> tile",
+          7: "dv MMAs done", 8: "dv -> tc_aux (attention done)", 11: "f -> tile", 3: "m complete (A of s1, s2)",
+          13: "s1 -> abuf", 16: "s2 MMAs done", 17: "s2 -> tile (edge update done)", 18: "CTA barrier: s1/s2 sums start",
+          19: "s1 sums done", 20: "s2 sums done", 31: "teardown done"}
+FWD_WS_GATHER = {32: "q*k rows -> tc_aux", 33: "dk seen", 34: "attention weights done", 35: "dv seen",
+                 36: "messages m done", 37: "xa aggregation done", 38: "f seen", 39: "edge update done"}
 FWD = {0: "kernel start", 1: "setup done (barriers)", 2: "f rows (= A) + meta loaded",
        4: "dk MMAs done", 5: "dk -> tile", 6: "attention weights done", 7: "dv MMAs done", 8: "dv -> tile",
        9: "messages m done", 10: "xa aggregation done", 11: "f MMAs done (96/128 rows: + A=m copy)",
@@ -51,6 +59,16 @@ def show(title, tl, names, mhz):
         t = int(tl[k])
         print(f"  [{k:2d}] {names[k]:<36} {(t - t0) / mhz:8.2f} us   (+{(t - prev) / mhz:6.2f})")
         prev = t
+
+
+def show_roles(title, tl, mma, gather, mhz):
+    t0 = int(tl[0])
+    print(f"--- {title} (M: MMA warps, G: gather warps) ---")
+    stamps = sorted([(int(tl[k]), "M", n) for k, n in mma.items() if tl[k]] + [(int(tl[k]), "G", n) for k, n in gather.items() if tl[k]])
+    last = {"M": t0, "G": t0}
+    for t, role, name in stamps:
+        print(f"  {role} {name:<36} {(t - t0) / mhz:8.2f} us   (+{(t - last[role]) / mhz:6.2f} on {role})")
+        last[role] = t
 
 
 def main():
@@ -86,7 +104,10 @@ def main():
     nl = 6
     tf = eng.debug_read("TL", args.layer, (64,), dtype=np.uint64)
     tb = eng.debug_read("TL", nl + args.layer, (64,), dtype=np.uint64)
-    show("edge_fwd_tc", tf, FWD, mhz)
+    if tf[32:].any():
+        show_roles("edge_fwd_tc", tf, FWD_WS, FWD_WS_GATHER, mhz)
+    else:
+        show("edge_fwd_tc", tf, FWD, mhz)
     show("edge_bwd_tc", tb, BWD, mhz)
     if eng.get_option("node_tc") == 0:
         EMB = {0: "start", 1: "previous kernel complete (pdl)", 2: "loads issued, rows staged", 3: "aggregation done", 4: "combine done", 5: "x written"}
