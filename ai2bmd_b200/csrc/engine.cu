@@ -185,6 +185,12 @@ struct vb_handle {
     long long* d_step = nullptr;
     long long ehist_cap = 1 << 16;
     float* md_ef = nullptr;              // caller-owned [3*n_protein + 1]
+    // frame recorder (k_md.cuh MdRecorder): control words and the ring in one allocation
+    MdRecorder rec{};
+    void* rec_mem = nullptr;
+    // host mirrors of the step counter and the frame count once all enqueued MD work has run (a guard that fires makes
+    // the device fall behind them); exact again at every call that synchronises
+    long long md_step_enq = 0, rec_frames_enq = 0;
     // Hookean restraints (k_md.cuh MdRestraints): term CSR + rf [3*n_protein + 1] in one allocation
     bool rs_ready = false;
     MdRestraints rs{};
@@ -234,8 +240,13 @@ struct vb_handle {
         cudaFree(rs_mem);
         rs_mem = nullptr; rs = MdRestraints{}; rs_ready = false;
     }
+    void free_rec() {
+        cudaFree(rec_mem);
+        rec_mem = nullptr; rec = MdRecorder{}; rec_frames_enq = 0;
+    }
     void free_md() {
         free_rs();                       // the restraints index the MD state
+        free_rec();                      // ... and so does the frame ring
         cudaFree(d_mx); cudaFree(d_mv); cudaFree(d_mmass); cudaFree(d_ehist);
         cudaFree(d_real); cudaFree(d_acc); cudaFree(d_rem); cudaFree(d_blen); cudaFree(d_step);
         d_mx = d_mv = d_mmass = d_ehist = nullptr; d_real = d_acc = d_rem = nullptr; d_blen = nullptr; d_step = nullptr;
@@ -1207,11 +1218,23 @@ int md_eval_enqueue(vb_handle* h, cudaStream_t st) {
     return VB_OK;
 }
 void md_kick1_enqueue(vb_handle* h, cudaStream_t st) {
-    md_kick1_kernel<<<1, MD_K1_THREADS, 0, st>>>(h->md, h->d_step, h->d_mmass, h->md_ef, h->rs.rf, h->d_mx, h->d_mv);
+    md_kick1_kernel<<<1, MD_K1_THREADS, 0, st>>>(h->md, h->d_step, h->d_mmass, h->md_ef, h->rs.rf, h->d_mx, h->d_mv,
+                                                 h->rec.ctl);
 }
 void md_kick2_enqueue(vb_handle* h, cudaStream_t st) {
-    md_kick2_kernel<<<1, MD_K2_THREADS, 0, st>>>(h->md, h->d_step, h->d_mmass, h->md_ef, h->rs.rf, h->d_mv, h->d_ehist,
-                                                 h->ehist_cap);
+    md_kick2_kernel<<<1, MD_K2_THREADS, 0, st>>>(h->md, h->d_step, h->d_mmass, h->md_ef, h->rs.rf, h->d_mx, h->d_mv,
+                                                 h->d_ehist, h->ehist_cap, h->rec);
+}
+// host mirrors after enqueueing n more steps
+void md_count_steps(vb_handle* h, long long n) {
+    if (h->rec.ctl) h->rec_frames_enq += (h->md_step_enq + n) / h->rec.every - h->md_step_enq / h->rec.every;
+    h->md_step_enq += n;
+}
+// after a device synchronisation: the mirrors from the device's own counters
+int md_resync(vb_handle* h) {
+    CUDA_TRY(h, cudaMemcpy(&h->md_step_enq, h->d_step, sizeof(long long), cudaMemcpyDeviceToHost));
+    if (h->rec.ctl) CUDA_TRY(h, cudaMemcpy(&h->rec_frames_enq, h->rec.ctl + MD_REC_FRAMES, sizeof(long long), cudaMemcpyDeviceToHost));
+    return VB_OK;
 }
 // `stepping`: the call enqueues or changes MD work, which a broken all-reduce would corrupt; reading the state stays
 // allowed, so a failed run can still be inspected
@@ -1266,6 +1289,7 @@ int vb_md_setup(vb_handle* h, int64_t n_protein_atoms, const double* masses_host
     CUDA_TRY(h, cudaMemset(h->d_step, 0, sizeof(long long)));
     h->md = MdParams{P, dt, kT, friction, (unsigned long long)seed, nullptr, 0};
     h->md_ef = ef_prot_dev;
+    h->md_step_enq = 0;
     h->md_ready = true;
     return VB_OK;
 }
@@ -1292,6 +1316,87 @@ int vb_md_set_state(vb_handle* h, const double* x_host, const double* v_host, in
     CUDA_TRY(h, cudaMemcpy(h->d_mx, x_host, sizeof(double) * 3 * h->n_protein, cudaMemcpyHostToDevice));
     CUDA_TRY(h, cudaMemcpy(h->d_mv, v_host, sizeof(double) * 3 * h->n_protein, cudaMemcpyHostToDevice));
     CUDA_TRY(h, cudaMemcpy(h->d_step, &s, sizeof(long long), cudaMemcpyHostToDevice));
+    if (h->rec.ctl) {               // a new state lifts the runaway guard; the frame count runs on
+        const long long none = -1;
+        CUDA_TRY(h, cudaMemcpy(h->rec.ctl + MD_REC_HALT, &none, sizeof(long long), cudaMemcpyHostToDevice));
+    }
+    return md_resync(h);
+}
+
+int vb_md_set_recorder(vb_handle* h, int64_t every, int64_t capacity, double runaway_factor) {
+    if (!h) return VB_ERR_ARG;
+    std::lock_guard<std::mutex> lk(h->mu);
+    if (int rc = md_check(h, "vb_md_set_recorder")) return rc;
+    if (every < 0 || (every > 0 && capacity < 1) || !std::isfinite(runaway_factor) || runaway_factor < 0.0) {
+        h->set_error("vb_md_set_recorder: bad arguments (every >= 0, capacity >= 1, runaway factor finite and >= 0)");
+        return VB_ERR_ARG;
+    }
+    const size_t n3 = 3 * (size_t)h->n_protein;
+    if (every > 0 && (size_t)capacity > ((size_t)1 << 34) / (16 * n3 + 32)) {
+        h->set_error("vb_md_set_recorder: a ring of %lld frames of %d atoms is too large", (long long)capacity, h->n_protein);
+        return VB_ERR_ARG;
+    }
+    CUDA_TRY(h, cudaSetDevice(h->device));
+    CUDA_TRY(h, cudaDeviceSynchronize());      // no enqueued step may still write the old ring
+    h->drop_graph();                           // the kicks and the frame copy hold the ring's pointers
+    h->free_rec();
+    if (int rc = md_resync(h)) return rc;
+    if (every == 0) return VB_OK;
+    const size_t C = (size_t)capacity;
+    size_t total = 0;
+    auto carve = [&](size_t bytes) { const size_t o = total; total += (bytes + 255) & ~(size_t)255; return o; };
+    const size_t o_ctl = carve(sizeof(long long) * MD_REC_CTL), o_step = carve(sizeof(long long) * C),
+                 o_epot = carve(sizeof(double) * C), o_ekin = carve(sizeof(double) * C), o_halt = carve(sizeof(int) * C),
+                 o_x = carve(sizeof(double) * C * n3), o_v = carve(sizeof(double) * C * n3);
+    CUDA_TRY(h, cudaMalloc(&h->rec_mem, total));
+    char* base = static_cast<char*>(h->rec_mem);
+    const long long ctl[MD_REC_CTL] = {0, -1};
+    CUDA_TRY(h, cudaMemcpy(base + o_ctl, ctl, sizeof(ctl), cudaMemcpyHostToDevice));
+    CUDA_TRY(h, cudaMemset(base + o_step, 0, o_x - o_step));     // scalars of unwritten slots read as zeros
+    MdRecorder& r = h->rec;
+    r.every = every; r.capacity = capacity; r.runaway_factor = runaway_factor;
+    r.ctl = reinterpret_cast<long long*>(base + o_ctl);
+    r.step = reinterpret_cast<long long*>(base + o_step);
+    r.epot = reinterpret_cast<double*>(base + o_epot);
+    r.ekin = reinterpret_cast<double*>(base + o_ekin);
+    r.halted = reinterpret_cast<int*>(base + o_halt);
+    r.x = reinterpret_cast<double*>(base + o_x);
+    r.v = reinterpret_cast<double*>(base + o_v);
+    h->rec_frames_enq = 0;
+    return VB_OK;
+}
+
+int vb_md_read_frames(vb_handle* h, int64_t first, int64_t n, int64_t* step_host, double* x_host, double* v_host,
+                      double* epot_host, double* ekin_host, int32_t* halted_host, void* stream) {
+    if (!h) return VB_ERR_ARG;
+    std::lock_guard<std::mutex> lk(h->mu);
+    if (int rc = md_check(h, "vb_md_read_frames", false)) return rc;
+    if (!h->rec.ctl) { h->set_error("vb_md_read_frames: the recorder is off (vb_md_set_recorder)"); return VB_ERR_STATE; }
+    const long long written = h->rec_frames_enq, C = h->rec.capacity;
+    if (first < 0 || n < 0 || first + n > written || first < written - C) {
+        h->set_error("vb_md_read_frames: frames [%lld, %lld) are not in the ring: %lld written or enqueued, the last %lld kept",
+                     (long long)first, (long long)(first + n), written, C);
+        return VB_ERR_ARG;
+    }
+    CUDA_TRY(h, cudaSetDevice(h->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t n3 = 3 * (size_t)h->n_protein;
+    // at most two contiguous runs of slots: up to the end of the ring, then from its start
+    for (long long done = 0; done < n;) {
+        const long long slot = (first + done) % C, len = std::min<long long>(n - done, C - slot);
+        auto copy = [&](void* dst, const void* src, size_t width) -> cudaError_t {
+            if (!dst) return cudaSuccess;
+            return cudaMemcpyAsync(static_cast<char*>(dst) + done * width, static_cast<const char*>(src) + slot * width,
+                                   len * width, cudaMemcpyDeviceToHost, st);
+        };
+        CUDA_TRY(h, copy(step_host, h->rec.step, sizeof(long long)));
+        CUDA_TRY(h, copy(x_host, h->rec.x, sizeof(double) * n3));
+        CUDA_TRY(h, copy(v_host, h->rec.v, sizeof(double) * n3));
+        CUDA_TRY(h, copy(epot_host, h->rec.epot, sizeof(double)));
+        CUDA_TRY(h, copy(ekin_host, h->rec.ekin, sizeof(double)));
+        CUDA_TRY(h, copy(halted_host, h->rec.halted, sizeof(int)));
+        done += len;
+    }
     return VB_OK;
 }
 
@@ -1401,6 +1506,7 @@ int vb_md_kick2(vb_handle* h, void* stream) {
     CUDA_TRY(h, cudaSetDevice(h->device));
     md_kick2_enqueue(h, (cudaStream_t)stream);
     CUDA_TRY(h, cudaGetLastError());
+    md_count_steps(h, 1);
     return VB_OK;
 }
 
@@ -1421,6 +1527,7 @@ int vb_md_run(vb_handle* h, int64_t n_steps, void* stream) {
             return (int)VB_OK;
         });
         if (rc != VB_OK) return rc;
+        md_count_steps(h, 1);
     }
     return VB_OK;
 }
@@ -1434,6 +1541,7 @@ int vb_md_get_state(vb_handle* h, double* x_host, double* v_host, int64_t* step_
     CUDA_TRY(h, cudaDeviceSynchronize());
     long long step = 0;
     CUDA_TRY(h, cudaMemcpy(&step, h->d_step, sizeof(long long), cudaMemcpyDeviceToHost));
+    if (int rc = md_resync(h)) return rc;
     if (x_host) CUDA_TRY(h, cudaMemcpy(x_host, h->d_mx, sizeof(double) * 3 * h->n_protein, cudaMemcpyDeviceToHost));
     if (v_host) CUDA_TRY(h, cudaMemcpy(v_host, h->d_mv, sizeof(double) * 3 * h->n_protein, cudaMemcpyDeviceToHost));
     if (step_out) *step_out = step;
@@ -1782,6 +1890,15 @@ int64_t vb_get_option(const vb_handle* h, const char* key) {
         int flag = 0;
         if (h->d_flags && cudaMemcpy(&flag, h->d_flags, sizeof(int), cudaMemcpyDeviceToHost) != cudaSuccess) return VB_ERR_CUDA;
         return flag;
+    }
+    if (k == "md_frames" || k == "md_halt_step") {
+        // frames the recorder has written / the step at which its runaway guard fired, -1 if none (synchronises)
+        long long v = k == "md_frames" ? 0 : -1;
+        if (h->rec.ctl && (cudaSetDevice(h->device) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess ||
+                           cudaMemcpy(&v, h->rec.ctl + (k == "md_frames" ? MD_REC_FRAMES : MD_REC_HALT), sizeof(v),
+                                      cudaMemcpyDeviceToHost) != cudaSuccess))
+            return VB_ERR_CUDA;
+        return v;
     }
     if (k == "timeline") return h->timeline;
     if (k == "tc_rows") return h->tc_rows;

@@ -8,6 +8,8 @@
 // State (positions, velocities) is fp64 like ASE's numpy arrays; forces arrive as the fp32 whole-protein buffer
 // [3*n_protein + 1] the signed fragment reduction writes.  Normals come from a counter-based Philox4x32-10 stream
 // keyed by (seed; step, component), so every rank of a sharded run draws identical numbers without communication.
+// An optional frame recorder (MdRecorder below) keeps every record step's state in a device ring and stops the
+// integration itself when the temperature runs away, so an observed run needs no host round trip per frame.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -52,6 +54,34 @@ __device__ inline void md_normals(const MdParams& p, long long step, int comp, d
     xi = r * co; eta = r * s;
 }
 
+// ---- frame recorder (vb_md_set_recorder / vb_md_read_frames) -------------------------------------------------------
+// The reference observes its run every --record-per-steps steps (MDObserver, src/utils/utils.py:114-166): it prints
+// Epot / Ekin / Etot, writes a trajectory frame and raises TemperatureRunawayError above 1.5 T0.  Here kick2 of a record
+// step (a step after which the counter is a multiple of `every`) sums Ekin in a fixed order, decides the runaway, and
+// writes the frame -- its scalars, and x and v copied by the threads that own those components -- into ring slot
+// frame % capacity.  The copy lives in kick2 rather than in a launch of its own: kick2 already holds v, x is final since
+// kick1, and a separate grid would add a launch to every step to move 8 KB (Chignolin) on a few of them.  Once the
+// runaway guard fires, kick1 and kick2 leave the state and the ring alone, so the device stays at the halting step
+// (whose frame is kept) however many steps are still enqueued behind it.  With the recorder off every pointer is null
+// and the kernels do exactly what they do without it.
+constexpr double MD_KB = 8.617330337217213e-05;     // eV / K, as ai2bmd_b200/md.py KB
+enum { MD_REC_FRAMES = 0, MD_REC_HALT = 1, MD_REC_CTL = 2 };
+struct MdRecorder {
+    long long every = 0, capacity = 0;
+    double runaway_factor = 0.0;   // > 0: halt when T > runaway_factor * T0, T0 = kT / k_B
+    // ctl[MD_REC_FRAMES]  frames written so far (frame f lives in slot f % capacity)
+    // ctl[MD_REC_HALT]    -1, or the step at which the guard fired
+    long long* ctl = nullptr;
+    long long* step = nullptr;     // per slot
+    double* epot = nullptr;        // per slot: restrained potential energy, ef[3n] + rf[3n]
+    double* ekin = nullptr;        // per slot: sum m v^2 / 2 after the centre-of-mass velocity removal
+    int* halted = nullptr;         // per slot: 1 on the frame whose temperature fired the guard
+    double* x = nullptr;           // [capacity][3 * n_protein]
+    double* v = nullptr;           // [capacity][3 * n_protein]
+};
+
+__device__ inline bool md_halted(const long long* ctl) { return ctl != nullptr && ctl[MD_REC_HALT] >= 0; }
+
 // Langevin coefficients of one atom (ase/md/langevin.py updatevars; md.py Langevin.__init__)
 struct MdCoef { double c1, c2, c3, c4, c5; };
 __device__ inline MdCoef md_coef(const MdParams& p, double mass) {
@@ -73,8 +103,10 @@ constexpr int MD_K1_THREADS = 1024;
 __global__ void __launch_bounds__(MD_K1_THREADS) md_kick1_kernel(MdParams p, const long long* __restrict__ step_ctr,
                                                                  const double* __restrict__ mass, const float* __restrict__ ef,
                                                                  const double* __restrict__ rf,
-                                                                 double* __restrict__ x, double* __restrict__ v) {
+                                                                 double* __restrict__ x, double* __restrict__ v,
+                                                                 const long long* __restrict__ rec_ctl) {
     __shared__ double shift[3];
+    if (md_halted(rec_ctl)) return;
     const int n3 = 3 * p.n_protein;
     const long long step = *step_ctr;
     const bool fixcm = p.fr > 0.0;
@@ -210,16 +242,19 @@ __global__ void md_place_kernel(int n_atoms, const int* __restrict__ real, const
     pos[3 * a] = (float)px; pos[3 * a + 1] = (float)py; pos[3 * a + 2] = (float)pz;
 }
 
-// second half-kick (+ centre-of-mass velocity removal when friction > 0, as md.py does) and step counter advance.
-// One CTA: the momentum sum is reduced in a fixed order.
+// second half-kick (+ centre-of-mass velocity removal when friction > 0, as md.py does) and step counter advance; on
+// record steps also the frame and the runaway guard.  One CTA: the momentum and kinetic-energy sums are
+// reduced in a fixed order, so they are bit-reproducible for the same v.
 constexpr int MD_K2_THREADS = 1024;
 __global__ void __launch_bounds__(MD_K2_THREADS) md_kick2_kernel(MdParams p, long long* __restrict__ step_ctr,
                                                                  const double* __restrict__ mass, const float* __restrict__ ef,
                                                                  const double* __restrict__ rf,
-                                                                 double* __restrict__ v, double* __restrict__ epot_hist,
-                                                                 long long hist_cap) {
+                                                                 const double* __restrict__ x, double* __restrict__ v,
+                                                                 double* __restrict__ epot_hist, long long hist_cap,
+                                                                 MdRecorder rec) {
     __shared__ double red[3][MD_K2_THREADS / 32];
     __shared__ double com[3];
+    if (md_halted(rec.ctl)) return;
     const long long step = *step_ctr;
     const int n3 = 3 * p.n_protein;
     for (int comp = threadIdx.x; comp < n3; comp += MD_K2_THREADS) {
@@ -262,9 +297,47 @@ __global__ void __launch_bounds__(MD_K2_THREADS) md_kick2_kernel(MdParams p, lon
         __syncthreads();
         for (int comp = threadIdx.x; comp < n3; comp += MD_K2_THREADS) v[comp] -= com[comp % 3] / mtot;
     }
+    // record step: the frame's x and v, and Ekin = sum m v^2 / 2 of the final velocities.  Each thread copies and sums
+    // only the components it wrote itself; warp shuffles, then the warp partials summed serially (the momentum
+    // reduction's pattern).  Every thread reads the frame count before the barrier, thread 0 advances it after.
+    const bool record = rec.ctl != nullptr && (step + 1) % rec.every == 0;
+    __shared__ double redk[MD_K2_THREADS / 32];
+    long long frame = 0;
+    if (record) {
+        frame = rec.ctl[MD_REC_FRAMES];
+        double* __restrict__ fx = rec.x + (frame % rec.capacity) * n3;
+        double* __restrict__ fv = rec.v + (frame % rec.capacity) * n3;
+        double e = 0.0;
+        for (int comp = threadIdx.x; comp < n3; comp += MD_K2_THREADS) {
+            const double vv = v[comp];
+            fx[comp] = x[comp];
+            fv[comp] = vv;
+            e += mass[comp / 3] * (vv * vv);
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) e += __shfl_xor_sync(0xffffffffu, e, o);
+        if ((threadIdx.x & 31) == 0) redk[threadIdx.x >> 5] = e;
+        __syncthreads();
+    }
     if (threadIdx.x == 0) {
         // with restraints, the restrained potential energy (ASE get_potential_energy(apply_constraint=True))
-        if (epot_hist != nullptr && hist_cap > 0) epot_hist[step % hist_cap] = (double)ef[n3] + (rf != nullptr ? rf[n3] : 0.0);
+        const double epot = (double)ef[n3] + (rf != nullptr ? rf[n3] : 0.0);
+        if (epot_hist != nullptr && hist_cap > 0) epot_hist[step % hist_cap] = epot;
+        if (record) {
+            double s = 0.0;
+            for (int w = 0; w < MD_K2_THREADS / 32; w++) s += redk[w];
+            const double ekin = 0.5 * s;
+            // md.py DeviceLangevin.temperature: T = 2 Ekin / (3 n k_B); the reference raises above 1.5 T0
+            const double temp = 2.0 * ekin / (3.0 * p.n_protein) / MD_KB;
+            const bool runaway = rec.runaway_factor > 0.0 && temp > rec.runaway_factor * p.kT / MD_KB;
+            const long long slot = frame % rec.capacity;
+            rec.step[slot] = step + 1;
+            rec.epot[slot] = epot;
+            rec.ekin[slot] = ekin;
+            rec.halted[slot] = runaway ? 1 : 0;
+            rec.ctl[MD_REC_FRAMES] = frame + 1;
+            if (runaway) rec.ctl[MD_REC_HALT] = step + 1;
+        }
         *step_ctr = step + 1;
     }
 }

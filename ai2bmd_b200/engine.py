@@ -40,7 +40,7 @@ EXPORTED_SYMBOLS = [
     "vb_forward_host", "vb_set_protein_map", "vb_forward_protein", "vb_get_edges", "vb_launches_per_forward",
     "vb_set_option", "vb_get_option", "vb_num_stages", "vb_stage_name", "vb_stage_kernel", "vb_debug_run", "vb_debug_read", "vb_profile_stages", "vb_tc_selftest", "vb_tc_selftest_rows",
     "vb_md_setup", "vb_md_set_normals", "vb_md_set_state", "vb_md_kick1", "vb_md_eval", "vb_md_kick2", "vb_md_run", "vb_md_get_state",
-    "vb_md_set_restraints",
+    "vb_md_set_restraints", "vb_md_set_recorder", "vb_md_read_frames",
     "vb_set_nonbonded", "vb_nonbonded",
     "vb_comm_init", "vb_comm_connect", "vb_comm_allreduce",
     "vb_set_caph", "vb_caph_relax",
@@ -113,6 +113,10 @@ def load_library(path: Optional[str] = None):
     lib.vb_md_run.argtypes = [vp, i64, vp]
     lib.vb_md_set_restraints.restype = C.c_int
     lib.vb_md_set_restraints.argtypes = [vp, i64, vp, C.c_double, i64, vp, vp, vp]
+    lib.vb_md_set_recorder.restype = C.c_int
+    lib.vb_md_set_recorder.argtypes = [vp, i64, i64, C.c_double]
+    lib.vb_md_read_frames.restype = C.c_int
+    lib.vb_md_read_frames.argtypes = [vp, i64, i64, vp, vp, vp, vp, vp, vp, vp]
     lib.vb_set_nonbonded.restype = C.c_int
     lib.vb_set_nonbonded.argtypes = [vp, i64, vp, vp, vp, vp, vp, i64, i64]
     lib.vb_nonbonded.restype = C.c_int
@@ -329,6 +333,28 @@ class Engine:
                                                   len(ij), ij.ctypes.data if len(ij) else None,
                                                   sk.ctypes.data if len(sk) else None, sr.ctypes.data if len(sr) else None),
                     "vb_md_set_restraints")
+
+    def md_set_recorder(self, every: int, capacity: int = 0, runaway_factor: float = 0.0):
+        """Frame ring of ``capacity`` frames, one after every step whose counter ends a multiple of ``every``, with the
+        runaway guard at ``runaway_factor`` x T0 (0: no guard); ``every = 0`` turns it off (vb_md_set_recorder)."""
+        self._check(self.lib.vb_md_set_recorder(self.h, int(every), int(capacity), float(runaway_factor)),
+                    "vb_md_set_recorder")
+
+    def md_read_frames_async(self, first: int, n: int, step_ptr, x_ptr, v_ptr, epot_ptr, ekin_ptr, halted_ptr,
+                             stream_ptr: int = 0):
+        """Frames [first, first + n) into host buffers (raw pointers, pinned by the caller, any may be None) as
+        asynchronous copies on ``stream_ptr``."""
+        self._check(self.lib.vb_md_read_frames(self.h, int(first), int(n), step_ptr, x_ptr, v_ptr, epot_ptr, ekin_ptr,
+                                               halted_ptr, stream_ptr), "vb_md_read_frames")
+
+    def md_read_frames(self, first: int, n: int):
+        """Frames [first, first + n) as numpy arrays: dict of step [n], x [n, P, 3], v [n, P, 3], epot [n], ekin [n],
+        halted [n]; synchronises the device."""
+        out = dict(step=np.empty(n, np.int64), x=np.empty((n, self._md_n, 3)), v=np.empty((n, self._md_n, 3)),
+                   epot=np.empty(n), ekin=np.empty(n), halted=np.empty(n, np.int32))
+        self.md_read_frames_async(first, n, *(out[k].ctypes.data for k in ("step", "x", "v", "epot", "ekin", "halted")))
+        self.get_option("md_frames")                  # a device synchronisation
+        return out
 
     def md_restraint_forces(self) -> np.ndarray:
         """The restraint buffer rf [3*n_protein + 1] (fp64 forces, then the energy) of the last evaluation; synchronises."""

@@ -176,9 +176,11 @@ class DeviceLangevin:
 
     def __init__(self, state_dict, frags: FragmentData, pm: ProteinMap, recipe: FragmentRecipe, positions, numbers,
                  dt_fs=1.0, temperature_K=300.0, friction_per_fs=0.001, seed=0, device: int = 0, velocities=None,
-                 group=None, engine: Engine = None, zero_com_momentum=False, caph=None):
+                 group=None, engine: Engine = None, zero_com_momentum=False, caph=None, step: int = 0):
         """``caph``: an :class:`ai2bmd_b200.caph.CapHProblem` -- the added hydrogens are then refined every step on the
-        device (one LBFGS call on the Amber terms, ``csrc/k_caph.cuh``) between their placement and the evaluation."""
+        device (one LBFGS call on the Amber terms, ``csrc/k_caph.cuh``) between their placement and the evaluation.
+        ``step``: the step counter to start from; with ``positions`` / ``velocities`` of a frame that ``run_observed``
+        recorded at step s, the run continues with the random numbers the original run drew after s."""
         import torch
         self.torch, self.group = torch, group
         self.n = pm.n_protein
@@ -206,8 +208,10 @@ class DeviceLangevin:
             velocities = rng.standard_normal(x.shape) * np.sqrt(self.kT / m)
             if zero_com_momentum:
                 velocities -= (velocities * m).sum(0) / m.sum()
-        engine.md_set_state(x, velocities, 0)
+        engine.md_set_state(x, velocities, step)
         self._eval()
+        self._copy_stream = None
+        self._frame_bufs = {}
 
     @property
     def _native_comm(self):
@@ -265,28 +269,65 @@ class DeviceLangevin:
         self.engine.md_set_restraints(() if tether_atoms is None else tether_atoms, tether_k_kcal * KCALMOL_EV, ij, k, rt)
 
     def run_observed(self, n_steps: int, record_per_steps=None, observer=None):
-        """``run(n_steps)`` in blocks that end at every step number divisible by ``record_per_steps``; there, like the
-        reference's ``MDObserver.printenergy`` (utils.py:143-159), the temperature is checked -- above 1.5 T0 raises
-        :class:`TemperatureRunawayError` -- and ``observer(step, x, v, epot, ekin)`` is called with the restrained
-        potential energy of that step."""
+        """``run(n_steps)`` observed at every step number divisible by ``record_per_steps``: there, like the reference's
+        ``MDObserver.printenergy`` (utils.py:143-159), the temperature is checked -- above 1.5 T0 raises
+        :class:`TemperatureRunawayError` -- and ``observer(step, x, v, epot, ekin)`` is called, in step order, with the
+        restrained potential energy of that step.
+
+        The device records the frames and makes the runaway decision itself (``vb_md_set_recorder``); this loop only
+        drains them.  It keeps at most ``max(2 record_per_steps, 64)`` steps enqueued beyond the last frame it handed to
+        the observer, in blocks that each end with one asynchronous copy of their frames into pinned memory on a side
+        stream, so the GPU steps on while the observer runs.  On a runaway the device stops at the halting step by
+        itself, the observer is not called for it, and the engine stays halted (``state()`` is that step, ``run`` changes
+        nothing) until ``engine.md_set_state``; otherwise the recorder is switched off again at the end."""
         if not record_per_steps:
             self.run(n_steps)
             return
+        torch, k = self.torch, int(record_per_steps)
         _, _, step, _ = self.state()
         end = step + n_steps
-        while step < end:
-            nxt = min(end, (step // record_per_steps + 1) * record_per_steps)
-            self.run(nxt - step)
-            step = nxt
-            if step % record_per_steps:
-                continue
-            x, v, _, hist = self.state(n_hist=1)
-            ekin = 0.5 * float((self.masses[:, None] * v * v).sum())
-            temp = 2.0 * ekin / (3 * self.n) / KB
-            if temp > 1.5 * self.kT / KB:
-                raise TemperatureRunawayError(f"temperature runaway at step {step}: {temp:.1f} K")
-            if observer is not None:
-                observer(step, x, v, float(hist[0]), ekin)
+        ahead = max(2 * k, 64)                       # steps enqueued beyond the last drained block, at most
+        block = max(k, ahead // 2 // k * k)          # blocks end at multiples of `block` (itself a multiple of k) and at `end`
+        # a block's frames are copied out before the lookahead lets later steps reuse their slots
+        self.engine.md_set_recorder(k, (ahead + block) // k + 2, RUNAWAY_FACTOR)
+        if self._copy_stream is None:
+            self._copy_stream = torch.cuda.Stream(self.ef.device)
+        copy, free = self._copy_stream, self._frame_bufs.setdefault(block // k, [])
+        inflight, frame, enq, drained, halted = [], 0, step, step, False
+        try:
+            while drained < end:
+                while enq < end and (not inflight or min(end, (enq // block + 1) * block) - drained <= ahead):
+                    nxt = min(end, (enq // block + 1) * block)
+                    self.run(nxt - enq)
+                    nf = nxt // k - enq // k
+                    enq = nxt
+                    buf = free.pop() if free else _FrameBuffers(torch, block // k, self.n)
+                    ran = torch.cuda.Event()
+                    ran.record(self.stream)
+                    copy.wait_event(ran)
+                    if nf:
+                        self.engine.md_read_frames_async(frame, nf, *buf.ptrs, copy.cuda_stream)
+                    copied = torch.cuda.Event()
+                    copied.record(copy)
+                    inflight.append((copied, nf, nxt, buf))
+                    frame += nf
+                copied, nf, nxt, buf = inflight.pop(0)
+                copied.synchronize()
+                for i in range(nf):
+                    if buf.halted[i]:
+                        temp = 2.0 * buf.ekin[i] / (3 * self.n) / KB
+                        halted = True
+                        raise TemperatureRunawayError(f"temperature runaway at step {int(buf.step[i])}: {temp:.1f} K")
+                    if observer is not None:
+                        x, v = buf.x[i].copy(), buf.v[i].copy()
+                        observer(int(buf.step[i]), x, v, float(buf.epot[i]), 0.5 * float((self.masses[:, None] * v * v).sum()))
+                drained = nxt
+                free.append(buf)
+        finally:
+            copy.synchronize()                       # no copy may still write a buffer that goes back to the pool
+            free.extend(b for _, _, _, b in inflight)
+            if not halted:
+                self.engine.md_set_recorder(0)
 
     def preequilibrate(self, steps_per_stage: int, schedule=PREEQ_SCHEDULE, atoms=None, record_per_steps=None, observer=None):
         """The reference's pre-equilibration: for each force constant of ``schedule`` (kcal/mol/A^2, the reference's
@@ -300,6 +341,22 @@ class DeviceLangevin:
                 self.run_observed(steps_per_stage, record_per_steps, observer)
             finally:
                 self.set_restraints()
+
+
+class _FrameBuffers:
+    """Pinned host buffers for ``n_frames`` recorder frames (``vb_md_read_frames``) and numpy views of them."""
+
+    def __init__(self, torch, n_frames: int, n_atoms: int):
+        f64, pin = torch.float64, dict(pin_memory=True)
+        t = [torch.empty(n_frames, dtype=torch.int64, **pin), torch.empty((n_frames, n_atoms, 3), dtype=f64, **pin),
+             torch.empty((n_frames, n_atoms, 3), dtype=f64, **pin), torch.empty(n_frames, dtype=f64, **pin),
+             torch.empty(n_frames, dtype=f64, **pin), torch.empty(n_frames, dtype=torch.int32, **pin)]
+        self._keep = t
+        self.ptrs = [a.data_ptr() for a in t]
+        self.step, self.x, self.v, self.epot, self.ekin, self.halted = (a.numpy() for a in t)
+
+
+RUNAWAY_FACTOR = 1.5        # the reference's guard: T > 1.5 T0 (src/utils/utils.py:154)
 
 
 class TemperatureRunawayError(RuntimeError):

@@ -103,6 +103,8 @@ int vb_md_setup(vb_handle* h, int64_t n_protein_atoms, const double* masses_host
 /* Optional externally supplied normals, device array [pool_steps][2][3*n_protein] (xi, eta), step s reads row
  * s % pool_steps; (NULL, 0) returns to Philox.  For parity tests against a host integrator. */
 int vb_md_set_normals(vb_handle* h, const double* pool_dev, int64_t pool_steps);
+/* Positions, velocities and the step counter (the normals of step s follow from (seed, s) alone, so a run restarted from
+ * a recorded frame draws the random stream the original run drew); synchronises and lifts a halt of the frame recorder. */
 int vb_md_set_state(vb_handle* h, const double* x_host, const double* v_host, int64_t step);
 /* The three phases, asynchronous on `stream`.  With several GPUs every rank holds the whole-protein state and its
  * own shard of fragments: kick1; eval; all-reduce ef_prot_dev (NCCL sum, by the caller); kick2. */
@@ -129,6 +131,23 @@ int vb_md_run(vb_handle* h, int64_t n_steps, void* stream);
  * energies recorded at the end of the last n_hist steps (oldest first). */
 int vb_md_get_state(vb_handle* h, double* x_host, double* v_host, int64_t* step_out, double* epot_hist_host,
                     int64_t n_hist);
+/* Frame recorder: the reference's observed run (MDObserver, src/utils/utils.py:114-166, attached every
+ * --record-per-steps steps at src/AIMD/simulator.py:125-137) without a host round trip per frame.  After every step whose
+ * counter ends a multiple of `every`, the step itself writes a frame into a device ring of `capacity` slots: the step,
+ * the restrained Epot (as the energy history), Ekin = sum m v^2 / 2 (fixed-order sum), a halt mark, and x, v [3n] fp64.
+ * With runaway_factor > 0 the frame's temperature T = 2 Ekin / (3 n k_B) is checked against runaway_factor * T0,
+ * T0 = kT / k_B of vb_md_setup; above it the frame is marked halted and the device stops integrating: every later step
+ * leaves x, v, the counter and the ring as they are, until vb_md_set_state (which lifts the halt) or vb_md_set_recorder.
+ * Synchronises; resets the frame count and the halt; drops the cached step graphs.  every = 0 turns the recorder off and
+ * frees the ring (the step is then exactly the one without it).  vb_md_kick2 records too, so the sharded phase-by-phase
+ * path writes the same frames.  "md_frames" / "md_halt_step" of vb_get_option read the device counters. */
+int vb_md_set_recorder(vb_handle* h, int64_t every, int64_t capacity, double runaway_factor);
+/* Frames [first, first + n) (frame f = the f-th record step since vb_md_set_recorder) into host arrays step[n],
+ * x[n][3n], v[n][3n], epot[n], ekin[n], halted[n] -- any may be NULL -- as asynchronous copies on `stream`; the caller
+ * pins the buffers and waits for the stream.  VB_ERR_ARG for frames overwritten or not yet enqueued, as far as the host
+ * knows (frames behind a halt are never written: read up to the first halted frame). */
+int vb_md_read_frames(vb_handle* h, int64_t first, int64_t n, int64_t* step_host, double* x_host, double* v_host,
+                      double* epot_host, double* ekin_host, int32_t* halted_host, void* stream);
 
 /* ---- Non-bonded MM term (SURVEY section 8f, rank 2) ---------------------------------------------------------------
  * All ordered pairs (src j, dst i), j != i, except pairs listed in the exclusion table (atoms sharing a dipeptide,
@@ -207,7 +226,8 @@ int vb_launches_per_forward(const vb_handle* h);
  * their 10 s deadline; once nonzero, vb_comm_allreduce and every vb_md_* call but vb_md_setup and vb_md_get_state fail
  * with VB_ERR_STATE), "comm_seq" (all-reduces completed since vb_comm_init: the window parity of the next one is its
  * parity plus one),
- * "caph_ready" and "caph_evals" (energy evaluations of the last hydrogen refinement). */
+ * "caph_ready" and "caph_evals" (energy evaluations of the last hydrogen refinement), "md_frames" (frames the recorder
+ * has written) and "md_halt_step" (-1, or the step at which its runaway guard fired); both synchronise. */
 int vb_set_option(vb_handle* h, const char* key, int64_t value);
 int64_t vb_get_option(const vb_handle* h, const char* key);   /* resolved value (after vb_set_topology) */
 
