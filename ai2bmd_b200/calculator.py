@@ -22,7 +22,7 @@ import numpy as np
 
 from .engine import Engine
 from .fragment_data import FragmentData
-from .weights import load_state_dict
+from .weights import load_checkpoint, resolve_derivative
 
 
 def _device_index(device: str) -> int:
@@ -34,26 +34,39 @@ def _device_index(device: str) -> int:
 
 
 class ViSNetModel:
-    """Energy and forces of a packed fragment batch with the ViSNet potential on one H100."""
+    """Energy and forces of a packed fragment batch with the ViSNet potential on one H100.
+
+    ``derivative=False`` is the reference's ``ViSNet(derivative=False)``: energies only, on a forward-only engine
+    (``dl_potential_loader`` returns ``(e, None)``)."""
 
     implemented_properties = ["energy", "forces"]
 
-    def __init__(self, state_dict: Dict[str, np.ndarray], device: str = "cuda:0"):
+    def __init__(self, state_dict: Dict[str, np.ndarray], device: str = "cuda:0", derivative: bool = True):
         self.device = device
-        self.engine = Engine(state_dict, _device_index(device))
+        self.derivative = bool(derivative)
+        self.engine = Engine(state_dict, _device_index(device), derivative=self.derivative)
         self._topo_key = None
+        if not self.derivative:
+            self.implemented_properties = ["energy"]
 
     @classmethod
     def from_file(cls, **kwargs):
+        """``from_file(model_path=..., device=..., derivative=None)``: ``derivative`` follows the reference's
+        ``load_model(path, derivative=...)`` -- the checkpoint's hyper-parameter unless given (an ``.npz`` counts as True)."""
         if "model_path" not in kwargs:
             raise ValueError("model_path must be provided")
-        return cls(load_state_dict(kwargs["model_path"]), device=kwargs.get("device", "cuda:0"))
+        sd, ckpt_derivative = load_checkpoint(kwargs["model_path"])
+        return cls(sd, device=kwargs.get("device", "cuda:0"),
+                   derivative=resolve_derivative(ckpt_derivative, kwargs.get("derivative")))
 
     @classmethod
     def from_engine(cls, engine: Engine, device: str, frag: FragmentData):
         """Wrap an engine whose topology is already ``frag``'s (e.g. a shard's engine with its protein map set)."""
         self = cls.__new__(cls)
         self.device, self.engine = device, engine
+        self.derivative = engine.derivative
+        if not self.derivative:
+            self.implemented_properties = ["energy"]
         self._topo_key = self._key(frag)[0]
         self._calibrated = True
         return self
@@ -79,10 +92,14 @@ class ViSNetModel:
                   and not frag.z.flags.writeable and not frag.batch.flags.writeable)
         self._topo_arrays = (frag.z, frag.batch) if frozen else None
 
-    def dl_potential_loader(self, frag_data: FragmentData) -> Tuple[np.ndarray, np.ndarray]:
-        """``FragmentData -> (e[G,1] float32 eV, f[N,3] float32 eV/A)`` as numpy arrays."""
+    def dl_potential_loader(self, frag_data: FragmentData) -> Tuple[np.ndarray, Optional[np.ndarray]]:
+        """``FragmentData -> (e[G,1] float32 eV, f[N,3] float32 eV/A)`` as numpy arrays; ``f`` is None on a
+        ``derivative=False`` model (``visnet.py:166``)."""
         self._ensure_topology(frag_data)
-        e, f = self.engine.forward_host(frag_data.pos)
+        if self.derivative:
+            e, f = self.engine.forward_host(frag_data.pos)
+        else:
+            e, f = self.engine.energy_host(frag_data.pos), None
         if not getattr(self, "_calibrated", True):      # once per topology: tile length from the real edge count
             self.engine.set_option("calibrate", 1)
             self._calibrated = True
@@ -92,12 +109,12 @@ class ViSNetModel:
 _local_calc: Dict[str, ViSNetModel] = {}
 
 
-def get_visnet_model(model_path: str, device: str) -> ViSNetModel:
-    """One engine per (device, checkpoint); the reference's sub-process proxies
+def get_visnet_model(model_path: str, device: str, derivative: Optional[bool] = None) -> ViSNetModel:
+    """One engine per (device, checkpoint[, derivative]); the reference's sub-process proxies
     (``ViSNetAsyncModel``) are unnecessary because every engine is in-process and asynchronous."""
-    signature = f"{device}-{model_path}"
+    signature = f"{device}-{model_path}" if derivative is None else f"{device}-{model_path}-derivative={bool(derivative)}"
     if signature not in _local_calc:
-        _local_calc[signature] = ViSNetModel.from_file(model_path=model_path, device=device)
+        _local_calc[signature] = ViSNetModel.from_file(model_path=model_path, device=device, derivative=derivative)
     return _local_calc[signature]
 
 
@@ -130,23 +147,28 @@ class _CalculatorBase:
 
 
 class ViSNetCalculator(_CalculatorBase):
-    """Feed the input through the ViSNet model without fragmentation (one graph)."""
+    """Feed the input through the ViSNet model without fragmentation (one graph).
 
-    def __init__(self, ckpt_path: str, ckpt_type: str, device: str = "cuda:0", is_root_calc=True, **kwargs):
+    ``derivative`` as in :meth:`ViSNetModel.from_file`; with ``derivative=False`` the calculator serves
+    ``get_potential_energy`` only and ``get_forces`` raises ``NotImplementedError``."""
+
+    def __init__(self, ckpt_path: str, ckpt_type: str, device: str = "cuda:0", is_root_calc=True,
+                 derivative: Optional[bool] = None, **kwargs):
         super().__init__()
         self.ckpt_path, self.ckpt_type, self.is_root_calc = ckpt_path, ckpt_type, is_root_calc
         model_path = osp.join(ckpt_path, f"visnet-uni-{ckpt_type}.ckpt")
         if not osp.exists(model_path) and osp.exists(ckpt_path) and osp.isfile(ckpt_path):
             model_path = ckpt_path
         self.device = device
-        self.model = get_visnet_model(model_path, device)
+        self.model = get_visnet_model(model_path, device, derivative)
+        self.implemented_properties = list(self.model.implemented_properties)
 
     def calculate(self, atoms, properties, system_changes):
         n = len(atoms.numbers)
         data = FragmentData(np.asarray(atoms.numbers), np.asarray(atoms.positions).astype(np.float32),
                             np.array([0], dtype=int), np.array([n], dtype=int), np.zeros((n,), dtype=int))
         e, f = self.model.dl_potential_loader(data)
-        self.results = {"energy": e, "forces": f}
+        self.results = {"energy": e} if f is None else {"energy": e, "forces": f}
 
 
 class DipeptideBondedCombiner:
@@ -174,6 +196,8 @@ class DLBondedCalculator:
     def __init__(self, ckpt_path: str, ckpt_type: str = "", device: str = "cuda:0", **kwargs):
         model_path = osp.join(ckpt_path, f"visnet-uni-{ckpt_type}.ckpt") if ckpt_type else ckpt_path
         self.models = [get_visnet_model(model_path, device)]
+        if not self.models[0].derivative:
+            raise ValueError(f"{model_path}: the bonded calculator needs forces, and the checkpoint has derivative=False")
         self.combiner = DipeptideBondedCombiner()
 
     def calculate(self, fragments: FragmentData):

@@ -135,10 +135,10 @@ struct vb_handle {
     char* arena = nullptr;
     size_t arena_bytes = 0;
     float* d_pos = nullptr;      // [N][3]
-    float* d_energy = nullptr;   // [G]
+    float* d_energy = nullptr;   // [G] (right after the forces with derivative = 1)
     unsigned long long* d_tl = nullptr;   // optional in-kernel timelines [4L+2][TC_TL_SLOTS]: edge fwd l, edge bwd L+l, node fwd 2L+k, node bwd 3L+1+k
     int timeline = 0;
-    float* d_forces = nullptr;   // [N][3]
+    float* d_forces = nullptr;   // [N][3] (none with derivative = 0)
     float *h_pos = nullptr, *h_energy = nullptr, *h_forces = nullptr;   // pinned staging
     cudaStream_t own_stream = nullptr;
     // protein map, as a CSR over protein (destination) atoms: entries of atom p are map_rowptr[p]..map_rowptr[p+1]
@@ -169,6 +169,7 @@ struct vb_handle {
     int node_tc = 0, node_tc_opt = -1;   // 1: node stage on tensor cores (k_node_tc.cuh); -1 = choose by problem size
     int embed_batch_opt = -1;            // embedding kernels: several nodes per CTA (1), one (0), by size (-1)
     int edge_tc = -1;  // bit 0: forward edge stage on tensor cores, bit 1: adjoint edge stage on tensor cores; -1 = by size
+    int derivative = 1;  // 0: forward-only workspace, energies only (the energy plan); read by vb_set_topology
     // graph cache: one instantiated graph per (kind, I/O pointer set); pointers are baked into the captured launches
     struct GraphEntry { int kind; StepIO io; cudaGraphExec_t exec; };
     std::vector<GraphEntry> graphs;
@@ -252,6 +253,21 @@ struct vb_handle {
         d_mx = d_mv = d_mmass = d_ehist = nullptr; d_real = d_acc = d_rem = nullptr; d_blen = nullptr; d_step = nullptr;
         md_ready = false;
     }
+    // drop the topology and everything sized by it (the caller has selected the device)
+    void clear_topology() {
+        drop_graph();
+        free_md();                 // the MD recipe indexes the fragment atoms of the old topology
+        free_map();                // ... and so does the protein map: it must be set again
+        free_caph();               // ... and the hydrogen-refinement terms
+        has_topology = false;
+        cudaFree(arena); arena = nullptr; arena_bytes = 0;
+        d_pos = d_energy = d_forces = nullptr;
+        cudaFreeHost(h_pos); cudaFreeHost(h_forces);
+        h_pos = h_energy = h_forces = nullptr;
+        ws = Workspace{};
+        edges_plan = 0;
+        stage_names.clear(); stage_kernels.clear(); launches = 0;
+    }
 };
 
 namespace {
@@ -315,6 +331,46 @@ void carve(ArenaPlan& plan, char* base, T*& ptr, size_t count) {
     ptr = base ? reinterpret_cast<T*>(base + o) : nullptr;
 }
 
+// Forward-only workspace (option "derivative" = 0): the energy plan reads a per-layer buffer only at layer l and l - 1
+// (node stage k: layers k - 1 and k; edge stage l: F[l] -> F[l + 1]; the head: X[L], V[L]), so layer l lives in slot
+// l % 2 of two.  Except layer 0 of V, V123 and TU: the plan reads them without writing them (the vector features entering
+// layer 0 are zero, the tensor-core node stage does not compute V123[0] / TU[0]), so they keep a zeroed slot of their own
+// that no later layer overwrites.  The edge pre-activations P1 / SP / ATT, which only the adjoint reads, get one scratch
+// slot that every layer writes over: the tensor-core edge kernels store them unconditionally, because a runtime null
+// check on those stores costs the 64-row warp-specialised forward 52 B of spill stores at its 128-register budget.
+template <typename T>
+void carve_layers(ArenaPlan& plan, char* base, T** ptr, int layers, size_t count, bool own_zero_layer) {
+    T* slot[3] = {};
+    for (int s = 0; s < (own_zero_layer ? 3 : 2); s++) carve(plan, base, slot[s], count);
+    for (int l = 0; l < layers; l++) ptr[l] = (own_zero_layer && l == 0) ? slot[2] : slot[l % 2];
+}
+
+void layout_energy_workspace(vb_handle* h, char* base, ArenaPlan& plan) {
+    Workspace& ws = h->ws;
+    const size_t N = ws.N, G = ws.G, E = ws.Ecap;
+    carve_layers(plan, base, ws.X, L + 1, N * D, false);
+    carve_layers(plan, base, ws.V, L + 1, N * 3 * D, true);
+    carve_layers(plan, base, ws.F, L, E * D, false);
+    carve_layers(plan, base, ws.VN, L, N * 3 * D, false);
+    carve_layers(plan, base, ws.QKV, L, N * 3 * D, false);
+    carve_layers(plan, base, ws.V123, L, N * 9 * D, true);
+    carve_layers(plan, base, ws.VDOT, L, N * D, false);
+    carve_layers(plan, base, ws.TU, L, N * 6 * D, true);
+    carve_layers(plan, base, ws.O, L, N * 3 * D, false);
+    float *p1 = nullptr, *sp = nullptr, *att = nullptr;
+    carve(plan, base, p1, E * 3 * D);
+    carve(plan, base, sp, E * 2 * D);
+    carve(plan, base, att, E * H);
+    for (int l = 0; l < L; l++) { ws.P1[l] = p1; ws.SP[l] = sp; ws.ATT[l] = att; }
+    carve(plan, base, ws.XA, N * D);
+    carve(plan, base, ws.VA, N * 3 * D);
+    carve(plan, base, ws.XN, N * D);
+    carve(plan, base, ws.eatom, N);
+    carve(plan, base, h->d_pos, N * 3);
+    carve(plan, base, h->d_energy, G);
+    h->d_forces = nullptr;
+}
+
 void layout_workspace(vb_handle* h, char* base, ArenaPlan& plan, int*& z, int*& frag_of, int*& frag_start) {
     Workspace& ws = h->ws;
     const size_t N = ws.N, G = ws.G, E = ws.Ecap;
@@ -328,6 +384,7 @@ void layout_workspace(vb_handle* h, char* base, ArenaPlan& plan, int*& z, int*& 
     carve(plan, base, ws.edst, E);
     carve(plan, base, ws.geom, E * 8);
     carve(plan, base, ws.rbf, E * NR);
+    if (!h->derivative) { layout_energy_workspace(h, base, plan); return; }
     carve(plan, base, ws.eacc, E * 4);
     carve(plan, base, ws.grbf, E * NR);
     for (int l = 0; l <= L; l++) { carve(plan, base, ws.X[l], N * D); carve(plan, base, ws.V[l], N * 3 * D); }
@@ -665,8 +722,15 @@ void enqueue_finalize(Launcher& Lc, const StepIO& io) {
     Lc.check();
 }
 
-// Enqueue one full evaluation (energy + forces [+ whole-protein reduction]) on Lc.st with the given I/O buffers.
-void enqueue_all(Launcher& Lc, const StepIO& io) {
+// Embedding bit of option "embed_batch": several nodes per CTA share the embedding weights (bit 0 forward kernel, bit 1
+// adjoint kernel); by size when unset
+bool embed_batch(const vb_handle* h, int bit) {
+    return h->embed_batch_opt >= 0 ? (h->embed_batch_opt & bit) != 0 : h->ws.N > 8 * h->sm_count;
+}
+
+// The forward sweep both plans share: neighbour list, geometry, embeddings, the six layers, the last node stage and the
+// head (per-atom energies; with the workspace's adjoint pointers set, the head also starts the reverse sweep).
+void enqueue_fwd(Launcher& Lc, const StepIO& io) {
     vb_handle* h = Lc.h;
     Workspace& ws = h->ws;
     const int N = ws.N;
@@ -678,11 +742,8 @@ void enqueue_all(Launcher& Lc, const StepIO& io) {
     }
     if (Lc.next("rowptr_scan")) { Lc.launch(rowptr_scan_kernel, dim3(1), dim3(1024), 0, N, ws.deg, ws.rowptr, ws.Ecap, h->d_flags); Lc.check(); }
     if (Lc.next("edge_geom")) { Lc.launch(edge_geom_kernel, dim3((N + 3) / 4), dim3(128), 0, N, io.pos, h->mw, ws); Lc.check(); }
-    // batches: several nodes per CTA share the embedding weights ("embed_batch": bit 0 forward kernel, bit 1 adjoint kernel)
-    const bool batch = h->embed_batch_opt >= 0 ? (h->embed_batch_opt & 1) : N > 8 * h->sm_count;
-    const bool batch_bwd = h->embed_batch_opt >= 0 ? (h->embed_batch_opt & 2) != 0 : N > 8 * h->sm_count;
     if (Lc.next("embed_node")) {
-        if (batch) Lc.launch(embed_node_kernel<8>, dim3((N + 7) / 8), dim3(EMB_THREADS), 0, h->mw, ws);
+        if (embed_batch(h, 1)) Lc.launch(embed_node_kernel<8>, dim3((N + 7) / 8), dim3(EMB_THREADS), 0, h->mw, ws);
         else Lc.launch(embed_node_small_kernel, dim3((N + EMS_NB - 1) / EMS_NB), dim3(EMS_THREADS), 0, h->mw, ws,
                        h->timeline ? h->d_tl + (size_t)2 * L * TC_TL_SLOTS + (size_t)(2 * L + 2) * N2_TL_SLOTS : (unsigned long long*)nullptr);
         Lc.check();
@@ -697,13 +758,6 @@ void enqueue_all(Launcher& Lc, const StepIO& io) {
             if (Lc.next(name)) edge_fwd(Lc, l);
         }
         node_fwd_tc(Lc, L);
-        if (Lc.next("head")) head(Lc);
-        for (int l = L - 1; l >= 0; l--) {
-            node_bwd_tc(Lc, l + 1);
-            snprintf(name, sizeof(name), "edge_bwd%d", l);
-            if (Lc.next(name)) edge_bwd(Lc, l);
-        }
-        node_bwd_tc(Lc, 0);
     } else {
         for (int l = 0; l < L; l++) {
             snprintf(name, sizeof(name), "node_fwd%d", l);
@@ -712,7 +766,25 @@ void enqueue_all(Launcher& Lc, const StepIO& io) {
             if (Lc.next(name)) edge_fwd(Lc, l);
         }
         if (Lc.next("node_fwd6")) node_fwd(Lc, L);
-        if (Lc.next("head")) head(Lc);
+    }
+    if (Lc.next("head")) head(Lc);
+}
+
+// Enqueue one full evaluation (energy + forces [+ whole-protein reduction]) on Lc.st with the given I/O buffers.
+void enqueue_all(Launcher& Lc, const StepIO& io) {
+    vb_handle* h = Lc.h;
+    Workspace& ws = h->ws;
+    const int N = ws.N;
+    char name[64];
+    enqueue_fwd(Lc, io);
+    if (h->node_tc) {
+        for (int l = L - 1; l >= 0; l--) {
+            node_bwd_tc(Lc, l + 1);
+            snprintf(name, sizeof(name), "edge_bwd%d", l);
+            if (Lc.next(name)) edge_bwd(Lc, l);
+        }
+        node_bwd_tc(Lc, 0);
+    } else {
         for (int l = L - 1; l >= 0; l--) {
             snprintf(name, sizeof(name), "node_bwd%d", l + 1);
             if (Lc.next(name)) node_bwd(Lc, l + 1);
@@ -727,10 +799,40 @@ void enqueue_all(Launcher& Lc, const StepIO& io) {
         Lc.check();
     }
     if (Lc.next("embed_node_bwd")) {
-        Lc.launch(embed_node_bwd_kernel, dim3(batch_bwd ? std::min(N, 5 * h->sm_count) : N), dim3(ENB_WARPS * 32), 0, h->mw, ws, io.forces);
+        Lc.launch(embed_node_bwd_kernel, dim3(embed_batch(h, 2) ? std::min(N, 5 * h->sm_count) : N), dim3(ENB_WARPS * 32), 0, h->mw, ws, io.forces);
         Lc.check();
     }
     if (Lc.next("finalize")) enqueue_finalize(Lc, io);
+}
+
+// The workspace as the energy plan sees it: the adjoint's buffers are null, so nbr_build zeroes no forces, edge_geom no
+// eacc, and the head ends after the per-atom energies (no GX / GVEC).  The edge kernels still store their pre-activations
+// (P1 / SP / ATT): into the layer's own buffers on a derivative = 1 handle, into one shared scratch slot with derivative = 0.
+Workspace energy_workspace(Workspace ws) {
+    ws.eacc = ws.grbf = nullptr;
+    ws.GX = ws.GVEC = ws.GF = ws.GXA = ws.GQKV = ws.GVNMSG = ws.GTU = nullptr;
+    ws.PX = ws.PV = ws.GO = nullptr;
+    return ws;
+}
+
+// Enqueue one energy-only evaluation: the forward sweep with the full plan's kernel choices, then the fragment energies.
+// No forces (nbr_build zeroes none) and no whole-protein reduction.
+void enqueue_energy(Launcher& Lc, const StepIO& io) {
+    vb_handle* h = Lc.h;
+    const Workspace full = h->ws;
+    h->ws = energy_workspace(full);     // the launch helpers pass h->ws by value; restored below
+    StepIO eio = io;
+    eio.forces = nullptr;
+    eio.ef = nullptr;
+    enqueue_fwd(Lc, eio);
+    if (Lc.next("finalize")) enqueue_finalize(Lc, eio);
+    h->ws = full;
+}
+
+// The plan a handle evaluates by default: the full one, or the energy plan when it was set up with derivative = 0
+void enqueue_plan(Launcher& Lc, const StepIO& io) {
+    if (Lc.h->derivative) enqueue_all(Lc, io);
+    else enqueue_energy(Lc, io);
 }
 
 template <typename K>
@@ -778,6 +880,7 @@ int clean_accumulators(vb_handle* h, cudaStream_t st) {
     const size_t N = ws.N;
     CUDA_TRY(h, cudaMemsetAsync(ws.XA, 0, N * D * 4, st));
     CUDA_TRY(h, cudaMemsetAsync(ws.VA, 0, N * 3 * D * 4, st));
+    if (!h->derivative) { h->accum_dirty = false; return VB_OK; }     // the forward-only workspace has no adjoint accumulators
     CUDA_TRY(h, cudaMemsetAsync(ws.GQKV, 0, N * 3 * D * 4, st));
     CUDA_TRY(h, cudaMemsetAsync(ws.GVNMSG, 0, N * 3 * D * 4, st));
     CUDA_TRY(h, cudaMemsetAsync(ws.GTU, 0, N * 6 * D * 4, st));
@@ -787,7 +890,7 @@ int clean_accumulators(vb_handle* h, cudaStream_t st) {
     return VB_OK;
 }
 
-enum { K_EVAL = 0, K_HOST = 1, K_MD_EVAL = 2, K_MD_STEP = 3 };
+enum { K_EVAL = 0, K_HOST = 1, K_MD_EVAL = 2, K_MD_STEP = 3, K_ENERGY = 4, K_ENERGY_HOST = 5 };
 
 // Run `enqueue(stream)` -- a sequence of launches / async copies that depends only on (kind, io) and the handle's
 // configuration -- either directly or as a replay of its cached CUDA graph.  A failed capture always ends the capture
@@ -859,6 +962,22 @@ int run_eval(vb_handle* h, cudaStream_t st, const StepIO& io) {
     return run_cached(h, st, K_EVAL, io, [&](cudaStream_t s) -> int { return enqueue_eval(h, s, io, true); });
 }
 
+// every launch of one energy-only evaluation
+int enqueue_energy_eval(vb_handle* h, cudaStream_t st, const StepIO& io) {
+    Launcher Lc{h, st, -1, 0, false};
+    enqueue_energy(Lc, io);
+    if (Lc.status != cudaSuccess) { h->set_error("kernel launch failed: %s", cudaGetErrorString(Lc.status)); return VB_ERR_CUDA; }
+    return VB_OK;
+}
+
+// the entries that need forces or the adjoint's buffers refuse a forward-only handle
+int need_derivative(vb_handle* h, const char* who) {
+    if (h->derivative) return VB_OK;
+    h->set_error("%s: the handle was set up with option derivative = 0 (energies only, no forces): use vb_forward_energy, "
+                 "or set derivative = 1 and call vb_set_topology again", who);
+    return VB_ERR_STATE;
+}
+
 StepIO internal_io(vb_handle* h, bool protein) {
     StepIO io;
     io.pos = h->d_pos; io.energy = h->d_energy; io.forces = h->d_forces;
@@ -882,7 +1001,7 @@ void record_stages(vb_handle* h) {
     h->stage_kernels.clear();
     Launcher Lc{h, nullptr, -1, 0, true};
     Lc.kernels = &h->stage_kernels;
-    enqueue_all(Lc, internal_io(h, false));
+    enqueue_plan(Lc, internal_io(h, false));
     h->stage_kernels.resize(h->stage_names.size());
     h->launches = (int)h->stage_names.size();
 }
@@ -1038,16 +1157,7 @@ int vb_set_topology(vb_handle* h, int64_t n_atoms, int64_t n_graphs, const int64
     }
     for (int64_t g = 0; g < n_graphs; g++) frag_start[g + 1] += frag_start[g];
     CUDA_TRY(h, cudaSetDevice(h->device));
-    h->drop_graph();
-    h->free_md();                 // the MD recipe indexes the fragment atoms of the old topology
-    h->free_map();                // ... and so does the protein map: it must be set again
-    h->free_caph();               // ... and the hydrogen-refinement terms
-    h->has_topology = false;
-    cudaFree(h->arena); h->arena = nullptr;
-    cudaFreeHost(h->h_pos); cudaFreeHost(h->h_forces);
-    h->h_pos = h->h_energy = h->h_forces = nullptr;
-    h->ws = Workspace{};
-    h->edges_plan = 0;
+    h->clear_topology();
     h->ws.N = (int)n_atoms;
     h->ws.G = (int)n_graphs;
     const int64_t worst = n_atoms * KNB;
@@ -1072,8 +1182,9 @@ int vb_set_topology(vb_handle* h, int64_t n_atoms, int64_t n_graphs, const int64
     CUDA_TRY(h, cudaMemcpy(dfo, frag_of.data(), sizeof(int) * n_atoms, cudaMemcpyHostToDevice));
     CUDA_TRY(h, cudaMemcpy(dfs, frag_start.data(), sizeof(int) * (n_graphs + 1), cudaMemcpyHostToDevice));
     CUDA_TRY(h, cudaMallocHost(&h->h_pos, sizeof(float) * 3 * n_atoms));
-    CUDA_TRY(h, cudaMallocHost(&h->h_forces, sizeof(float) * (3 * n_atoms + n_graphs)));   // forces, then energies (one copy)
-    h->h_energy = h->h_forces + 3 * n_atoms;
+    const int64_t n_force = h->derivative ? 3 * n_atoms : 0;
+    CUDA_TRY(h, cudaMallocHost(&h->h_forces, sizeof(float) * (n_force + n_graphs)));   // forces, then energies (one copy)
+    h->h_energy = h->h_forces + n_force;
     choose_defaults(h);
     record_stages(h);
     h->has_topology = true;
@@ -1085,6 +1196,7 @@ int vb_forward(vb_handle* h, const float* pos_dev, float* energy_dev, float* for
     if (!h) return VB_ERR_ARG;
     std::lock_guard<std::mutex> lk(h->mu);
     if (!h->has_topology) { h->set_error("vb_forward: call vb_set_topology first"); return VB_ERR_STATE; }
+    if (int rc = need_derivative(h, "vb_forward")) return rc;
     if (!pos_dev || !energy_dev || !forces_dev) { h->set_error("vb_forward: null buffer"); return VB_ERR_ARG; }
     CUDA_TRY(h, cudaSetDevice(h->device));
     StepIO io;
@@ -1110,6 +1222,7 @@ int vb_forward_host(vb_handle* h, const float* pos_host, float* energy_host, flo
     if (!h) return VB_ERR_ARG;
     std::lock_guard<std::mutex> lk(h->mu);
     if (!h->has_topology) { h->set_error("vb_forward_host: call vb_set_topology first"); return VB_ERR_STATE; }
+    if (int rc = need_derivative(h, "vb_forward_host")) return rc;
     if (!pos_host || !energy_host || !forces_host) { h->set_error("vb_forward_host: null buffer"); return VB_ERR_ARG; }
     const int N = h->ws.N, G = h->ws.G;
     cudaStream_t st = h->own_stream;
@@ -1128,6 +1241,44 @@ int vb_forward_host(vb_handle* h, const float* pos_host, float* energy_host, flo
     if (int r = check_edge_overflow(h, "vb_forward_host")) return r;
     memcpy(energy_host, h->h_energy, sizeof(float) * G);
     memcpy(forces_host, h->h_forces, sizeof(float) * 3 * N);
+    return VB_OK;
+}
+
+int vb_forward_energy(vb_handle* h, const float* pos_dev, float* energy_dev, void* stream) {
+    NvtxRange nvtx_("vb_forward_energy");
+    if (!h) return VB_ERR_ARG;
+    std::lock_guard<std::mutex> lk(h->mu);
+    if (!h->has_topology) { h->set_error("vb_forward_energy: call vb_set_topology first"); return VB_ERR_STATE; }
+    if (!pos_dev || !energy_dev) { h->set_error("vb_forward_energy: null buffer"); return VB_ERR_ARG; }
+    CUDA_TRY(h, cudaSetDevice(h->device));
+    StepIO io;
+    io.pos = pos_dev; io.energy = energy_dev;
+    return run_cached(h, (cudaStream_t)stream, K_ENERGY, io, [&](cudaStream_t s) -> int { return enqueue_energy_eval(h, s, io); });
+}
+
+int vb_forward_energy_host(vb_handle* h, const float* pos_host, float* energy_host) {
+    NvtxRange nvtx_("vb_forward_energy_host");
+    if (!h) return VB_ERR_ARG;
+    std::lock_guard<std::mutex> lk(h->mu);
+    if (!h->has_topology) { h->set_error("vb_forward_energy_host: call vb_set_topology first"); return VB_ERR_STATE; }
+    if (!pos_host || !energy_host) { h->set_error("vb_forward_energy_host: null buffer"); return VB_ERR_ARG; }
+    const int N = h->ws.N, G = h->ws.G;
+    cudaStream_t st = h->own_stream;
+    CUDA_TRY(h, cudaSetDevice(h->device));
+    memcpy(h->h_pos, pos_host, sizeof(float) * 3 * N);
+    // H2D of the positions, the energy plan, D2H of the energies: one graph replay
+    StepIO io;
+    io.pos = h->d_pos; io.energy = h->d_energy;
+    int rc = run_cached(h, st, K_ENERGY_HOST, io, [&](cudaStream_t s) -> int {
+        CUDA_TRY(h, cudaMemcpyAsync(h->d_pos, h->h_pos, sizeof(float) * 3 * N, cudaMemcpyHostToDevice, s));
+        if (int r = enqueue_energy_eval(h, s, io)) return r;
+        CUDA_TRY(h, cudaMemcpyAsync(h->h_energy, h->d_energy, sizeof(float) * G, cudaMemcpyDeviceToHost, s));
+        return (int)VB_OK;
+    });
+    if (rc != VB_OK) return rc;
+    CUDA_TRY(h, cudaStreamSynchronize(st));
+    if (int r = check_edge_overflow(h, "vb_forward_energy_host")) return r;
+    memcpy(energy_host, h->h_energy, sizeof(float) * G);
     return VB_OK;
 }
 
@@ -1186,6 +1337,7 @@ int vb_forward_protein(vb_handle* h, const float* pos_dev, float* ef_prot_dev, v
     if (!h) return VB_ERR_ARG;
     std::lock_guard<std::mutex> lk(h->mu);
     if (!h->has_topology || h->n_protein <= 0) { h->set_error("vb_forward_protein: topology / protein map not set"); return VB_ERR_STATE; }
+    if (int rc = need_derivative(h, "vb_forward_protein")) return rc;
     if (!pos_dev || !ef_prot_dev) { h->set_error("vb_forward_protein: null buffer"); return VB_ERR_ARG; }
     CUDA_TRY(h, cudaSetDevice(h->device));
     StepIO io = internal_io(h, false);
@@ -1250,6 +1402,7 @@ int vb_md_setup(vb_handle* h, int64_t n_protein_atoms, const double* masses_host
     if (!h) return VB_ERR_ARG;
     std::lock_guard<std::mutex> lk(h->mu);
     if (!h->has_topology || h->n_protein <= 0) { h->set_error("vb_md_setup: topology / protein map not set"); return VB_ERR_STATE; }
+    if (int rc = need_derivative(h, "vb_md_setup")) return rc;
     if (n_protein_atoms != h->n_protein || !masses_host || !real_host || !acc_host || !rem_host || !blen_host || !ef_prot_dev ||
         !(dt > 0.0) || kT < 0.0 || friction < 0.0) {
         h->set_error("vb_md_setup: bad arguments (n_protein must equal the protein map's)");
@@ -1841,6 +1994,15 @@ int vb_set_option(vb_handle* h, const char* key, int64_t value) {
     else if (k == "krot" && (value == 0 || value == 1)) h->krot = (int)value;
     else if (k == "node_tc" && (value == 0 || value == 1)) { h->node_tc = h->node_tc_opt = (int)value; set_gxa_parts(h); }
     else if (k == "comm_auto" && (value == 0 || value == 1)) h->comm_auto = (int)value;
+    else if (k == "derivative" && (value == 0 || value == 1)) {
+        // the workspace layout depends on it: drop the topology (and the map, MD and refinement state sized by it)
+        if (cudaSetDevice(h->device) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess) {
+            h->set_error("vb_set_option: derivative: %s", cudaGetErrorString(cudaGetLastError()));
+            return VB_ERR_CUDA;
+        }
+        h->derivative = (int)value;
+        h->clear_topology();
+    }
     else if (k == "embed_batch" && value >= -1 && value <= 3) h->embed_batch_opt = (int)value;
     else if (k == "timeline" && (value == 0 || value == 1)) {
         if (value && !h->d_tl) {
@@ -1870,6 +2032,8 @@ int64_t vb_get_option(const vb_handle* h, const char* key) {
     if (k == "krot") return h->krot;
     if (k == "node_tc") return h->node_tc;
     if (k == "comm_auto") return h->comm_auto;
+    if (k == "derivative") return h->derivative;
+    if (k == "arena_bytes") return (int64_t)h->arena_bytes;
     if (k == "caph_ready") return h->caph_ready ? 1 : 0;
     if (k == "caph_evals") {           // energy evaluations of the last refinement (synchronises)
         int v = 0;
@@ -1926,7 +2090,7 @@ int vb_debug_run(vb_handle* h, const float* pos_dev, int n_stages) {
     CUDA_TRY(h, cudaMemcpy(h->d_pos, pos_dev, sizeof(float) * 3 * h->ws.N, cudaMemcpyDeviceToDevice));
     if (h->accum_dirty) { if (int rc = clean_accumulators(h, h->own_stream)) return rc; }
     Launcher Lc{h, h->own_stream, n_stages, 0, false};
-    enqueue_all(Lc, internal_io(h, h->n_protein > 0));
+    enqueue_plan(Lc, internal_io(h, h->n_protein > 0));
     if (Lc.status != cudaSuccess) { h->set_error("debug launch failed: %s", cudaGetErrorString(Lc.status)); return VB_ERR_CUDA; }
     CUDA_TRY(h, cudaStreamSynchronize(h->own_stream));
     h->accum_dirty = n_stages >= 0 && n_stages < (int)h->stage_names.size();   // a consumer stage may not have re-zeroed its accumulators
@@ -1947,7 +2111,7 @@ int vb_profile_stages(vb_handle* h, const float* pos_dev, int n_iter, float* ms_
     for (int it = 0; it < n_iter + 1 && rc == VB_OK; it++) {      // iteration 0 is an untimed warm-up
         Launcher Lc{h, h->own_stream, -1, 0, false};
         Lc.events = &ev;
-        enqueue_all(Lc, internal_io(h, h->n_protein > 0));
+        enqueue_plan(Lc, internal_io(h, h->n_protein > 0));
         cudaEventRecord(ev[ns], h->own_stream);
         if (Lc.status != cudaSuccess || cudaStreamSynchronize(h->own_stream) != cudaSuccess) {
             h->set_error("vb_profile_stages: launch failed: %s", cudaGetErrorString(cudaGetLastError()));
@@ -2010,17 +2174,30 @@ int64_t vb_debug_read(vb_handle* h, const char* name, int layer, void* host_dst,
     const void* src = nullptr;
     size_t bytes = 0;
     const std::string k(name);
+    if (!h->derivative) {
+        for (const char* a : {"P1", "SP", "ATT", "GX", "GVEC", "GF", "GXA", "GXA3", "GQKV", "GVNMSG", "GTU", "eacc", "grbf", "forces"})
+            if (k == a) {
+                h->set_error("vb_debug_read: %s is kept only for the reverse sweep; the handle was set up with derivative = 0", name);
+                return VB_ERR_STATE;
+            }
+    }
     auto lay = [&](int hi) { return layer >= 0 && layer < hi; };
+    // derivative = 0: layers of one parity share a slot, so only the last layer written to a slot can be read back
+    bool overwritten = false;
+    auto per_layer = [&](float* const* p, int n, size_t count) {
+        src = p[layer]; bytes = count * 4;
+        for (int m = layer + 1; m < n; m++) overwritten = overwritten || p[m] == p[layer];
+    };
 #define BUF(key, ptr, count, elt) if (k == key) { src = (ptr); bytes = (size_t)(count) * (elt); }
-    if (k == "X" && lay(L + 1)) { src = ws.X[layer]; bytes = N * D * 4; }
-    else if (k == "V" && lay(L + 1)) { src = ws.V[layer]; bytes = N * 3 * D * 4; }
-    else if (k == "F" && lay(L)) { src = ws.F[layer]; bytes = E * D * 4; }
-    else if (k == "VN" && lay(L)) { src = ws.VN[layer]; bytes = N * 3 * D * 4; }
-    else if (k == "QKV" && lay(L)) { src = ws.QKV[layer]; bytes = N * 3 * D * 4; }
-    else if (k == "V123" && lay(L)) { src = ws.V123[layer]; bytes = N * 9 * D * 4; }
-    else if (k == "VDOT" && lay(L)) { src = ws.VDOT[layer]; bytes = N * D * 4; }
-    else if (k == "TU" && lay(L)) { src = ws.TU[layer]; bytes = N * 6 * D * 4; }
-    else if (k == "O" && lay(L)) { src = ws.O[layer]; bytes = N * 3 * D * 4; }
+    if (k == "X" && lay(L + 1)) per_layer(ws.X, L + 1, N * D);
+    else if (k == "V" && lay(L + 1)) per_layer(ws.V, L + 1, N * 3 * D);
+    else if (k == "F" && lay(L)) per_layer(ws.F, L, E * D);
+    else if (k == "VN" && lay(L)) per_layer(ws.VN, L, N * 3 * D);
+    else if (k == "QKV" && lay(L)) per_layer(ws.QKV, L, N * 3 * D);
+    else if (k == "V123" && lay(L)) per_layer(ws.V123, L, N * 9 * D);
+    else if (k == "VDOT" && lay(L)) per_layer(ws.VDOT, L, N * D);
+    else if (k == "TU" && lay(L)) per_layer(ws.TU, L, N * 6 * D);
+    else if (k == "O" && lay(L)) per_layer(ws.O, L, N * 3 * D);
     else if (k == "P1" && lay(L)) { src = ws.P1[layer]; bytes = E * 3 * D * 4; }
     else if (k == "SP" && lay(L)) { src = ws.SP[layer]; bytes = E * 2 * D * 4; }
     else if (k == "ATT" && lay(L)) { src = ws.ATT[layer]; bytes = E * H * 4; }
@@ -2050,6 +2227,10 @@ int64_t vb_debug_read(vb_handle* h, const char* name, int layer, void* host_dst,
     else if (k == "RF" && h->rs_ready) { src = h->rs.rf; bytes = (3 * (size_t)h->n_protein + 1) * 8; }
 #undef BUF
     if (!src) { h->set_error("vb_debug_read: unknown buffer %s[%d]", name, layer); return VB_ERR_ARG; }
+    if (overwritten) {
+        h->set_error("vb_debug_read: %s[%d] shares its slot with a later layer (derivative = 0)", name, layer);
+        return VB_ERR_STATE;
+    }
     if ((int64_t)bytes > cap_bytes) bytes = (size_t)cap_bytes;
     if (cudaSetDevice(h->device) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess ||
         cudaMemcpy(host_dst, src, bytes, cudaMemcpyDeviceToHost) != cudaSuccess) {

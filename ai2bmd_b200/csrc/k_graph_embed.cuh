@@ -19,7 +19,7 @@ __global__ void __launch_bounds__(128) nbr_build_kernel(int N, const float* __re
     pdl_entry();
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= N) return;
-    forces[3 * i] = 0.f; forces[3 * i + 1] = 0.f; forces[3 * i + 2] = 0.f;   // accumulated by the last kernel of the sweep
+    if (forces) { forces[3 * i] = 0.f; forces[3 * i + 1] = 0.f; forces[3 * i + 2] = 0.f; }   // accumulated by the last kernel of the sweep (none in the energy plan)
     const int g = frag_of[i];
     const int j0 = frag_start[g], j1 = frag_start[g + 1];
     const float xi = pos[3 * i], yi = pos[3 * i + 1], zi = pos[3 * i + 2];
@@ -112,7 +112,7 @@ __global__ void __launch_bounds__(128) edge_geom_kernel(int N, const float* __re
             ws.edst[e] = i;
             st4(ws.geom + (size_t)e * 8, f4(r, C, dx, dy));
             st4(ws.geom + (size_t)e * 8 + 4, f4(dz, inv_r, __int_as_float(ws.z[j]), 0.f));   // [6]: z of the source atom (embed_node)
-            st4(ws.eacc + (size_t)e * 4, f4s(0.f));
+            if (ws.eacc) st4(ws.eacc + (size_t)e * 4, f4s(0.f));       // adjoint accumulators (absent in the energy plan)
         }
     }
     const float mu = __ldg(mw.rbf_means + lane), beta = __ldg(mw.rbf_betas + lane);

@@ -135,6 +135,7 @@ __global__ void __launch_bounds__(NODE_WARPS * 32) head_kernel(ModelW mw, Worksp
         const int node = n0 + nd;
         if (lane == 0 && node < ws.N) ws.eatom[node] = e * stdv + __ldg(mw.atomref + ws.z[node]);
     }
+    if (ws.GX == nullptr) return;         // energy plan: no adjoint outputs in the workspace
     // ================= adjoint (dE_total/de_atom = 1) =================
 #pragma unroll
     for (int nd = 0; nd < NPW; nd++) {
@@ -370,6 +371,7 @@ __global__ void __launch_bounds__(128) head2_kernel(ModelW mw, Workspace ws) {
         const float e = warp_sum(silu_(preb[0][0]) * u2.x + silu_(preb[0][1]) * u2.y) + __ldg(mw.h1_b2);
         if (threadIdx.x == 0) ws.eatom[node] = e * stdv + __ldg(mw.atomref + ws.z[node]);
     }
+    if (ws.GX == nullptr) return;         // energy plan: no adjoint outputs in the workspace
     // ================= adjoint =================
     if (w0) {
         sm.gpb[c2] = stdv * u2.x * dsilu_(preb[0][0]);

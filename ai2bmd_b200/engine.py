@@ -37,7 +37,7 @@ class _CaphProblem(C.Structure):
 # every symbol include/visnet_b200.h declares (tests check that the library exports each of them)
 EXPORTED_SYMBOLS = [
     "vb_weight_manifest", "vb_create", "vb_destroy", "vb_last_error", "vb_set_topology", "vb_forward",
-    "vb_forward_host", "vb_set_protein_map", "vb_forward_protein", "vb_get_edges", "vb_launches_per_forward",
+    "vb_forward_host", "vb_set_protein_map", "vb_forward_protein", "vb_forward_energy", "vb_forward_energy_host", "vb_get_edges", "vb_launches_per_forward",
     "vb_set_option", "vb_get_option", "vb_num_stages", "vb_stage_name", "vb_stage_kernel", "vb_debug_run", "vb_debug_read", "vb_profile_stages", "vb_tc_selftest", "vb_tc_selftest_rows",
     "vb_md_setup", "vb_md_set_normals", "vb_md_set_state", "vb_md_kick1", "vb_md_eval", "vb_md_kick2", "vb_md_run", "vb_md_get_state",
     "vb_md_set_restraints", "vb_md_set_recorder", "vb_md_read_frames",
@@ -76,6 +76,10 @@ def load_library(path: Optional[str] = None):
     lib.vb_set_protein_map.argtypes = [vp, i64, i64, vp, vp, vp, vp]
     lib.vb_forward_protein.restype = C.c_int
     lib.vb_forward_protein.argtypes = [vp, vp, vp, vp]
+    lib.vb_forward_energy.restype = C.c_int
+    lib.vb_forward_energy.argtypes = [vp, vp, vp, vp]
+    lib.vb_forward_energy_host.restype = C.c_int
+    lib.vb_forward_energy_host.argtypes = [vp, vp, vp]
     lib.vb_get_edges.restype = C.c_int
     lib.vb_get_edges.argtypes = [vp, vp, vp]
     lib.vb_launches_per_forward.restype = C.c_int
@@ -144,9 +148,13 @@ def weight_manifest() -> str:
 
 class Engine:
     """One engine per CUDA device (the reference keeps one ``ViSNetModel`` per device,
-    ``src/Calculators/bonded.py:40-44``)."""
+    ``src/Calculators/bonded.py:40-44``).
 
-    def __init__(self, state_dict: Dict[str, np.ndarray], device: int = 0, cutoff: float = 5.0):
+    ``derivative=False`` lays out a forward-only workspace (option ``"derivative"`` = 0): only :meth:`energy_host` /
+    :meth:`energy_device` evaluate, the reference's ``ViSNet(derivative=False)``.  With ``derivative=True`` both the
+    force entries and the energy entries work."""
+
+    def __init__(self, state_dict: Dict[str, np.ndarray], device: int = 0, cutoff: float = 5.0, derivative: bool = True):
         self.lib = load_library()
         blob = pack_weights(state_dict, self.lib.vb_weight_manifest().decode())
         hp = _HParams(128, 6, 8, 32, 32, cutoff)
@@ -156,6 +164,9 @@ class Engine:
             raise RuntimeError(f"vb_create failed ({rc}): {self.lib.vb_last_error(None).decode()}")
         self.h = handle
         self.device = int(device)
+        self.derivative = bool(derivative)
+        if not self.derivative:
+            self.set_option("derivative", 0)
         self.n_atoms = 0
         self.n_graphs = 0
         self.n_protein = 0
@@ -201,6 +212,9 @@ class Engine:
 
     def set_option(self, key: str, value: int):
         self._check(self.lib.vb_set_option(self.h, key.encode(), int(value)), "vb_set_option")
+        if key == "derivative":          # the library dropped the topology: set_topology again
+            self.derivative = bool(value)
+            self.n_atoms = self.n_graphs = self.n_protein = 0
 
     def get_option(self, key: str) -> int:
         return int(self.lib.vb_get_option(self.h, key.encode()))
@@ -223,6 +237,21 @@ class Engine:
     def forward_device(self, pos_ptr: int, energy_ptr: int, forces_ptr: int, stream_ptr: int = 0):
         """Raw device pointers (e.g. ``tensor.data_ptr()``) and a ``cudaStream_t``; asynchronous."""
         self._check(self.lib.vb_forward(self.h, pos_ptr, energy_ptr, forces_ptr, stream_ptr), "vb_forward")
+
+    def energy_host(self, pos: np.ndarray) -> np.ndarray:
+        """Energies only: host positions [N,3] in, fragment energies e[G] out (vb_forward_energy_host)."""
+        pos = np.ascontiguousarray(pos, dtype=np.float32)
+        if pos.shape != (self.n_atoms, 3):
+            raise ValueError(f"pos must be [{self.n_atoms},3]")
+        e = np.empty((self.n_graphs,), dtype=np.float32)
+        rc = self.lib.vb_forward_energy_host(self.h, pos.__array_interface__["data"][0], e.__array_interface__["data"][0])
+        if rc < 0:
+            self._check(rc, "vb_forward_energy_host")
+        return e
+
+    def energy_device(self, pos_ptr: int, e_ptr: int, stream_ptr: int = 0):
+        """Energies only, raw device pointers (positions [N,3], energies [G]) and a ``cudaStream_t``; asynchronous."""
+        self._check(self.lib.vb_forward_energy(self.h, pos_ptr, e_ptr, stream_ptr), "vb_forward_energy")
 
     def forward_protein_device(self, pos_ptr: int, ef_ptr: int, stream_ptr: int = 0):
         self._check(self.lib.vb_forward_protein(self.h, pos_ptr, ef_ptr, stream_ptr), "vb_forward_protein")

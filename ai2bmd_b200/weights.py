@@ -8,7 +8,7 @@ GEMMs; fused matrices ([q|k|v], [dk|dv|f], [w_trg|w_src]) are concatenated along
 from __future__ import annotations
 
 import re
-from typing import Dict
+from typing import Dict, Optional, Tuple
 
 import numpy as np
 
@@ -17,9 +17,22 @@ D, L = 128, 6
 
 def load_state_dict(path: str) -> Dict[str, np.ndarray]:
     """``.ckpt`` (Lightning checkpoint as shipped by the reference) or ``.npz`` (extracted state_dict)."""
+    return load_checkpoint(path)[0]
+
+
+def resolve_derivative(checkpoint_derivative: bool, derivative: Optional[bool] = None) -> bool:
+    """The reference's rule (``load_model(path, derivative=...)``, ``visnet.py:73-81``): the checkpoint's hyper-parameter,
+    overridden by an explicit keyword."""
+    return bool(checkpoint_derivative) if derivative is None else bool(derivative)
+
+
+def load_checkpoint(path: str) -> Tuple[Dict[str, np.ndarray], bool]:
+    """(state_dict, the checkpoint's ``derivative`` hyper-parameter).  An ``.npz`` carries no hyper-parameters and counts
+    as ``derivative=True``, as does a checkpoint that does not set it.  Every other hyper-parameter must be the one the
+    kernels are specialised for."""
     if path.endswith(".npz"):
         z = np.load(path)
-        return {k: np.asarray(z[k], dtype=np.float32) for k in z.files}
+        return {k: np.asarray(z[k], dtype=np.float32) for k in z.files}, True
     import torch
     try:
         ck = torch.load(path, map_location="cpu", weights_only=True)
@@ -30,11 +43,14 @@ def load_state_dict(path: str) -> Dict[str, np.ndarray]:
     if hp:
         want = dict(embedding_dimension=128, num_layers=6, num_heads=8, num_rbf=32, lmax=1, max_num_neighbors=32,
                     vecnorm_type="max_min", rbf_type="expnorm", activation="silu", attn_activation="silu", cutoff=5.0,
-                    max_z=100, prior_model="Atomref", reduce_op="add", derivative=True)
+                    max_z=100, prior_model="Atomref", reduce_op="add")
         for k, v in want.items():
             if k in hp and hp[k] != v:
                 raise ValueError(f"checkpoint hyper-parameter {k}={hp.get(k)!r} is not the supported {v!r}")
-    return {re.sub(r"^model\.", "", k): v.float().numpy() for k, v in ck["state_dict"].items()}
+        if "derivative" in hp and hp["derivative"] not in (True, False):
+            raise ValueError(f"checkpoint hyper-parameter derivative={hp['derivative']!r} is not a bool")
+    sd = {re.sub(r"^model\.", "", k): v.float().numpy() for k, v in ck["state_dict"].items()}
+    return sd, bool(hp.get("derivative", True)) if hp else True
 
 
 def _named_arrays(sd: Dict[str, np.ndarray]) -> Dict[str, np.ndarray]:

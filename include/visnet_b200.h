@@ -82,6 +82,28 @@ int vb_set_protein_map(vb_handle* h, int64_t n_protein_atoms, int64_t n_map, con
  * the caller all-reduces ef_prot_dev (NCCL sum).  Replaces: DLBondedCalculator.__call__, bonded.py:102-123. */
 int vb_forward_protein(vb_handle* h, const float* pos_dev, float* ef_prot_dev, void* stream);
 
+/* ---- Energies without forces -------------------------------------------------------------------------------
+ * Option "derivative" (vb_set_option, 0 or 1, default 1) selects the workspace vb_set_topology lays out:
+ *   1  the full one: vb_forward* evaluate energies and forces; the energy entries below run on it too.
+ *   0  a forward-only one of about a fifth of the size (no adjoint buffers, the per-layer node and edge tensors in two
+ *      slots by layer parity): only the energy entries below evaluate; vb_forward, vb_forward_host, vb_forward_protein,
+ *      vb_md_setup and vb_debug_read of an adjoint buffer fail with VB_ERR_STATE, and the diagnostics (vb_num_stages,
+ *      vb_stage_name, vb_stage_kernel, vb_debug_run, vb_profile_stages, vb_launches_per_forward) describe and run the
+ *      energy plan.
+ * Setting the option drops the topology (and the protein map, MD and hydrogen-refinement state): call vb_set_topology
+ * again.  vb_get_option("derivative") answers the setting, vb_get_option("arena_bytes") the workspace size in bytes of
+ * the current topology.
+ *
+ * The energy plan runs the full plan's forward launches with the same kernel choices (node / edge stage variants, tile
+ * plan, calibration), so its energies equal vb_forward's bit for bit, then writes the fragment energies; no adjoint.
+ * Replaces: ViSNet.forward with derivative=False, src/ViSNet/model/visnet.py:135-166 (returns (E, None)). */
+
+/* pos_dev[N*3] -> energy_dev[G], device buffers, asynchronous on `stream` (one replay of a cached CUDA graph). */
+int vb_forward_energy(vb_handle* h, const float* pos_dev, float* energy_dev, void* stream);
+/* The same with HOST buffers (pinned staging, one H2D and one D2H inside), synchronous; like vb_forward_host it fails
+ * with VB_ERR_STATE when a step produced more edges than a trimmed max_edges holds. */
+int vb_forward_energy_host(vb_handle* h, const float* pos_host, float* energy_host);
+
 /* ---- Device-resident MD step (SURVEY section 8f, rank 3 and the first half of rank 1) ------------------------
  * State (protein positions / velocities, fp64) stays on the GPU; one step is
  *   kick1 (half-kick + drift) -> eval (place fragment atoms, ViSNet, signed reduction into ef) -> kick2.
