@@ -175,11 +175,14 @@ def frag_bar(what):
     return FRAG_BAR
 
 
-def check_plan(case, detail):
-    """What the case claims to run: kernels (template arguments included), tile plan, node-stage mode."""
+def check_plan(case, detail, forward_only=False):
+    """What the case claims to run: kernels (template arguments included), tile plan, node-stage mode.  forward_only:
+    the energy plan of a derivative = 0 handle, which runs the case's kernels but no adjoint ones."""
     _, _, _, extra, plan = STAGE_CASES[case]
     ran = _kernel_set(detail["kernels"])
     want = set(_pinned(f"stage:{case}")) | set(extra)
+    if forward_only:
+        want = {k for k in want if not re.search(r"_bwd|node_tc_kernel<[23]>", k)}
     assert want <= ran, f"{case} does not run {sorted(want - ran)}; it runs {sorted(ran)}"
     opts = detail["options"]
     for k, v in plan.items():

@@ -18,8 +18,11 @@ sys.path.insert(0, os.path.join(ROOT, "tools"))
 pytestmark = pytest.mark.gpu
 
 
-@pytest.mark.parametrize("opts", [pytest.param("", id="default"), "edge_tc=0", "edge_tc=1", "edge_tc=2", "node_tc=1",
-                                  "node_nb=2", "node_nb=3", "node_nb=4", "node_nb=8"])     # default here: node_nb=1 (one wave)
+# default here: node_nb=1 (one wave); test_stale_workspace_gpu.py runs the same list after a decoy geometry
+OPTS = ["", "edge_tc=0", "edge_tc=1", "edge_tc=2", "node_tc=1", "node_nb=2", "node_nb=3", "node_nb=4", "node_nb=8"]
+
+
+@pytest.mark.parametrize("opts", OPTS, ids=lambda o: o or "default")
 @pytest.mark.parametrize("weights", ["real", "3"])
 def test_every_stage_against_the_fp64_adjoint_oracle(opts, weights):
     from stage_check import stage_report

@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Stage-by-stage parity of the CUDA engine against the hand-adjoint oracle (GPU box diagnostic).
 
-    python tools/stage_check.py [--weights real|random] [--frags chig] [--calibrate] [--out stage_check.txt]
+    python tools/stage_check.py [--weights real|random] [--frags chig] [--calibrate] [--decoy dense|nan] [--energy]
+                                [--out stage_check.txt]
 
 Runs the evaluation one launch at a time (``vb_debug_run``), reads the engine's internal buffers after
 each stage and compares them with the tensors of ``oracle/adjoint_ref.py`` (fp64).  The first stage whose
@@ -41,7 +42,74 @@ def fragment_rel(got, ref, frag, n_frags):
     return float(rel[g]), g
 
 
-def stage_report(frags="chig", weights="real", max_frags=0, opts="", calibrate=False, detail=None):
+def decoy_positions(pos, batch, kind, seed=0):
+    """Positions of another geometry on the same z / batch topology, to run just before the geometry under test, so
+    that whatever a stage reads before this evaluation writes it holds some other evaluation's data (float32 [N,3]).
+
+    "dense": every fragment contracted toward its centroid by 0.85, then a seeded 0.2 A Gaussian displacement.  The
+    neighbour lists, degrees, row pointers and the edge count all change, and the edge count grows by more than one
+    128-row tile, so every edge row of the target and the rows past its last edge hold some other edge's finite data.
+    "nan": the dense decoy with the second atom of every fragment of >= 2 atoms placed exactly on the first one.  The
+    coordinates stay finite and the pair stays neighbours, so r = 0 for j != i gives d = 0/0 in edge_geom: NaN spreads
+    through every vector feature and every later buffer of that fragment (and the shared memory the kernels leave
+    behind).  No kernel turns a feature value into an index (the only float-to-int reinterpretation is the atomic number
+    edge_geom copies into the geometry rows, and the VecLayerNorm max / min paths compare keys whose index bits are the
+    channel, whatever the value), so the poison stays in values."""
+    pos = np.asarray(pos, dtype=np.float64)
+    batch = np.asarray(batch)
+    if kind not in ("dense", "nan"):
+        raise ValueError(f"decoy kind {kind!r}: 'dense' or 'nan'")
+    out = pos.copy()
+    for g in np.unique(batch):
+        m = batch == g
+        c = out[m].mean(0)
+        out[m] = c + 0.85 * (out[m] - c)
+    out = (out + 0.2 * np.random.default_rng(seed).standard_normal(out.shape)).astype(np.float32)
+    if kind == "nan":
+        first = np.flatnonzero(np.r_[True, batch[1:] != batch[:-1]])
+        for a in first:
+            if a + 1 < len(batch) and batch[a + 1] == batch[a]:
+                out[a + 1] = out[a]
+    return out
+
+
+# Forward-only workspace (derivative = 0): layer l of a per-layer buffer lives in slot l % 2, and layer 0 of V / V123 /
+# TU in a zeroed slot of its own (DESIGN section 3).  vb_debug_read refuses a layer that a later layer shares its slot
+# with; the checks read each layer right after the stage that writes it, before that slot is written again, so they ask
+# for the same slot under the last layer that maps to it.  No forward check of the full plan has to be skipped: each one
+# reads only buffers its own stage writes (node stage k: X / V / VN / QKV / V123 / VDOT / TU of layer k and O of layer
+# k - 1; tensor-core "norm k": VDOT of layer k - 1; edge stage l: F of layer l + 1), and no stage writes two layers that
+# share a slot.  The adjoint's checks (gx_out / gvec_out at the head, every backward stage) have no buffers here.
+PER_LAYER = ("X", "V", "F", "VN", "QKV", "V123", "VDOT", "TU", "O")
+OWN_ZERO_LAYER = ("V", "V123", "TU")
+
+
+def energy_slot_layer(name, layer):
+    if layer == 0 and name in OWN_ZERO_LAYER:
+        return 0
+    n = L + 1 if name in ("X", "V") else L
+    return max(range(layer, n, 2))
+
+
+_oracle_cache = {}
+
+
+def _oracle(key, sd, z, pos, batch, ei):
+    """fp64 hand-adjoint tensors of one geometry; the last one is kept, so that runs of cases on one fixture (and one
+    case under several decoys) build it once."""
+    if key is not None and key in _oracle_cache:
+        return _oracle_cache[key]
+    adj = AdjointViSNet(O.OracleViSNet(sd, torch.float64))
+    Eo, Fo, S, B = adj.energy_and_forces(z, pos, batch, ei)
+    out = ({k: v.numpy() for k, v in S.items()}, {k: v.numpy() for k, v in B.items()})
+    _oracle_cache.clear()
+    if key is not None:
+        _oracle_cache[key] = out
+    return out
+
+
+def stage_report(frags="chig", weights="real", max_frags=0, opts="", calibrate=False, detail=None, decoy=None,
+                 derivative=True):
     """Run the evaluation one launch at a time and compare every buffer a stage produces with the fp64 hand-adjoint
     oracle.  Returns (lines, worst) where worst = [(stage, what, rel)] of the comparisons, rel relative to the largest
     reference entry of the buffer.
@@ -65,22 +133,21 @@ def stage_report(frags="chig", weights="real", max_frags=0, opts="", calibrate=F
     slots, deg = O.radius_graph_canonical(pos, batch)
     ei = torch.from_numpy(O.slots_to_edge_index(slots, deg))
     E, N = ei.shape[1], len(z)
-    adj = AdjointViSNet(O.OracleViSNet(sd, torch.float64))
-    Eo, Fo, S, B = adj.energy_and_forces(z, pos, batch, ei)
-    S = {k: v.numpy() for k, v in S.items()}
-    B = {k: v.numpy() for k, v in B.items()}
+    S, B = _oracle((frags, max_frags, str(weights)) if isinstance(frags, str) else None, sd, z, pos, batch, ei)
 
-    eng = Engine({k: v.numpy() for k, v in sd.items()}, 0)
+    eng = Engine({k: v.numpy() for k, v in sd.items()}, 0, derivative=derivative)
     G = int(batch.max()) + 1
     eng.set_topology(z, batch, n_graphs=G)
     for kv in filter(None, opts.split(",")):
         k, v = kv.split("=")
         eng.set_option(k, int(v))
+    host_eval = eng.forward_host if derivative else eng.energy_host
     if calibrate:
-        eng.forward_host(pos)
+        host_eval(pos)
         eng.set_option("calibrate", 1)
     names = eng.stage_names()
     dpos = torch.from_numpy(pos).cuda()
+    ddecoy = torch.from_numpy(decoy_positions(pos, batch, decoy)).cuda() if decoy else None
     lines, worst = [], []
     assert E != N, "node and edge rows must be told apart by their count"
     row_frag = {N: batch, E: batch[ei[1].numpy()], G: np.arange(G)}
@@ -89,7 +156,7 @@ def stage_report(frags="chig", weights="real", max_frags=0, opts="", calibrate=F
         detail["fragments"] = per_frag
         detail["kernels"] = eng.stage_kernels()
         detail["options"] = {k: eng.get_option(k) for k in ("tile_rows", "tc_rows", "gxa_parts", "node_tc", "node_nb",
-                                                             "edge_tc", "npw")}
+                                                             "edge_tc", "npw", "use_pdl")}
         detail["n_edges"], detail["n_atoms"], detail["max_degree"] = E, N, int(deg.max())
 
     def report(stage, what, got, ref):
@@ -111,6 +178,8 @@ def stage_report(frags="chig", weights="real", max_frags=0, opts="", calibrate=F
         per_frag.append((stage, text, 0.0 if ok else float("inf"), 0))
 
     def rd(name, layer, shape):
+        if not derivative and name in PER_LAYER:
+            layer = energy_slot_layer(name, layer)
         return eng.debug_read(name, layer, shape)
 
     def cat(*xs):
@@ -144,6 +213,8 @@ def stage_report(frags="chig", weights="real", max_frags=0, opts="", calibrate=F
             report(st, "g_tu", rd("GTU", 0, (N, 3, 2 * D)), cat(B[f"g_t{l}"], B[f"g_u{l}"]))
 
     for si, st in enumerate(names):
+        if ddecoy is not None:
+            eng.debug_run(ddecoy.data_ptr(), -1)
         eng.debug_run(dpos.data_ptr(), si + 1)
         if st == "nbr_build":
             s2, d2 = eng.get_edges()
@@ -198,8 +269,9 @@ def stage_report(frags="chig", weights="real", max_frags=0, opts="", calibrate=F
                 report(st, f"f_in{l+1}", rd("F", l + 1, (N * 32, D))[:E], S[f"f_in{l+1}"])
         elif st == "head":
             report(st, "e_atom", rd("eatom", 0, (N,)), S["e_atom"][:, 0])
-            report(st, "gx_out", rd("GX", 0, (N, D)), B["gx_out"])
-            report(st, "gvec_out", rd("GVEC", 0, (N, 3, D)), B["gvec_out"])
+            if derivative:                       # the energy plan's head stops at the per-atom energies
+                report(st, "gx_out", rd("GX", 0, (N, D)), B["gx_out"])
+                report(st, "gvec_out", rd("GVEC", 0, (N, 3, D)), B["gvec_out"])
         elif st in ("energy_reduce", "finalize"):
             report(st, "E", rd("energy", 0, (eng.n_graphs,)), S["E"][:, 0])
         elif st.startswith("node_bwd"):
@@ -213,9 +285,16 @@ def stage_report(frags="chig", weights="real", max_frags=0, opts="", calibrate=F
             report(st, "g_d", ea[:, 1:4] * S["mask"][:, None], B["g_d"] * S["mask"][:, None])
             report(st, "forces", rd("forces", 0, (N, 3)), B["forces"])
     # full evaluation through the public host entry
-    e, f = eng.forward_host(pos)
-    report("forward_host", "E", e, S["E"][:, 0])
-    report("forward_host", "forces", f, B["forces"])
+    if ddecoy is not None:
+        eng.debug_run(ddecoy.data_ptr(), -1)
+    if derivative:
+        e, f = eng.forward_host(pos)
+        report("forward_host", "E", e, S["E"][:, 0])
+        report("forward_host", "forces", f, B["forces"])
+    else:
+        report("energy_host", "E", eng.energy_host(pos), S["E"][:, 0])
+    if detail is not None:
+        detail["options"]["use_pdl_after"] = eng.get_option("use_pdl")
     return lines, worst
 
 
@@ -227,8 +306,11 @@ def main():
     ap.add_argument("--out", default="")
     ap.add_argument("--opts", default="", help="comma list key=value for vb_set_option")
     ap.add_argument("--calibrate", action="store_true", help="plan the edge tiles from the real edge count first")
+    ap.add_argument("--decoy", default=None, choices=["dense", "nan"], help="evaluate a decoy geometry before each prefix")
+    ap.add_argument("--energy", action="store_true", help="check the energy plan on a derivative = 0 handle")
     args = ap.parse_args()
-    lines, _ = stage_report(args.frags, args.weights, args.max_frags, args.opts, args.calibrate)
+    lines, _ = stage_report(args.frags, args.weights, args.max_frags, args.opts, args.calibrate, decoy=args.decoy,
+                            derivative=not args.energy)
     text = "\n".join(lines)
     print(text)
     if args.out:
