@@ -37,27 +37,32 @@ class ViSNetModel:
     """Energy and forces of a packed fragment batch with the ViSNet potential on one H100.
 
     ``derivative=False`` is the reference's ``ViSNet(derivative=False)``: energies only, on a forward-only engine
-    (``dl_potential_loader`` returns ``(e, None)``)."""
+    (``dl_potential_loader`` returns ``(e, None)``).  ``chunk_size`` is the reference's ``--chunk-size``: the batch is
+    evaluated in contiguous fragment chunks of about that many atoms on one workspace sized for the largest chunk
+    (``Engine(chunk_atoms=...)``); None or 0 evaluates it in one pass."""
 
     implemented_properties = ["energy", "forces"]
 
-    def __init__(self, state_dict: Dict[str, np.ndarray], device: str = "cuda:0", derivative: bool = True):
+    def __init__(self, state_dict: Dict[str, np.ndarray], device: str = "cuda:0", derivative: bool = True,
+                 chunk_size: Optional[int] = None):
         self.device = device
         self.derivative = bool(derivative)
-        self.engine = Engine(state_dict, _device_index(device), derivative=self.derivative)
+        self.engine = Engine(state_dict, _device_index(device), derivative=self.derivative, chunk_atoms=int(chunk_size or 0))
         self._topo_key = None
         if not self.derivative:
             self.implemented_properties = ["energy"]
 
     @classmethod
     def from_file(cls, **kwargs):
-        """``from_file(model_path=..., device=..., derivative=None)``: ``derivative`` follows the reference's
-        ``load_model(path, derivative=...)`` -- the checkpoint's hyper-parameter unless given (an ``.npz`` counts as True)."""
+        """``from_file(model_path=..., device=..., derivative=None, chunk_size=None)``: ``derivative`` follows the
+        reference's ``load_model(path, derivative=...)`` -- the checkpoint's hyper-parameter unless given (an ``.npz``
+        counts as True)."""
         if "model_path" not in kwargs:
             raise ValueError("model_path must be provided")
         sd, ckpt_derivative = load_checkpoint(kwargs["model_path"])
         return cls(sd, device=kwargs.get("device", "cuda:0"),
-                   derivative=resolve_derivative(ckpt_derivative, kwargs.get("derivative")))
+                   derivative=resolve_derivative(ckpt_derivative, kwargs.get("derivative")),
+                   chunk_size=kwargs.get("chunk_size"))
 
     @classmethod
     def from_engine(cls, engine: Engine, device: str, frag: FragmentData):
@@ -109,12 +114,16 @@ class ViSNetModel:
 _local_calc: Dict[str, ViSNetModel] = {}
 
 
-def get_visnet_model(model_path: str, device: str, derivative: Optional[bool] = None) -> ViSNetModel:
-    """One engine per (device, checkpoint[, derivative]); the reference's sub-process proxies
+def get_visnet_model(model_path: str, device: str, derivative: Optional[bool] = None,
+                     chunk_size: Optional[int] = None) -> ViSNetModel:
+    """One engine per (device, checkpoint[, derivative][, chunk size]); the reference's sub-process proxies
     (``ViSNetAsyncModel``) are unnecessary because every engine is in-process and asynchronous."""
     signature = f"{device}-{model_path}" if derivative is None else f"{device}-{model_path}-derivative={bool(derivative)}"
+    if chunk_size:
+        signature += f"-chunk_size={int(chunk_size)}"
     if signature not in _local_calc:
-        _local_calc[signature] = ViSNetModel.from_file(model_path=model_path, device=device, derivative=derivative)
+        _local_calc[signature] = ViSNetModel.from_file(model_path=model_path, device=device, derivative=derivative,
+                                                       chunk_size=chunk_size)
     return _local_calc[signature]
 
 
@@ -153,14 +162,14 @@ class ViSNetCalculator(_CalculatorBase):
     ``get_potential_energy`` only and ``get_forces`` raises ``NotImplementedError``."""
 
     def __init__(self, ckpt_path: str, ckpt_type: str, device: str = "cuda:0", is_root_calc=True,
-                 derivative: Optional[bool] = None, **kwargs):
+                 derivative: Optional[bool] = None, chunk_size: Optional[int] = None, **kwargs):
         super().__init__()
         self.ckpt_path, self.ckpt_type, self.is_root_calc = ckpt_path, ckpt_type, is_root_calc
         model_path = osp.join(ckpt_path, f"visnet-uni-{ckpt_type}.ckpt")
         if not osp.exists(model_path) and osp.exists(ckpt_path) and osp.isfile(ckpt_path):
             model_path = ckpt_path
         self.device = device
-        self.model = get_visnet_model(model_path, device, derivative)
+        self.model = get_visnet_model(model_path, device, derivative, chunk_size)
         self.implemented_properties = list(self.model.implemented_properties)
 
     def calculate(self, atoms, properties, system_changes):
@@ -191,11 +200,14 @@ class DLBondedCalculator:
 
     ``calculate(fragments)`` keeps the reference's return signature (``bonded.py:51-100``).  The
     whole-protein reduction can also run on the device through ``Engine.set_protein_map`` /
-    ``forward_protein_device`` (used by ``parallel.ShardedBondedCalculator`` for the multi-GPU path)."""
+    ``forward_protein_device`` (used by ``parallel.ShardedBondedCalculator`` for the multi-GPU path).
+    ``chunk_size`` is the reference's ``--chunk-size`` (``DeviceStrategy._chunk_size``): the engine evaluates the batch
+    in fragment chunks of about that many atoms, one after the other on one bounded workspace (None: one pass)."""
 
-    def __init__(self, ckpt_path: str, ckpt_type: str = "", device: str = "cuda:0", **kwargs):
+    def __init__(self, ckpt_path: str, ckpt_type: str = "", device: str = "cuda:0", chunk_size: Optional[int] = None,
+                 **kwargs):
         model_path = osp.join(ckpt_path, f"visnet-uni-{ckpt_type}.ckpt") if ckpt_type else ckpt_path
-        self.models = [get_visnet_model(model_path, device)]
+        self.models = [get_visnet_model(model_path, device, chunk_size=chunk_size)]
         if not self.models[0].derivative:
             raise ValueError(f"{model_path}: the bonded calculator needs forces, and the checkpoint has derivative=False")
         self.combiner = DipeptideBondedCombiner()

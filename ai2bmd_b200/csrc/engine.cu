@@ -57,6 +57,9 @@ std::string g_create_error;
 //   [0, fb)        warp per fragment:      energy[g] = float(sum_a eatom[a] + mean)         (visnet.py:146-149)
 //   [fb, fb + pb)  thread per protein atom: ef[3p..] = sum_m sign[m] * forces[src[m]]       (combiner.py:38-39)
 //   fb + pb        one block:               ef[3P]   = sum_g frag_sign[g] * energy[g]       (combiner.py:11-21)
+// A chunked evaluation (option "chunk_atoms") launches it once per chunk without the protein blocks, then once with
+// fb = 0 and from_energy = 1: the energy block then reads the fragment energies every chunk wrote, since ws.eatom holds
+// the last chunk's atoms only.
 // ---------------------------------------------------------------------------------------------------------
 constexpr int FIN_THREADS = 256;
 __device__ __forceinline__ float fragment_energy(const Workspace& ws, int g, float mean, int lane) {
@@ -71,7 +74,7 @@ __global__ void __launch_bounds__(FIN_THREADS) finalize_kernel(Workspace ws, con
                                                                const int* __restrict__ map_src, const float* __restrict__ map_sign,
                                                                const float* __restrict__ frag_sign,
                                                                const float* __restrict__ forces, float* __restrict__ energy,
-                                                               float* __restrict__ ef) {
+                                                               float* __restrict__ ef, int from_energy) {
     pdl_entry();
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const float mean = __ldg(scalars + 1);
@@ -97,7 +100,7 @@ __global__ void __launch_bounds__(FIN_THREADS) finalize_kernel(Workspace ws, con
         __shared__ double red[FIN_THREADS / 32];
         double acc = 0.0;
         for (int g = warp; g < ws.G; g += FIN_THREADS / 32) {
-            const float e = fragment_energy(ws, g, mean, lane);
+            const float e = from_energy ? energy[g] : fragment_energy(ws, g, mean, lane);
             acc += (double)frag_sign[g] * (double)e;
         }
         if (lane == 0) red[warp] = acc;
@@ -170,6 +173,21 @@ struct vb_handle {
     int embed_batch_opt = -1;            // embedding kernels: several nodes per CTA (1), one (0), by size (-1)
     int edge_tc = -1;  // bit 0: forward edge stage on tensor cores, bit 1: adjoint edge stage on tensor cores; -1 = by size
     int derivative = 1;  // 0: forward-only workspace, energies only (the energy plan); read by vb_set_topology
+    int chunk_atoms = 0; // > 0: evaluate the batch as contiguous fragment chunks of about this many atoms on one arena
+                         // sized for the largest chunk; read by vb_set_topology
+    // The launch plan of one pass over a contiguous range of fragments: the workspace view the kernels see and the
+    // kernel choices made from its size.  A chunked handle keeps one per chunk and swaps it into the fields above
+    // while it enqueues that chunk.
+    struct Plan {
+        Workspace ws{};
+        int node_tc = 0, npw = 0, te_fwd = 0, edge_tc = 0, tc_rows = 0, tile_rows = 0;
+        long long edges_plan = 0;
+        int* edge_total = nullptr;   // where rowptr_scan stores the pass's edge total (chunks only)
+        int a0 = 0, g0 = 0;          // first atom and fragment of the chunk in the batch
+    };
+    std::vector<Plan> chunks;    // empty: the batch is one pass (chunk_atoms = 0)
+    int* d_chunk_edges = nullptr;   // [chunks] edge total of each chunk's last evaluation (in the arena)
+    int* edge_total = nullptr;      // the current pass's slot of d_chunk_edges, or none
     // graph cache: one instantiated graph per (kind, I/O pointer set); pointers are baked into the captured launches
     struct GraphEntry { int kind; StepIO io; cudaGraphExec_t exec; };
     std::vector<GraphEntry> graphs;
@@ -266,6 +284,7 @@ struct vb_handle {
         h_pos = h_energy = h_forces = nullptr;
         ws = Workspace{};
         edges_plan = 0;
+        chunks.clear(); d_chunk_edges = edge_total = nullptr;
         stage_names.clear(); stage_kernels.clear(); launches = 0;
     }
 };
@@ -345,9 +364,14 @@ void carve_layers(ArenaPlan& plan, char* base, T** ptr, int layers, size_t count
     for (int l = 0; l < layers; l++) ptr[l] = (own_zero_layer && l == 0) ? slot[2] : slot[l % 2];
 }
 
-void layout_energy_workspace(vb_handle* h, char* base, ArenaPlan& plan) {
+// Batch-wide sizes of a layout: every fragment atom and fragment, and the number of chunks.  The arrays sized by them
+// (topology, neighbour slots, positions, forces and energies) index the whole batch, so vb_get_edges, the MD placement
+// and the hydrogen refinement read them as they do without chunks; everything else is sized by h->ws, the largest chunk.
+struct BatchSizes { size_t N, G, chunks; };
+
+void layout_energy_workspace(vb_handle* h, char* base, ArenaPlan& plan, const BatchSizes& b) {
     Workspace& ws = h->ws;
-    const size_t N = ws.N, G = ws.G, E = ws.Ecap;
+    const size_t N = ws.N, E = ws.Ecap;
     carve_layers(plan, base, ws.X, L + 1, N * D, false);
     carve_layers(plan, base, ws.V, L + 1, N * 3 * D, true);
     carve_layers(plan, base, ws.F, L, E * D, false);
@@ -366,25 +390,26 @@ void layout_energy_workspace(vb_handle* h, char* base, ArenaPlan& plan) {
     carve(plan, base, ws.VA, N * 3 * D);
     carve(plan, base, ws.XN, N * D);
     carve(plan, base, ws.eatom, N);
-    carve(plan, base, h->d_pos, N * 3);
-    carve(plan, base, h->d_energy, G);
+    carve(plan, base, h->d_pos, b.N * 3);
+    carve(plan, base, h->d_energy, b.G);
     h->d_forces = nullptr;
 }
 
-void layout_workspace(vb_handle* h, char* base, ArenaPlan& plan, int*& z, int*& frag_of, int*& frag_start) {
+void layout_workspace(vb_handle* h, char* base, ArenaPlan& plan, const BatchSizes& b, int*& z, int*& frag_of, int*& frag_start) {
     Workspace& ws = h->ws;
-    const size_t N = ws.N, G = ws.G, E = ws.Ecap;
-    carve(plan, base, z, N);
-    carve(plan, base, frag_of, N);
-    carve(plan, base, frag_start, G + 1);
-    carve(plan, base, ws.deg, N);
-    carve(plan, base, ws.slots, N * KNB);
+    const size_t N = ws.N, E = ws.Ecap;
+    carve(plan, base, z, b.N);
+    carve(plan, base, frag_of, b.N);
+    carve(plan, base, frag_start, b.G + b.chunks);          // chunk-local offsets: G_c + 1 per chunk
+    carve(plan, base, ws.deg, b.N);
+    carve(plan, base, ws.slots, b.N * KNB);
+    if (!h->chunks.empty()) carve(plan, base, h->d_chunk_edges, b.chunks);
     carve(plan, base, ws.rowptr, N + 1);
     carve(plan, base, ws.esrc, E);
     carve(plan, base, ws.edst, E);
     carve(plan, base, ws.geom, E * 8);
     carve(plan, base, ws.rbf, E * NR);
-    if (!h->derivative) { layout_energy_workspace(h, base, plan); return; }
+    if (!h->derivative) { layout_energy_workspace(h, base, plan, b); return; }
     carve(plan, base, ws.eacc, E * 4);
     carve(plan, base, ws.grbf, E * NR);
     for (int l = 0; l <= L; l++) { carve(plan, base, ws.X[l], N * D); carve(plan, base, ws.V[l], N * 3 * D); }
@@ -414,9 +439,9 @@ void layout_workspace(vb_handle* h, char* base, ArenaPlan& plan, int*& z, int*& 
     carve(plan, base, ws.GVNMSG, N * 3 * D);
     carve(plan, base, ws.GTU, N * 6 * D);
     carve(plan, base, ws.eatom, N);
-    carve(plan, base, h->d_pos, N * 3);
-    carve(plan, base, h->d_forces, N * 3 + G);          // forces, then the fragment energies: one D2H copy brings both back
-    h->d_energy = h->d_forces ? h->d_forces + N * 3 : nullptr;
+    carve(plan, base, h->d_pos, b.N * 3);
+    carve(plan, base, h->d_forces, b.N * 3 + b.G);      // forces, then the fragment energies: one D2H copy brings both back
+    h->d_energy = h->d_forces ? h->d_forces + b.N * 3 : nullptr;
 }
 
 // ---- launch sequence --------------------------------------------------------------------------------
@@ -451,9 +476,10 @@ struct Launcher {
     std::vector<cudaEvent_t>* events = nullptr;   // optional: one event recorded before every stage
     // dry run: launch() appends the label of the kernel it would launch to the current stage's entry and enqueues nothing
     std::vector<std::string>* kernels = nullptr;
+    std::string prefix;                           // "c<k>/" while a chunk of a chunked evaluation is enqueued
 
     bool next(const char* name) {
-        if (record_names) h->stage_names.push_back(name);
+        if (record_names) h->stage_names.push_back(prefix + name);
         if (limit >= 0 && count >= limit) return false;
         if (events && count < (int)events->size()) cudaEventRecord((*events)[count], st);
         count++;
@@ -718,8 +744,55 @@ void enqueue_finalize(Launcher& Lc, const StepIO& io) {
     const int fb = (ws.G + FIN_THREADS / 32 - 1) / (FIN_THREADS / 32);
     const int pb = prot ? (h->n_protein + FIN_THREADS - 1) / FIN_THREADS : 0;
     Lc.launch(finalize_kernel, dim3(fb + pb + (prot ? 1 : 0)), dim3(FIN_THREADS), 0, ws, h->mw.scalars, fb, pb, h->n_protein,
-              h->d_map_rowptr, h->d_map_src, h->d_map_sign, h->d_frag_sign, io.forces, io.energy, io.ef);
+              h->d_map_rowptr, h->d_map_src, h->d_map_sign, h->d_frag_sign, io.forces, io.energy, io.ef, 0);
     Lc.check();
+}
+
+// The whole-protein reduction of a chunked evaluation, after its last chunk: forces of every fragment atom and the
+// energies every chunk's finalize wrote (h->ws is the batch-wide view here: G is every fragment)
+void enqueue_protein(Launcher& Lc, const StepIO& io) {
+    vb_handle* h = Lc.h;
+    const int pb = (h->n_protein + FIN_THREADS - 1) / FIN_THREADS;
+    Lc.launch(finalize_kernel, dim3(pb + 1), dim3(FIN_THREADS), 0, h->ws, h->mw.scalars, 0, pb, h->n_protein,
+              h->d_map_rowptr, h->d_map_src, h->d_map_sign, h->d_frag_sign, io.forces, io.energy, io.ef, 1);
+    Lc.check();
+}
+
+void plan_save(const vb_handle* h, vb_handle::Plan& p) {
+    p.ws = h->ws;
+    p.node_tc = h->node_tc; p.npw = h->npw; p.te_fwd = h->te_fwd; p.edge_tc = h->edge_tc;
+    p.tc_rows = h->tc_rows; p.tile_rows = h->tile_rows; p.edges_plan = h->edges_plan;
+    p.edge_total = h->edge_total;
+}
+void plan_load(vb_handle* h, const vb_handle::Plan& p) {
+    h->ws = p.ws;
+    h->node_tc = p.node_tc; h->npw = p.npw; h->te_fwd = p.te_fwd; h->edge_tc = p.edge_tc;
+    h->tc_rows = p.tc_rows; h->tile_rows = p.tile_rows; h->edges_plan = p.edges_plan;
+    h->edge_total = p.edge_total;
+}
+
+// Run `pass(io)` once for the whole batch, or, on a chunked handle, once per chunk in order with that chunk's plan
+// swapped in (the launch helpers read the handle's fields) and the I/O buffers offset to its atoms and fragments.
+// Every chunk reuses the one arena, so the chunks run one after the other on the stream.
+template <typename F>
+void each_chunk(Launcher& Lc, const StepIO& io, F&& pass) {
+    vb_handle* h = Lc.h;
+    if (h->chunks.empty()) { pass(io); return; }
+    vb_handle::Plan batch;
+    plan_save(h, batch);
+    for (size_t c = 0; c < h->chunks.size(); c++) {
+        const vb_handle::Plan& k = h->chunks[c];
+        plan_load(h, k);
+        StepIO cio = io;
+        cio.pos = io.pos + 3 * (size_t)k.a0;
+        cio.forces = io.forces ? io.forces + 3 * (size_t)k.a0 : nullptr;
+        cio.energy = io.energy + k.g0;
+        cio.ef = nullptr;
+        Lc.prefix = "c" + std::to_string(c) + "/";
+        pass(cio);
+    }
+    Lc.prefix.clear();
+    plan_load(h, batch);
 }
 
 // Embedding bit of option "embed_batch": several nodes per CTA share the embedding weights (bit 0 forward kernel, bit 1
@@ -740,7 +813,10 @@ void enqueue_fwd(Launcher& Lc, const StepIO& io) {
                   ws.slots, ws.deg, io.forces);
         Lc.check();
     }
-    if (Lc.next("rowptr_scan")) { Lc.launch(rowptr_scan_kernel, dim3(1), dim3(1024), 0, N, ws.deg, ws.rowptr, ws.Ecap, h->d_flags); Lc.check(); }
+    if (Lc.next("rowptr_scan")) {
+        Lc.launch(rowptr_scan_kernel, dim3(1), dim3(1024), 0, N, ws.deg, ws.rowptr, ws.Ecap, h->d_flags, h->edge_total);
+        Lc.check();
+    }
     if (Lc.next("edge_geom")) { Lc.launch(edge_geom_kernel, dim3((N + 3) / 4), dim3(128), 0, N, io.pos, h->mw, ws); Lc.check(); }
     if (Lc.next("embed_node")) {
         if (embed_batch(h, 1)) Lc.launch(embed_node_kernel<8>, dim3((N + 7) / 8), dim3(EMB_THREADS), 0, h->mw, ws);
@@ -770,8 +846,8 @@ void enqueue_fwd(Launcher& Lc, const StepIO& io) {
     if (Lc.next("head")) head(Lc);
 }
 
-// Enqueue one full evaluation (energy + forces [+ whole-protein reduction]) on Lc.st with the given I/O buffers.
-void enqueue_all(Launcher& Lc, const StepIO& io) {
+// Enqueue one full pass (energy + forces [+ whole-protein reduction]) over the fragments of h->ws.
+void enqueue_pass(Launcher& Lc, const StepIO& io) {
     vb_handle* h = Lc.h;
     Workspace& ws = h->ws;
     const int N = ws.N;
@@ -805,6 +881,12 @@ void enqueue_all(Launcher& Lc, const StepIO& io) {
     if (Lc.next("finalize")) enqueue_finalize(Lc, io);
 }
 
+// Enqueue one full evaluation (energy + forces [+ whole-protein reduction]) on Lc.st with the given I/O buffers.
+void enqueue_all(Launcher& Lc, const StepIO& io) {
+    each_chunk(Lc, io, [&](const StepIO& cio) { enqueue_pass(Lc, cio); });
+    if (!Lc.h->chunks.empty() && io.ef && Lc.next("protein")) enqueue_protein(Lc, io);
+}
+
 // The workspace as the energy plan sees it: the adjoint's buffers are null, so nbr_build zeroes no forces, edge_geom no
 // eacc, and the head ends after the per-atom energies (no GX / GVEC).  The edge kernels still store their pre-activations
 // (P1 / SP / ATT): into the layer's own buffers on a derivative = 1 handle, into one shared scratch slot with derivative = 0.
@@ -819,14 +901,16 @@ Workspace energy_workspace(Workspace ws) {
 // No forces (nbr_build zeroes none) and no whole-protein reduction.
 void enqueue_energy(Launcher& Lc, const StepIO& io) {
     vb_handle* h = Lc.h;
-    const Workspace full = h->ws;
-    h->ws = energy_workspace(full);     // the launch helpers pass h->ws by value; restored below
     StepIO eio = io;
     eio.forces = nullptr;
     eio.ef = nullptr;
-    enqueue_fwd(Lc, eio);
-    if (Lc.next("finalize")) enqueue_finalize(Lc, eio);
-    h->ws = full;
+    each_chunk(Lc, eio, [&](const StepIO& cio) {
+        const Workspace full = h->ws;
+        h->ws = energy_workspace(full);     // the launch helpers pass h->ws by value; restored below
+        enqueue_fwd(Lc, cio);
+        if (Lc.next("finalize")) enqueue_finalize(Lc, cio);
+        h->ws = full;
+    });
 }
 
 // The plan a handle evaluates by default: the full one, or the energy plan when it was set up with derivative = 0
@@ -1049,6 +1133,27 @@ void choose_defaults(vb_handle* h) {
     plan_tiles(h, h->edges_plan > 0 ? h->edges_plan : (long long)N * 17);
 }
 
+// Every chunk's kernel choices from its own atom count (and its own calibrated edge count) by the rules above, after
+// the topology or an option changed; the batch-wide fields stay as choose_defaults set them for the whole batch.
+void plan_chunks(vb_handle* h) {
+    vb_handle::Plan batch;
+    plan_save(h, batch);
+    for (auto& k : h->chunks) {
+        plan_load(h, k);
+        choose_defaults(h);
+        plan_save(h, k);
+    }
+    plan_load(h, batch);
+}
+
+// the stage diagnostics launch an evaluation stage by stage, which a chunked handle has once per chunk
+int refuse_chunked(vb_handle* h, const char* who) {
+    if (h->chunks.empty()) return VB_OK;
+    h->set_error("%s: the handle evaluates its batch in %d chunks (option chunk_atoms = %d); the stage diagnostics run on "
+                 "an unchunked handle (chunk_atoms = 0)", who, (int)h->chunks.size(), h->chunk_atoms);
+    return VB_ERR_STATE;
+}
+
 }  // namespace
 
 // =====================================================================================================
@@ -1156,15 +1261,33 @@ int vb_set_topology(vb_handle* h, int64_t n_atoms, int64_t n_graphs, const int64
         frag_start[g + 1]++;
     }
     for (int64_t g = 0; g < n_graphs; g++) frag_start[g + 1] += frag_start[g];
+    // chunks [bounds[c], bounds[c + 1]) of fragments: the whole batch unless option chunk_atoms is set.  Each chunk's
+    // kernels index its own atoms and fragments from 0, so frag_of / frag_start are stored chunk-local (frag_start with
+    // G_c + 1 entries per chunk).
+    std::vector<int64_t> bounds(n_graphs + 1), fs64(frag_start.begin(), frag_start.end());
+    int nc = 1;
+    bounds[0] = 0; bounds[1] = n_graphs;
+    if (h->chunk_atoms > 0) nc = vb_chunk_fragments(n_graphs, fs64.data(), h->chunk_atoms, bounds.data());
+    std::vector<int> lfs(n_graphs + nc);
+    int64_t n_max = 0, g_max = 0, e_max = 0;
+    auto capacity = [&](int64_t n) { return (max_edges > 0 && max_edges < n * KNB) ? max_edges : n * KNB; };
+    for (int c = 0; c < nc; c++) {
+        const int64_t g0 = bounds[c], g1 = bounds[c + 1], a0 = frag_start[g0], a1 = frag_start[g1];
+        for (int64_t g = g0; g <= g1; g++) lfs[g + c] = (int)(frag_start[g] - a0);
+        for (int64_t a = a0; a < a1; a++) frag_of[a] -= (int)g0;
+        n_max = std::max(n_max, a1 - a0); g_max = std::max(g_max, g1 - g0); e_max = std::max(e_max, capacity(a1 - a0));
+    }
     CUDA_TRY(h, cudaSetDevice(h->device));
     h->clear_topology();
-    h->ws.N = (int)n_atoms;
-    h->ws.G = (int)n_graphs;
-    const int64_t worst = n_atoms * KNB;
-    h->ws.Ecap = (int)((max_edges > 0 && max_edges < worst) ? max_edges : worst);
+    if (h->chunk_atoms > 0) h->chunks.resize(nc);
+    // the arena holds one pass of the largest chunk (the whole batch without chunks) plus the batch-wide arrays
+    h->ws.N = (int)n_max;
+    h->ws.G = (int)g_max;
+    h->ws.Ecap = (int)e_max;
+    const BatchSizes bs{(size_t)n_atoms, (size_t)n_graphs, (size_t)nc};
     int *dz = nullptr, *dfo = nullptr, *dfs = nullptr;
     ArenaPlan dry;
-    layout_workspace(h, nullptr, dry, dz, dfo, dfs);
+    layout_workspace(h, nullptr, dry, bs, dz, dfo, dfs);
     h->arena_bytes = dry.off;
     if (cudaMalloc(&h->arena, h->arena_bytes) != cudaSuccess) {
         cudaGetLastError();
@@ -1173,19 +1296,34 @@ int vb_set_topology(vb_handle* h, int64_t n_atoms, int64_t n_graphs, const int64
         return VB_ERR_ALLOC;
     }
     ArenaPlan real;
-    layout_workspace(h, h->arena, real, dz, dfo, dfs);
+    layout_workspace(h, h->arena, real, bs, dz, dfo, dfs);
     h->ws.z = dz; h->ws.frag_of = dfo; h->ws.frag_start = dfs;
+    h->ws.N = (int)n_atoms;
+    h->ws.G = (int)n_graphs;
+    for (int c = 0; c < (int)h->chunks.size(); c++) {        // each chunk's view of the batch-wide arrays
+        vb_handle::Plan& k = h->chunks[c];
+        k.g0 = (int)bounds[c]; k.a0 = frag_start[k.g0];
+        k.ws = h->ws;
+        k.ws.N = frag_start[bounds[c + 1]] - k.a0;
+        k.ws.G = (int)(bounds[c + 1] - bounds[c]);
+        k.ws.Ecap = (int)capacity(k.ws.N);
+        k.ws.z += k.a0; k.ws.frag_of += k.a0; k.ws.frag_start += k.g0 + c;
+        k.ws.deg += k.a0; k.ws.slots += (size_t)k.a0 * KNB;
+        k.edge_total = h->d_chunk_edges + c;
+    }
     CUDA_TRY(h, cudaMemset(h->arena, 0, h->arena_bytes));
+    h->accum_dirty = false;          // the zeroed arena holds no accumulator a truncated diagnostic run left behind
     if (!h->d_flags) CUDA_TRY(h, cudaMalloc(&h->d_flags, sizeof(int) * 4));
     CUDA_TRY(h, cudaMemset(h->d_flags, 0, sizeof(int) * 4));
     CUDA_TRY(h, cudaMemcpy(dz, z.data(), sizeof(int) * n_atoms, cudaMemcpyHostToDevice));
     CUDA_TRY(h, cudaMemcpy(dfo, frag_of.data(), sizeof(int) * n_atoms, cudaMemcpyHostToDevice));
-    CUDA_TRY(h, cudaMemcpy(dfs, frag_start.data(), sizeof(int) * (n_graphs + 1), cudaMemcpyHostToDevice));
+    CUDA_TRY(h, cudaMemcpy(dfs, lfs.data(), sizeof(int) * lfs.size(), cudaMemcpyHostToDevice));
     CUDA_TRY(h, cudaMallocHost(&h->h_pos, sizeof(float) * 3 * n_atoms));
     const int64_t n_force = h->derivative ? 3 * n_atoms : 0;
     CUDA_TRY(h, cudaMallocHost(&h->h_forces, sizeof(float) * (n_force + n_graphs)));   // forces, then energies (one copy)
     h->h_energy = h->h_forces + n_force;
     choose_defaults(h);
+    plan_chunks(h);
     record_stages(h);
     h->has_topology = true;
     return VB_OK;
@@ -1206,9 +1344,26 @@ int vb_forward(vb_handle* h, const float* pos_dev, float* energy_dev, float* for
 
 namespace {
 int check_edge_overflow(vb_handle* h, const char* who) {
-    if ((int64_t)h->ws.Ecap >= (int64_t)h->ws.N * KNB) return VB_OK;      // worst-case capacity: cannot overflow
+    bool trimmed = (int64_t)h->ws.Ecap < (int64_t)h->ws.N * KNB;
+    if (!h->chunks.empty()) {
+        trimmed = false;
+        for (const auto& k : h->chunks) trimmed = trimmed || (int64_t)k.ws.Ecap < (int64_t)k.ws.N * KNB;
+    }
+    if (!trimmed) return VB_OK;      // worst-case capacity: cannot overflow
     int flag = 0;
     CUDA_TRY(h, cudaMemcpy(&flag, h->d_flags, sizeof(int), cudaMemcpyDeviceToHost));
+    if (flag && !h->chunks.empty()) {
+        std::vector<int> total(h->chunks.size());
+        CUDA_TRY(h, cudaMemcpy(total.data(), h->d_chunk_edges, sizeof(int) * total.size(), cudaMemcpyDeviceToHost));
+        for (size_t c = 0; c < total.size(); c++) {
+            const vb_handle::Plan& k = h->chunks[c];
+            if (total[c] > k.ws.Ecap) {
+                h->set_error("%s: chunk %zu (fragments [%d, %d), %d atoms) produced %d edges, more than the max_edges = %d "
+                             "given to vb_set_topology (results invalid)", who, c, k.g0, k.g0 + k.ws.G, k.ws.N, total[c], k.ws.Ecap);
+                return VB_ERR_STATE;
+            }
+        }
+    }
     if (flag) {
         h->set_error("%s: a step produced more edges than the max_edges = %d given to vb_set_topology (results invalid)", who, h->ws.Ecap);
         return VB_ERR_STATE;
@@ -1960,10 +2115,36 @@ int vb_get_edges(vb_handle* h, int32_t* slots_host, int32_t* deg_host) {
     CUDA_TRY(h, cudaDeviceSynchronize());
     CUDA_TRY(h, cudaMemcpy(slots_host, h->ws.slots, sizeof(int) * (size_t)h->ws.N * KNB, cudaMemcpyDeviceToHost));
     CUDA_TRY(h, cudaMemcpy(deg_host, h->ws.deg, sizeof(int) * (size_t)h->ws.N, cudaMemcpyDeviceToHost));
+    for (const auto& k : h->chunks)           // a chunk's kernels store its own atom indices: batch indices here
+        for (size_t i = (size_t)k.a0 * KNB; i < (size_t)(k.a0 + k.ws.N) * KNB; i++)
+            if (slots_host[i] >= 0) slots_host[i] += k.a0;
     return VB_OK;
 }
 
 int vb_launches_per_forward(const vb_handle* h) { return h ? h->launches : 0; }
+
+int vb_chunk_fragments(int64_t n_graphs, const int64_t* frag_start_host, int64_t chunk_atoms, int64_t* out_bounds) {
+    if (n_graphs <= 0 || !frag_start_host || !out_bounds || chunk_atoms < 0 || frag_start_host[0] < 0) return VB_ERR_ARG;
+    const int64_t* fs = frag_start_host;
+    for (int64_t g = 0; g < n_graphs; g++)
+        if (fs[g + 1] < fs[g]) return VB_ERR_ARG;
+    int64_t n = 0;
+    out_bounds[0] = 0;
+    if (chunk_atoms == 0) { out_bounds[1] = n_graphs; return 1; }
+    for (int64_t lo = 0; lo < n_graphs;) {
+        // the fragment boundary nearest to start[lo] + chunk: the last fragment starting at or before it is cut off
+        // when the target lies nearer to its start than to its end (device_strategy.py, the chunk loop)
+        const int64_t target = fs[lo] + chunk_atoms;
+        int64_t hi = std::upper_bound(fs, fs + n_graphs, target) - fs;
+        if (target - fs[hi - 1] < fs[hi] - target) hi--;
+        hi = std::max(hi, lo + 1);                              // at least one fragment ...
+        while (hi < n_graphs && fs[hi] == fs[lo]) hi++;         // ... and at least one atom
+        out_bounds[++n] = hi;
+        lo = hi;
+    }
+    if (n > 1 && fs[out_bounds[n - 1]] == fs[n_graphs]) out_bounds[--n] = n_graphs;   // trailing empty fragments join the last chunk
+    return (int)n;
+}
 
 int vb_set_option(vb_handle* h, const char* key, int64_t value) {
     if (!h || !key) return VB_ERR_ARG;
@@ -1983,11 +2164,15 @@ int vb_set_option(vb_handle* h, const char* key, int64_t value) {
         // re-plan the tile length from the edge count of the last evaluation (synchronises)
         if (!h->has_topology) { h->set_error("vb_set_option: calibrate needs a topology"); return VB_ERR_STATE; }
         int e = 0;
+        std::vector<int> total(h->chunks.size());    // chunked: every chunk's own count (plan_chunks below re-plans)
         if (cudaSetDevice(h->device) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess ||
-            cudaMemcpy(&e, h->ws.rowptr + h->ws.N, sizeof(int), cudaMemcpyDeviceToHost) != cudaSuccess) {
+            (total.empty() && cudaMemcpy(&e, h->ws.rowptr + h->ws.N, sizeof(int), cudaMemcpyDeviceToHost) != cudaSuccess) ||
+            (!total.empty() && cudaMemcpy(total.data(), h->d_chunk_edges, sizeof(int) * total.size(), cudaMemcpyDeviceToHost) != cudaSuccess)) {
             h->set_error("vb_set_option: calibrate failed: %s", cudaGetErrorString(cudaGetLastError()));
             return VB_ERR_CUDA;
         }
+        for (size_t c = 0; c < total.size(); c++)
+            if (total[c] > 0) h->chunks[c].edges_plan = total[c];
         if (e > 0) plan_tiles(h, e);
     }
     else if (k == "node_nb" && (value == 0 || value == 1 || value == 2 || value == 3 || value == 4 || value == 8)) h->node_nb = (int)value;
@@ -2003,8 +2188,25 @@ int vb_set_option(vb_handle* h, const char* key, int64_t value) {
         h->derivative = (int)value;
         h->clear_topology();
     }
+    else if (k == "chunk_atoms" && value >= 0 && value <= (1 << 30)) {
+        // the arena is sized for the largest chunk: drop the topology as "derivative" does
+        if (value > 0 && h->timeline) {
+            h->set_error("vb_set_option: chunk_atoms: the in-kernel timeline (option timeline = 1) describes one unchunked pass");
+            return VB_ERR_STATE;
+        }
+        if (cudaSetDevice(h->device) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess) {
+            h->set_error("vb_set_option: chunk_atoms: %s", cudaGetErrorString(cudaGetLastError()));
+            return VB_ERR_CUDA;
+        }
+        h->chunk_atoms = (int)value;
+        h->clear_topology();
+    }
     else if (k == "embed_batch" && value >= -1 && value <= 3) h->embed_batch_opt = (int)value;
     else if (k == "timeline" && (value == 0 || value == 1)) {
+        if (value && h->chunk_atoms > 0) {
+            h->set_error("vb_set_option: timeline: the handle evaluates in chunks (option chunk_atoms = %d)", h->chunk_atoms);
+            return VB_ERR_STATE;
+        }
         if (value && !h->d_tl) {
             if (cudaSetDevice(h->device) != cudaSuccess || cudaMalloc(&h->d_tl, sizeof(unsigned long long) * (2 * L * TC_TL_SLOTS + (2 * L + 3) * N2_TL_SLOTS)) != cudaSuccess) {
                 h->set_error("vb_set_option: timeline buffer allocation failed"); return VB_ERR_CUDA;
@@ -2015,6 +2217,7 @@ int vb_set_option(vb_handle* h, const char* key, int64_t value) {
     }
     else { h->set_error("vb_set_option: unknown key or bad value: %s", key); return VB_ERR_ARG; }
     h->drop_graph();
+    if (h->has_topology) plan_chunks(h);
     if (h->has_topology) record_stages(h);
     return VB_OK;
 }
@@ -2069,6 +2272,37 @@ int64_t vb_get_option(const vb_handle* h, const char* key) {
     if (k == "tile_rows") return h->tile_rows;
     if (k == "n_edges_capacity") return h->ws.Ecap;
     if (k == "gxa_parts") return h->ws.gxa_parts;
+    if (k == "chunk_atoms") return h->chunk_atoms;
+    if (k == "chunks") return h->has_topology ? std::max<int64_t>(1, (int64_t)h->chunks.size()) : 0;
+    // "c<k>/<key>": the plan of chunk k (an unchunked handle is its own chunk 0), e.g. "c1/tile_rows"
+    int c = -1, n = 0;
+    if (h->has_topology && sscanf(key, "c%d/%n", &c, &n) == 1 && n > 0 && c >= 0 &&
+        c < std::max(1, (int)h->chunks.size())) {
+        vb_handle::Plan p;
+        if (h->chunks.empty()) plan_save(h, p);
+        else p = h->chunks[c];
+        const std::string f(key + n);
+        if (f == "atoms") return p.ws.N;
+        if (f == "graphs") return p.ws.G;
+        if (f == "first_atom") return p.a0;
+        if (f == "first_graph") return p.g0;
+        if (f == "n_edges_capacity") return p.ws.Ecap;
+        if (f == "node_tc") return p.node_tc;
+        if (f == "npw") return p.npw;
+        if (f == "te_fwd") return p.te_fwd;
+        if (f == "edge_tc") return p.edge_tc;
+        if (f == "tc_rows") return p.tc_rows;
+        if (f == "tile_rows") return p.tile_rows;
+        if (f == "gxa_parts") return p.ws.gxa_parts;
+        if (f == "edges_plan") return p.edges_plan;
+        if (f == "edges") {          // the edge count of the chunk's last evaluation (synchronises)
+            int e = 0;
+            const int* src = h->chunks.empty() ? h->ws.rowptr + h->ws.N : h->d_chunk_edges + c;
+            if (cudaSetDevice(h->device) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess ||
+                cudaMemcpy(&e, src, sizeof(int), cudaMemcpyDeviceToHost) != cudaSuccess) return VB_ERR_CUDA;
+            return e;
+        }
+    }
     return VB_ERR_ARG;
 }
 
@@ -2086,6 +2320,7 @@ int vb_debug_run(vb_handle* h, const float* pos_dev, int n_stages) {
     if (!h) return VB_ERR_ARG;
     std::lock_guard<std::mutex> lk(h->mu);
     if (!h->has_topology || !pos_dev) { h->set_error("vb_debug_run: bad state/arguments"); return VB_ERR_STATE; }
+    if (int rc = refuse_chunked(h, "vb_debug_run")) return rc;
     CUDA_TRY(h, cudaSetDevice(h->device));
     CUDA_TRY(h, cudaMemcpy(h->d_pos, pos_dev, sizeof(float) * 3 * h->ws.N, cudaMemcpyDeviceToDevice));
     if (h->accum_dirty) { if (int rc = clean_accumulators(h, h->own_stream)) return rc; }
@@ -2101,6 +2336,7 @@ int vb_profile_stages(vb_handle* h, const float* pos_dev, int n_iter, float* ms_
     if (!h) return VB_ERR_ARG;
     std::lock_guard<std::mutex> lk(h->mu);
     if (!h->has_topology || !pos_dev || !ms_per_stage_host || n_iter <= 0) { h->set_error("vb_profile_stages: bad state/arguments"); return VB_ERR_STATE; }
+    if (int rc = refuse_chunked(h, "vb_profile_stages")) return rc;
     CUDA_TRY(h, cudaSetDevice(h->device));
     const int ns = (int)h->stage_names.size();
     std::vector<cudaEvent_t> ev(ns + 1);
@@ -2174,6 +2410,10 @@ int64_t vb_debug_read(vb_handle* h, const char* name, int layer, void* host_dst,
     const void* src = nullptr;
     size_t bytes = 0;
     const std::string k(name);
+    if (!h->chunks.empty() && k != "energy" && k != "forces" && k != "pos" && k != "RF") {
+        h->set_error("vb_debug_read: %s holds only the last chunk of a chunked handle; energy, forces, pos and RF span the batch", name);
+        return VB_ERR_STATE;
+    }
     if (!h->derivative) {
         for (const char* a : {"P1", "SP", "ATT", "GX", "GVEC", "GF", "GXA", "GXA3", "GQKV", "GVNMSG", "GTU", "eacc", "grbf", "forces"})
             if (k == a) {

@@ -41,8 +41,11 @@ __global__ void __launch_bounds__(128) nbr_build_kernel(int N, const float* __re
 // K2: exclusive scan of deg -> rowptr (single block; N is small enough that this is latency only).
 // A total above the workspace's edge capacity (a caller-trimmed max_edges that a step exceeded) raises flags[0]; the
 // row pointers are clamped to the capacity, so nothing is written out of bounds and the host can report the overflow.
+// `total` (a chunk's slot on a chunked handle, else null) receives the unclamped edge total: calibration and the
+// overflow report of each chunk read it after later chunks have reused rowptr.
 __global__ void __launch_bounds__(1024) rowptr_scan_kernel(int N, const int* __restrict__ deg,
-                                                           int* __restrict__ rowptr, int ecap, int* __restrict__ flags) {
+                                                           int* __restrict__ rowptr, int ecap, int* __restrict__ flags,
+                                                           int* __restrict__ total) {
     pdl_entry();
     __shared__ int wsum[32];
     __shared__ int carry_s;
@@ -80,6 +83,7 @@ __global__ void __launch_bounds__(1024) rowptr_scan_kernel(int N, const int* __r
     if (tid == 0) {
         rowptr[N] = min(carry_s, ecap);
         if (carry_s > ecap) flags[0] = 1;
+        if (total) *total = carry_s;
     }
 }
 

@@ -43,7 +43,7 @@ EXPORTED_SYMBOLS = [
     "vb_md_set_restraints", "vb_md_set_recorder", "vb_md_read_frames",
     "vb_set_nonbonded", "vb_nonbonded",
     "vb_comm_init", "vb_comm_connect", "vb_comm_allreduce",
-    "vb_set_caph", "vb_caph_relax",
+    "vb_set_caph", "vb_caph_relax", "vb_chunk_fragments",
 ]
 
 
@@ -137,6 +137,8 @@ def load_library(path: Optional[str] = None):
     lib.vb_caph_relax.argtypes = [vp, vp, vp]
     lib.vb_md_get_state.restype = C.c_int
     lib.vb_md_get_state.argtypes = [vp, vp, vp, vp, vp, i64]
+    lib.vb_chunk_fragments.restype = C.c_int
+    lib.vb_chunk_fragments.argtypes = [i64, vp, i64, vp]
     if path == _build.LIB_PATH:
         _lib = lib
     return lib
@@ -152,9 +154,16 @@ class Engine:
 
     ``derivative=False`` lays out a forward-only workspace (option ``"derivative"`` = 0): only :meth:`energy_host` /
     :meth:`energy_device` evaluate, the reference's ``ViSNet(derivative=False)``.  With ``derivative=True`` both the
-    force entries and the energy entries work."""
+    force entries and the energy entries work.
 
-    def __init__(self, state_dict: Dict[str, np.ndarray], device: int = 0, cutoff: float = 5.0, derivative: bool = True):
+    ``chunk_atoms=C > 0`` (option ``"chunk_atoms"``) evaluates the batch in contiguous fragment chunks of about C atoms
+    (:func:`ai2bmd_b200.parallel.chunk_fragments`) on one workspace sized for the largest chunk: the reference's
+    ``--chunk-size``, a bound on the engine's device memory.  0 evaluates the batch in one pass."""
+
+    def __init__(self, state_dict: Dict[str, np.ndarray], device: int = 0, cutoff: float = 5.0, derivative: bool = True,
+                 chunk_atoms: int = 0):
+        if int(chunk_atoms) < 0:
+            raise ValueError(f"chunk_atoms must be >= 0, not {chunk_atoms}")
         self.lib = load_library()
         blob = pack_weights(state_dict, self.lib.vb_weight_manifest().decode())
         hp = _HParams(128, 6, 8, 32, 32, cutoff)
@@ -167,6 +176,9 @@ class Engine:
         self.derivative = bool(derivative)
         if not self.derivative:
             self.set_option("derivative", 0)
+        self.chunk_atoms = int(chunk_atoms)
+        if self.chunk_atoms:
+            self.set_option("chunk_atoms", self.chunk_atoms)
         self.n_atoms = 0
         self.n_graphs = 0
         self.n_protein = 0
@@ -212,8 +224,8 @@ class Engine:
 
     def set_option(self, key: str, value: int):
         self._check(self.lib.vb_set_option(self.h, key.encode(), int(value)), "vb_set_option")
-        if key == "derivative":          # the library dropped the topology: set_topology again
-            self.derivative = bool(value)
+        if key in ("derivative", "chunk_atoms"):      # the library dropped the topology: set_topology again
+            setattr(self, key, bool(value) if key == "derivative" else int(value))
             self.n_atoms = self.n_graphs = self.n_protein = 0
 
     def get_option(self, key: str) -> int:

@@ -176,11 +176,14 @@ class DeviceLangevin:
 
     def __init__(self, state_dict, frags: FragmentData, pm: ProteinMap, recipe: FragmentRecipe, positions, numbers,
                  dt_fs=1.0, temperature_K=300.0, friction_per_fs=0.001, seed=0, device: int = 0, velocities=None,
-                 group=None, engine: Engine = None, zero_com_momentum=False, caph=None, step: int = 0):
+                 group=None, engine: Engine = None, zero_com_momentum=False, caph=None, step: int = 0,
+                 chunk_atoms: int = 0):
         """``caph``: an :class:`ai2bmd_b200.caph.CapHProblem` -- the added hydrogens are then refined every step on the
         device (one LBFGS call on the Amber terms, ``csrc/k_caph.cuh``) between their placement and the evaluation.
         ``step``: the step counter to start from; with ``positions`` / ``velocities`` of a frame that ``run_observed``
-        recorded at step s, the run continues with the random numbers the original run drew after s."""
+        recorded at step s, the run continues with the random numbers the original run drew after s.
+        ``chunk_atoms``: the engine this creates evaluates the fragments in chunks of about that many atoms
+        (``Engine(chunk_atoms=...)``); the step stays one graph replay."""
         import torch
         self.torch, self.group = torch, group
         self.n = pm.n_protein
@@ -189,7 +192,7 @@ class DeviceLangevin:
         self.fr = friction_per_fs / FS
         dev = torch.device("cuda", device)
         if engine is None:
-            engine = Engine(state_dict, device)
+            engine = Engine(state_dict, device, chunk_atoms=chunk_atoms)
             engine.set_topology(frags.z, frags.batch, n_graphs=len(frags))
             engine.set_protein_map(pm.n_protein, pm.src_atom, pm.dst_atom, pm.sign, pm.frag_sign)
             engine.forward_host(np.asarray(frags.pos, dtype=np.float32))

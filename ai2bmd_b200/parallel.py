@@ -53,6 +53,32 @@ def partition_fragments(start: Sequence[int], end: Sequence[int], n_parts: int) 
     return out
 
 
+def chunk_fragments(start: Sequence[int], end: Sequence[int], chunk_atoms: int) -> List[Tuple[int, int]]:
+    """Contiguous fragment ranges [lo, hi) of about ``chunk_atoms`` atoms each: the chunk loop of the reference's
+    ``_set_combined_work_partitions`` (``--chunk-size``), applied to one block of packed fragments.
+
+    The rule is the engine's own (``vb_chunk_fragments`` of the C library, which ``Engine(chunk_atoms=...)`` runs): each
+    chunk ends at the fragment boundary nearest to ``start[lo] + chunk_atoms``.  Every chunk takes at least one fragment
+    and one atom, where the reference would loop forever; fragments without atoms go with the chunk they fall in.
+    ``chunk_atoms = 0`` is one chunk.  The fragments must be packed (``end[g] == start[g + 1]``)."""
+    import ctypes as C
+    from .engine import load_library
+    start = np.asarray(start, dtype=np.int64)
+    end = np.asarray(end, dtype=np.int64)
+    if int(chunk_atoms) < 0:
+        raise ValueError(f"chunk_atoms must be >= 0, not {chunk_atoms}")
+    if len(start) == 0 or len(start) != len(end) or (start[1:] != end[:-1]).any():
+        raise ValueError("start / end must describe a non-empty run of packed fragments")
+    offsets = np.ascontiguousarray(np.append(start, end[-1]) - start[0])
+    bounds = np.zeros(len(start) + 1, dtype=np.int64)
+    lib = load_library()
+    n = lib.vb_chunk_fragments(len(start), offsets.ctypes.data_as(C.c_void_p), int(chunk_atoms),
+                               bounds.ctypes.data_as(C.c_void_p))
+    if n < 1:
+        raise ValueError(f"vb_chunk_fragments rejected the fragments ({n})")
+    return [(int(bounds[c]), int(bounds[c + 1])) for c in range(n)]
+
+
 def shard_protein_map(pm: ProteinMap, frags: FragmentData, lo: int, hi: int) -> ProteinMap:
     """Restrict the signed force map to fragments [lo, hi), re-basing fragment-atom indices to the shard."""
     if hi <= lo:
@@ -117,10 +143,13 @@ class DeviceShard:
     With ``native_comm`` (default) the ranks exchange CUDA IPC handles once (``torch.distributed`` is only the host
     transport for those 64 bytes) and every evaluation then ends with the engine's own one-shot all-reduce over NVLink
     peer memory, captured in the step's CUDA graph (``csrc/k_comm.cuh``).  If peer mapping is not possible on this box
-    the ranks fall back -- together -- to ``torch.distributed.all_reduce`` (NCCL) enqueued after the evaluation."""
+    the ranks fall back -- together -- to ``torch.distributed.all_reduce`` (NCCL) enqueued after the evaluation.
+
+    ``chunk_atoms`` > 0 evaluates the rank's block in chunks of about that many atoms (``Engine(chunk_atoms=...)``): the
+    reference's order, blocks per device first, then chunks inside each block."""
 
     def __init__(self, state_dict, frags: FragmentData, pm: ProteinMap, rank: int, world_size: int, device: int,
-                 native_comm: bool = True):
+                 native_comm: bool = True, chunk_atoms: int = 0):
         import torch
         from .engine import Engine
         self.torch = torch
@@ -132,7 +161,7 @@ class DeviceShard:
         self.native = False
         local = self.plan.local_fragments(frags)
         if local is not None:
-            self.engine = Engine(state_dict, device)
+            self.engine = Engine(state_dict, device, chunk_atoms=chunk_atoms)
             self.engine.set_topology(local.z, local.batch, n_graphs=len(local))
             m = self.plan.local_map
             self.engine.set_protein_map(m.n_protein, m.src_atom, m.dst_atom, m.sign, m.frag_sign)

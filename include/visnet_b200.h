@@ -104,6 +104,35 @@ int vb_forward_energy(vb_handle* h, const float* pos_dev, float* energy_dev, voi
  * with VB_ERR_STATE when a step produced more edges than a trimmed max_edges holds. */
 int vb_forward_energy_host(vb_handle* h, const float* pos_host, float* energy_host);
 
+/* ---- Evaluation in fragment chunks (the reference's --chunk-size) -------------------------------------------------
+ * Option "chunk_atoms" (vb_set_option, >= 0, default 0) is read by vb_set_topology, like "derivative", and setting it
+ * drops the topology.  With C > 0 the batch is evaluated as a sequence of contiguous fragment chunks of about C atoms
+ * (vb_chunk_fragments), one after the other on one workspace sized for the largest chunk, so the workspace no longer
+ * grows with the batch: about 700 B per atom of the largest chunk with forces (155 B energy-only), plus about 170 B per
+ * batch atom for the arrays that span the batch (topology, neighbour slots, positions, forces, energies).  Every entry
+ * evaluates the same way -- vb_forward*, vb_forward_energy*, vb_forward_protein (the whole-protein reduction runs once,
+ * after the last chunk) and the MD step -- and all chunks of one evaluation are one CUDA graph replay.  Each chunk gets
+ * its own launch plan from its own size (node / edge stage variants, tile plan; "calibrate" plans each chunk from its
+ * own edge count), and a trimmed max_edges of vb_set_topology is the edge capacity of every chunk (an overflow names
+ * the chunk).  vb_get_option answers "chunk_atoms", "chunks" (the chunk count; 1 without chunks) and, per chunk k,
+ * "c<k>/<key>" with key atoms, graphs, first_atom, first_graph, n_edges_capacity, node_tc, npw, te_fwd, edge_tc,
+ * tc_rows, tile_rows, gxa_parts, edges_plan, or edges (the chunk's edge count in the last evaluation; synchronises).
+ * vb_stage_name / vb_stage_kernel / vb_launches_per_forward list the chunked sequence, stage names prefixed "c<k>/".
+ * A chunked handle refuses vb_debug_run, vb_profile_stages, option "timeline" and vb_debug_read of anything but
+ * "energy", "forces", "pos" and "RF" with VB_ERR_STATE.  C = 0 is exactly the unchunked engine.
+ * Replaces: the chunk loop of DeviceStrategy._set_combined_work_partitions (src/Calculators/device_strategy.py:83-125,
+ *           --chunk-size of src/AIMD/arguments.py:189-197) and the per-chunk dl_potential_loader calls of
+ *           DLBondedCalculator._inference_impl (src/Calculators/bonded.py:46-49,65-77). */
+
+/* The chunk rule, a pure host function (no handle, no device): fragments [0, n_graphs) with atom offsets
+ * frag_start_host[n_graphs + 1] are cut into contiguous chunks; out_bounds[0 .. n] (n_graphs + 1 entries of room)
+ * receives the fragment boundaries of the n chunks, and n is returned (VB_ERR_ARG for a negative chunk_atoms or offsets
+ * that decrease).  Each chunk ends at the fragment boundary nearest to frag_start[first] + chunk_atoms, a tie keeping
+ * the straddling fragment, as the reference does.  Unlike the reference, whose loop never ends once chunk_atoms is
+ * below about half a fragment, every chunk takes at least one fragment and at least one atom: fragments without atoms
+ * go with the chunk they fall in.  chunk_atoms = 0 is one chunk. */
+int vb_chunk_fragments(int64_t n_graphs, const int64_t* frag_start_host, int64_t chunk_atoms, int64_t* out_bounds);
+
 /* ---- Device-resident MD step (SURVEY section 8f, rank 3 and the first half of rank 1) ------------------------
  * State (protein positions / velocities, fp64) stays on the GPU; one step is
  *   kick1 (half-kick + drift) -> eval (place fragment atoms, ViSNet, signed reduction into ef) -> kick2.
