@@ -214,6 +214,9 @@ struct vb_handle {
     bool rs_ready = false;
     MdRestraints rs{};
     void* rs_mem = nullptr;
+    // the reference's noise stream (k_md.cuh MdNoise): state, tables, the step's normals and scratch in one allocation
+    MdNoise nz{};
+    void* nz_mem = nullptr;
     // non-bonded MM term (k_nonbonded.cuh)
     bool nb_ready = false;
     NbParams nb{};
@@ -263,9 +266,14 @@ struct vb_handle {
         cudaFree(rec_mem);
         rec_mem = nullptr; rec = MdRecorder{}; rec_frames_enq = 0;
     }
+    void free_nz() {
+        cudaFree(nz_mem);
+        nz_mem = nullptr; nz = MdNoise{};
+    }
     void free_md() {
         free_rs();                       // the restraints index the MD state
         free_rec();                      // ... and so does the frame ring
+        free_nz();                       // ... and the noise buffers
         cudaFree(d_mx); cudaFree(d_mv); cudaFree(d_mmass); cudaFree(d_ehist);
         cudaFree(d_real); cudaFree(d_acc); cudaFree(d_rem); cudaFree(d_blen); cudaFree(d_step);
         d_mx = d_mv = d_mmass = d_ehist = nullptr; d_real = d_acc = d_rem = nullptr; d_blen = nullptr; d_step = nullptr;
@@ -1526,7 +1534,7 @@ int md_eval_enqueue(vb_handle* h, cudaStream_t st) {
 }
 void md_kick1_enqueue(vb_handle* h, cudaStream_t st) {
     md_kick1_kernel<<<1, MD_K1_THREADS, 0, st>>>(h->md, h->d_step, h->d_mmass, h->md_ef, h->rs.rf, h->d_mx, h->d_mv,
-                                                 h->rec.ctl);
+                                                 h->rec.ctl, h->nz);
 }
 void md_kick2_enqueue(vb_handle* h, cudaStream_t st) {
     md_kick2_kernel<<<1, MD_K2_THREADS, 0, st>>>(h->md, h->d_step, h->d_mmass, h->md_ef, h->rs.rf, h->d_mx, h->d_mv,
@@ -1607,9 +1615,85 @@ int vb_md_set_normals(vb_handle* h, const double* pool_dev, int64_t pool_steps) 
     std::lock_guard<std::mutex> lk(h->mu);
     if (int rc = md_check(h, "vb_md_set_normals")) return rc;
     if ((pool_dev == nullptr) != (pool_steps == 0) || pool_steps < 0) { h->set_error("vb_md_set_normals: bad arguments"); return VB_ERR_ARG; }
+    if (h->nz.kind == 1) {          // the step's normals come from the reference's stream through the pool pointer
+        if (pool_dev == nullptr) return VB_OK;
+        h->set_error("vb_md_set_normals: the reference noise stream is on (vb_md_set_noise kind 1)");
+        return VB_ERR_STATE;
+    }
     h->md.pool = pool_dev;
     h->md.pool_steps = pool_steps;
     h->drop_graph();              // kernel arguments are baked into the captured step
+    return VB_OK;
+}
+
+int vb_md_set_noise(vb_handle* h, int32_t kind, uint64_t state_hi, uint64_t state_lo, uint64_t inc_hi, uint64_t inc_lo,
+                    const double* wi_host, const uint64_t* ki_host, const double* fi_host) {
+    if (!h) return VB_ERR_ARG;
+    std::lock_guard<std::mutex> lk(h->mu);
+    if (int rc = md_check(h, "vb_md_set_noise")) return rc;
+    if ((kind != 0 && kind != 1) || (kind == 1 && (!wi_host || !ki_host || !fi_host || !(inc_lo & 1)))) {
+        h->set_error("vb_md_set_noise: bad arguments (kind 0 or 1; kind 1 needs the three tables and an odd increment)");
+        return VB_ERR_ARG;
+    }
+    if (kind == 1 && h->md.pool != nullptr && h->nz.kind != 1) {
+        h->set_error("vb_md_set_noise: a normals pool is set (vb_md_set_normals); remove it first");
+        return VB_ERR_STATE;
+    }
+    CUDA_TRY(h, cudaSetDevice(h->device));
+    CUDA_TRY(h, cudaDeviceSynchronize());      // no enqueued step may still use the old buffers
+    h->drop_graph();                           // kick1 holds the noise pointers, both kicks the pool pointer
+    if (h->nz.kind == 1) { h->md.pool = nullptr; h->md.pool_steps = 0; }
+    h->free_nz();
+    if (kind == 0) return VB_OK;
+    const size_t n3 = 3 * (size_t)h->n_protein;
+    size_t total = 0;
+    auto carve = [&](size_t bytes) { const size_t o = total; total += (bytes + 255) & ~(size_t)255; return o; };
+    const size_t o_st = carve(4 * sizeof(unsigned long long)), o_wi = carve(256 * sizeof(double)),
+                 o_ki = carve(256 * sizeof(unsigned long long)), o_fi = carve(256 * sizeof(double)),
+                 o_out = carve(2 * n3 * sizeof(double)), o_val = carve(NZ_WIN * sizeof(double)), o_cost = carve(NZ_WIN * sizeof(int));
+    CUDA_TRY(h, cudaMalloc(&h->nz_mem, total));
+    char* base = static_cast<char*>(h->nz_mem);
+    const unsigned long long st[4] = {state_hi, state_lo, inc_hi, inc_lo};
+    CUDA_TRY(h, cudaMemcpy(base + o_st, st, sizeof(st), cudaMemcpyHostToDevice));
+    CUDA_TRY(h, cudaMemcpy(base + o_wi, wi_host, 256 * sizeof(double), cudaMemcpyHostToDevice));
+    CUDA_TRY(h, cudaMemcpy(base + o_ki, ki_host, 256 * sizeof(uint64_t), cudaMemcpyHostToDevice));
+    CUDA_TRY(h, cudaMemcpy(base + o_fi, fi_host, 256 * sizeof(double), cudaMemcpyHostToDevice));
+    CUDA_TRY(h, cudaMemset(base + o_out, 0, 2 * n3 * sizeof(double)));
+    MdNoise& z = h->nz;
+    z.kind = 1;
+    z.state = reinterpret_cast<unsigned long long*>(base + o_st);
+    z.wi = reinterpret_cast<const double*>(base + o_wi);
+    z.ki = reinterpret_cast<const unsigned long long*>(base + o_ki);
+    z.fi = reinterpret_cast<const double*>(base + o_fi);
+    z.out = reinterpret_cast<double*>(base + o_out);
+    z.val = reinterpret_cast<double*>(base + o_val);
+    z.cost = reinterpret_cast<int*>(base + o_cost);
+    h->md.pool = z.out;                        // both kicks read the step's normals as a one-step pool
+    h->md.pool_steps = 1;
+    return VB_OK;
+}
+
+int vb_md_get_noise_state(vb_handle* h, uint64_t* state_out) {
+    if (!h) return VB_ERR_ARG;
+    std::lock_guard<std::mutex> lk(h->mu);
+    if (int rc = md_check(h, "vb_md_get_noise_state", false)) return rc;
+    if (!state_out) { h->set_error("vb_md_get_noise_state: bad arguments"); return VB_ERR_ARG; }
+    if (h->nz.kind != 1) { h->set_error("vb_md_get_noise_state: the reference noise stream is off"); return VB_ERR_STATE; }
+    CUDA_TRY(h, cudaSetDevice(h->device));
+    CUDA_TRY(h, cudaDeviceSynchronize());
+    CUDA_TRY(h, cudaMemcpy(state_out, h->nz.state, 2 * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+    return VB_OK;
+}
+
+int vb_md_get_noise(vb_handle* h, double* normals_host) {
+    if (!h) return VB_ERR_ARG;
+    std::lock_guard<std::mutex> lk(h->mu);
+    if (int rc = md_check(h, "vb_md_get_noise", false)) return rc;
+    if (!normals_host) { h->set_error("vb_md_get_noise: bad arguments"); return VB_ERR_ARG; }
+    if (h->nz.kind != 1) { h->set_error("vb_md_get_noise: the reference noise stream is off"); return VB_ERR_STATE; }
+    CUDA_TRY(h, cudaSetDevice(h->device));
+    CUDA_TRY(h, cudaDeviceSynchronize());
+    CUDA_TRY(h, cudaMemcpy(normals_host, h->nz.out, 6 * (size_t)h->n_protein * sizeof(double), cudaMemcpyDeviceToHost));
     return VB_OK;
 }
 
@@ -2316,13 +2400,25 @@ const char* vb_stage_kernel(const vb_handle* h, int stage) {
     return h->stage_kernels[stage].c_str();
 }
 
+namespace {
+// The caller's positions into d_pos for the debug entries.  The copy runs on the legacy default stream, so it follows
+// the caller's work there; a device-to-device copy returns before it is done, and own_stream (non-blocking) does not
+// wait for the default stream, so it is finished here: otherwise the neighbour list and the geometry of the stages
+// enqueued next can read the previous call's positions.
+int debug_positions(vb_handle* h, const float* pos_dev) {
+    CUDA_TRY(h, cudaMemcpyAsync(h->d_pos, pos_dev, sizeof(float) * 3 * h->ws.N, cudaMemcpyDeviceToDevice, cudaStreamLegacy));
+    CUDA_TRY(h, cudaStreamSynchronize(cudaStreamLegacy));
+    return VB_OK;
+}
+}  // namespace
+
 int vb_debug_run(vb_handle* h, const float* pos_dev, int n_stages) {
     if (!h) return VB_ERR_ARG;
     std::lock_guard<std::mutex> lk(h->mu);
     if (!h->has_topology || !pos_dev) { h->set_error("vb_debug_run: bad state/arguments"); return VB_ERR_STATE; }
     if (int rc = refuse_chunked(h, "vb_debug_run")) return rc;
     CUDA_TRY(h, cudaSetDevice(h->device));
-    CUDA_TRY(h, cudaMemcpy(h->d_pos, pos_dev, sizeof(float) * 3 * h->ws.N, cudaMemcpyDeviceToDevice));
+    if (int rc = debug_positions(h, pos_dev)) return rc;
     if (h->accum_dirty) { if (int rc = clean_accumulators(h, h->own_stream)) return rc; }
     Launcher Lc{h, h->own_stream, n_stages, 0, false};
     enqueue_plan(Lc, internal_io(h, h->n_protein > 0));
@@ -2342,7 +2438,7 @@ int vb_profile_stages(vb_handle* h, const float* pos_dev, int n_iter, float* ms_
     std::vector<cudaEvent_t> ev(ns + 1);
     for (auto& e : ev) CUDA_TRY(h, cudaEventCreate(&e));
     std::vector<double> acc(ns, 0.0);
-    CUDA_TRY(h, cudaMemcpy(h->d_pos, pos_dev, sizeof(float) * 3 * h->ws.N, cudaMemcpyDeviceToDevice));
+    if (int rc = debug_positions(h, pos_dev)) return rc;
     int rc = VB_OK;
     for (int it = 0; it < n_iter + 1 && rc == VB_OK; it++) {      // iteration 0 is an untimed warm-up
         Launcher Lc{h, h->own_stream, -1, 0, false};

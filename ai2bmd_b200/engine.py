@@ -40,7 +40,7 @@ EXPORTED_SYMBOLS = [
     "vb_forward_host", "vb_set_protein_map", "vb_forward_protein", "vb_forward_energy", "vb_forward_energy_host", "vb_get_edges", "vb_launches_per_forward",
     "vb_set_option", "vb_get_option", "vb_num_stages", "vb_stage_name", "vb_stage_kernel", "vb_debug_run", "vb_debug_read", "vb_profile_stages", "vb_tc_selftest", "vb_tc_selftest_rows",
     "vb_md_setup", "vb_md_set_normals", "vb_md_set_state", "vb_md_kick1", "vb_md_eval", "vb_md_kick2", "vb_md_run", "vb_md_get_state",
-    "vb_md_set_restraints", "vb_md_set_recorder", "vb_md_read_frames",
+    "vb_md_set_restraints", "vb_md_set_recorder", "vb_md_read_frames", "vb_md_set_noise", "vb_md_get_noise_state", "vb_md_get_noise",
     "vb_set_nonbonded", "vb_nonbonded",
     "vb_comm_init", "vb_comm_connect", "vb_comm_allreduce",
     "vb_set_caph", "vb_caph_relax", "vb_chunk_fragments",
@@ -110,6 +110,12 @@ def load_library(path: Optional[str] = None):
     lib.vb_md_set_normals.argtypes = [vp, vp, i64]
     lib.vb_md_set_state.restype = C.c_int
     lib.vb_md_set_state.argtypes = [vp, vp, vp, i64]
+    lib.vb_md_set_noise.restype = C.c_int
+    lib.vb_md_set_noise.argtypes = [vp, C.c_int32, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64, vp, vp, vp]
+    lib.vb_md_get_noise_state.restype = C.c_int
+    lib.vb_md_get_noise_state.argtypes = [vp, vp]
+    lib.vb_md_get_noise.restype = C.c_int
+    lib.vb_md_get_noise.argtypes = [vp, vp]
     for name in ("vb_md_kick1", "vb_md_eval", "vb_md_kick2"):
         getattr(lib, name).restype = C.c_int
         getattr(lib, name).argtypes = [vp, vp]
@@ -341,6 +347,33 @@ class Engine:
 
     def md_set_normals(self, pool_ptr: int, pool_steps: int):
         self._check(self.lib.vb_md_set_normals(self.h, pool_ptr, int(pool_steps)), "vb_md_set_normals")
+
+    def md_set_noise(self, kind: int, state: int = 0, inc: int = 1, tables=None):
+        """Noise source of the MD step: 0 Philox (default), 1 the reference's numpy stream from the 128-bit PCG64
+        ``state`` / ``inc`` with numpy's ziggurat ``tables`` (:func:`ai2bmd_b200.refnoise.tables`)."""
+        m = (1 << 64) - 1
+        wi = ki = fi = None
+        if kind == 1:
+            wi = np.ascontiguousarray(tables["wi"], dtype=np.float64)
+            ki = np.ascontiguousarray(tables["ki"], dtype=np.uint64)
+            fi = np.ascontiguousarray(tables["fi"], dtype=np.float64)
+            if wi.shape != (256,) or ki.shape != (256,) or fi.shape != (256,):
+                raise ValueError("ziggurat tables must have 256 entries")
+        ptr = lambda a: None if a is None else a.ctypes.data     # noqa: E731
+        self._check(self.lib.vb_md_set_noise(self.h, int(kind), (state >> 64) & m, state & m, (inc >> 64) & m, inc & m,
+                                             ptr(wi), ptr(ki), ptr(fi)), "vb_md_set_noise")
+
+    def md_get_noise_state(self) -> int:
+        """The reference stream's 128-bit PCG64 state after the last step (synchronises)."""
+        out = np.zeros(2, dtype=np.uint64)
+        self._check(self.lib.vb_md_get_noise_state(self.h, out.ctypes.data), "vb_md_get_noise_state")
+        return (int(out[0]) << 64) | int(out[1])
+
+    def md_get_noise(self):
+        """The last step's normals of the reference stream: (xi, eta), each [n_protein, 3] (synchronises)."""
+        out = np.empty((2, self._md_n, 3), dtype=np.float64)
+        self._check(self.lib.vb_md_get_noise(self.h, out.ctypes.data), "vb_md_get_noise")
+        return out[0], out[1]
 
     def md_set_state(self, x, v, step: int = 0):
         x = np.ascontiguousarray(x, dtype=np.float64)

@@ -68,12 +68,19 @@ class Langevin:
     ``friction=0`` reduces to velocity Verlet (no random numbers, no centre-of-mass handling)."""
 
     def __init__(self, positions, numbers, force_fn, dt_fs=1.0, temperature_K=300.0, friction_per_fs=0.001, seed=0,
-                 normal_source=None, zero_com_momentum=False):
+                 normal_source=None, zero_com_momentum=False, noise="numpy"):
         """``normal_source(step) -> (xi, eta)`` overrides the numpy generator for the per-step normals (used to
         drive this host integrator with the device's Philox stream in the parity tests).  ``zero_com_momentum``
         removes the centre-of-mass momentum of the Maxwell-Boltzmann draw; the reference does not
-        (``simulator.py:96`` calls ``MaxwellBoltzmannDistribution`` only, no ``Stationary``)."""
-        self.normal_source = normal_source
+        (``simulator.py:96`` calls ``MaxwellBoltzmannDistribution`` only, no ``Stationary``).
+
+        ``noise="reference"`` draws as the reference does: the start velocities from ``np.random.RandomState(seed)``
+        (:func:`reference_velocities`) and every step's xi, eta from ``np.random.default_rng(seed)`` in ``RNGPool``
+        order, at friction 0 too (ASE's step draws regardless).  The default ``"numpy"`` takes both from one
+        ``default_rng(seed)`` and draws nothing at friction 0."""
+        if noise not in ("numpy", "reference"):
+            raise ValueError(f"noise must be 'numpy' or 'reference', not {noise!r}")
+        self.normal_source, self.noise = normal_source, noise
         self.nsteps = 0
         self.x = np.array(positions, dtype=np.float64)
         self.m = np.array([MASSES[int(z)] for z in numbers], dtype=np.float64)[:, None]
@@ -83,7 +90,10 @@ class Langevin:
         self.fr = friction_per_fs / FS
         self.rng = np.random.default_rng(seed)
         # Maxwell-Boltzmann start (simulator.py:96)
-        self.v = self.rng.standard_normal(self.x.shape) * np.sqrt(self.T / self.m)
+        if noise == "reference":
+            self.v = reference_velocities(seed, self.m[:, 0], self.T)
+        else:
+            self.v = self.rng.standard_normal(self.x.shape) * np.sqrt(self.T / self.m)
         if zero_com_momentum:
             self.v -= (self.v * self.m).sum(0) / self.m.sum()
         self.energy, self.f = force_fn(self.x)
@@ -105,6 +115,8 @@ class Langevin:
         """(xi, eta) of the current step: from ``normal_source``, else two draws of the numpy generator (0 at friction 0)."""
         if self.fr > 0 and self.normal_source is not None:
             return self.normal_source(self.nsteps)
+        if self.noise == "reference":
+            return self.rng.standard_normal(self.x.shape), self.rng.standard_normal(self.x.shape)
         xi = self.rng.standard_normal(self.x.shape) if self.fr > 0 else 0.0
         eta = self.rng.standard_normal(self.x.shape) if self.fr > 0 else 0.0
         return xi, eta
@@ -138,6 +150,14 @@ class Langevin:
     def run(self, n_steps):
         for _ in range(n_steps):
             self.step()
+
+
+def reference_velocities(seed: int, masses, kT: float):
+    """The reference's start velocities: ASE's ``MaxwellBoltzmannDistribution(atoms, temperature_K,
+    rng=np.random.RandomState(seed))`` (``simulator.py:96``; ASE 3.22, recalled, not pinned), i.e. one
+    ``standard_normal((n, 3))`` of the legacy generator scaled by sqrt(kT / m)."""
+    m = np.asarray(masses, dtype=np.float64)[:, None]
+    return np.random.RandomState(seed).standard_normal((len(m), 3)) * np.sqrt(kT / m)
 
 
 # ---------------------------------------------------------------------------------------------------------
@@ -177,13 +197,22 @@ class DeviceLangevin:
     def __init__(self, state_dict, frags: FragmentData, pm: ProteinMap, recipe: FragmentRecipe, positions, numbers,
                  dt_fs=1.0, temperature_K=300.0, friction_per_fs=0.001, seed=0, device: int = 0, velocities=None,
                  group=None, engine: Engine = None, zero_com_momentum=False, caph=None, step: int = 0,
-                 chunk_atoms: int = 0):
+                 chunk_atoms: int = 0, noise: str = "philox", noise_state: int = None):
         """``caph``: an :class:`ai2bmd_b200.caph.CapHProblem` -- the added hydrogens are then refined every step on the
         device (one LBFGS call on the Amber terms, ``csrc/k_caph.cuh``) between their placement and the evaluation.
         ``step``: the step counter to start from; with ``positions`` / ``velocities`` of a frame that ``run_observed``
         recorded at step s, the run continues with the random numbers the original run drew after s.
         ``chunk_atoms``: the engine this creates evaluates the fragments in chunks of about that many atoms
-        (``Engine(chunk_atoms=...)``); the step stays one graph replay."""
+        (``Engine(chunk_atoms=...)``); the step stays one graph replay.
+        ``noise``: ``"philox"`` (default) draws the step's normals from the counter-based Philox stream keyed by
+        (seed, step); ``"reference"`` draws exactly the numbers the reference's ``RNGPool(seed)`` hands ASE's Langevin
+        (numpy's ``default_rng(seed)``, generated on the device, :mod:`ai2bmd_b200.refnoise`), and the default start
+        velocities are the reference's (:func:`reference_velocities`).  Its stream starts from ``PCG64(seed)`` unless
+        ``noise_state`` (a 128-bit state from :meth:`noise_state`) is given: like the reference's ``--restart``, which
+        builds a fresh ``RNGPool(seed)``, a run started from a recorded frame reseeds unless it is handed the saved
+        state.  Every rank of a sharded run generates the same stream."""
+        if noise not in ("philox", "reference"):
+            raise ValueError(f"noise must be 'philox' or 'reference', not {noise!r}")
         import torch
         self.torch, self.group = torch, group
         self.n = pm.n_protein
@@ -204,11 +233,17 @@ class DeviceLangevin:
         self.stream = torch.cuda.current_stream(dev)
         engine.md_setup(self.masses, recipe.real, recipe.acc, recipe.rem, recipe.blen, dt_fs * FS, self.kT, self.fr,
                         seed, self.ef.data_ptr())
+        if noise == "reference":
+            from . import refnoise
+            s0, inc = refnoise.pcg_state(seed)
+            engine.md_set_noise(1, s0 if noise_state is None else int(noise_state), inc, refnoise.tables())
         x = np.array(positions, dtype=np.float64)
         if velocities is None:      # Maxwell-Boltzmann start, as Langevin above (simulator.py:96)
-            rng = np.random.default_rng(seed)
             m = self.masses[:, None]
-            velocities = rng.standard_normal(x.shape) * np.sqrt(self.kT / m)
+            if noise == "reference":
+                velocities = reference_velocities(seed, self.masses, self.kT)
+            else:
+                velocities = np.random.default_rng(seed).standard_normal(x.shape) * np.sqrt(self.kT / m)
             if zero_com_momentum:
                 velocities -= (velocities * m).sum(0) / m.sum()
         engine.md_set_state(x, velocities, step)
@@ -235,6 +270,11 @@ class DeviceLangevin:
             return
         self._pool = self.torch.as_tensor(np.ascontiguousarray(pool, dtype=np.float64)).to(self.ef.device)
         self.engine.md_set_normals(self._pool.data_ptr(), self._pool.shape[0])
+
+    def noise_state(self) -> int:
+        """The 128-bit PCG64 state of the reference noise stream after the last step (``noise="reference"``;
+        synchronises).  Hand it to a new ``DeviceLangevin(noise_state=...)`` to continue the stream."""
+        return self.engine.md_get_noise_state()
 
     def run(self, n_steps: int):
         sp = self.stream.cuda_stream

@@ -152,8 +152,22 @@ int vb_md_setup(vb_handle* h, int64_t n_protein_atoms, const double* masses_host
                 const int32_t* acc_host, const int32_t* rem_host, const float* blen_host, double dt, double kT,
                 double friction, uint64_t seed, float* ef_prot_dev);
 /* Optional externally supplied normals, device array [pool_steps][2][3*n_protein] (xi, eta), step s reads row
- * s % pool_steps; (NULL, 0) returns to Philox.  For parity tests against a host integrator. */
+ * s % pool_steps; (NULL, 0) returns to Philox.  For parity tests against a host integrator.  VB_ERR_STATE while the
+ * reference noise stream is on (a NULL pool is then accepted and changes nothing). */
 int vb_md_set_normals(vb_handle* h, const double* pool_dev, int64_t pool_steps);
+/* Noise source of the step.  kind 0: the Philox stream above (the default).  kind 1: the reference's stream -- numpy's
+ * np.random.default_rng: PCG64 with the 128-bit state (state_hi, state_lo) and increment (inc_hi, inc_lo, odd) under
+ * numpy's ziggurat with its tables wi[256], ki[256], fi[256] (ai2bmd_b200/refnoise.py recovers them) -- generated on the
+ * device, 2 * 3 * n_protein normals per step (xi, then eta, C order), advancing the state by exactly the draws numpy
+ * consumes; it advances at friction 0 too, and not on a step the frame recorder halted.  Synchronises, drops the
+ * captured step graph; the stream survives vb_md_set_state and is freed with the MD state.  VB_ERR_STATE with a
+ * normals pool set. */
+int vb_md_set_noise(vb_handle* h, int32_t kind, uint64_t state_hi, uint64_t state_lo, uint64_t inc_hi, uint64_t inc_lo,
+                    const double* wi, const uint64_t* ki, const double* fi);
+/* kind 1 only (else VB_ERR_STATE); synchronise.  state_out[2] = (hi, lo) of the PCG64 state after the last step;
+ * normals_host[2 * 3 * n_protein] = the last step's xi, eta. */
+int vb_md_get_noise_state(vb_handle* h, uint64_t* state_out);
+int vb_md_get_noise(vb_handle* h, double* normals_host);
 /* Positions, velocities and the step counter (the normals of step s follow from (seed, s) alone, so a run restarted from
  * a recorded frame draws the random stream the original run drew); synchronises and lifts a halt of the frame recorder. */
 int vb_md_set_state(vb_handle* h, const double* x_host, const double* v_host, int64_t step);
