@@ -204,6 +204,9 @@ struct vb_handle {
     long long* d_step = nullptr;
     long long ehist_cap = 1 << 16;
     float* md_ef = nullptr;              // caller-owned [3*n_protein + 1]
+    // un-fragmented step (vb_md_setup with real_host == NULL): the topology is the protein as one graph, n_protein is the
+    // MD state's (no protein map), and the evaluation writes forces / energy straight into md_ef
+    bool md_unfrag = false;
     // frame recorder (k_md.cuh MdRecorder): control words and the ring in one allocation
     MdRecorder rec{};
     void* rec_mem = nullptr;
@@ -278,6 +281,7 @@ struct vb_handle {
         cudaFree(d_real); cudaFree(d_acc); cudaFree(d_rem); cudaFree(d_blen); cudaFree(d_step);
         d_mx = d_mv = d_mmass = d_ehist = nullptr; d_real = d_acc = d_rem = nullptr; d_blen = nullptr; d_step = nullptr;
         md_ready = false;
+        if (md_unfrag) { md_unfrag = false; n_protein = 0; }   // that n_protein came from vb_md_setup, not from a map
     }
     // drop the topology and everything sized by it (the caller has selected the device)
     void clear_topology() {
@@ -1450,6 +1454,11 @@ int vb_set_protein_map(vb_handle* h, int64_t n_protein_atoms, int64_t n_map, con
     if (!h) return VB_ERR_ARG;
     std::lock_guard<std::mutex> lk(h->mu);
     if (!h->has_topology) { h->set_error("vb_set_protein_map: call vb_set_topology first"); return VB_ERR_STATE; }
+    if (h->md_unfrag) {
+        h->set_error("vb_set_protein_map: the MD step is set up un-fragmented (vb_md_setup with real_host = NULL), which "
+                     "uses no protein map; call vb_set_topology again for a fragment batch");
+        return VB_ERR_STATE;
+    }
     if (n_protein_atoms <= 0 || n_protein_atoms > (1 << 28) || n_map < 0 || !frag_sign_host ||
         (n_map > 0 && (!src_atom_host || !dst_atom_host || !sign_host))) {
         h->set_error("vb_set_protein_map: bad arguments");
@@ -1499,7 +1508,7 @@ int vb_forward_protein(vb_handle* h, const float* pos_dev, float* ef_prot_dev, v
     NvtxRange nvtx_("vb_forward_protein");
     if (!h) return VB_ERR_ARG;
     std::lock_guard<std::mutex> lk(h->mu);
-    if (!h->has_topology || h->n_protein <= 0) { h->set_error("vb_forward_protein: topology / protein map not set"); return VB_ERR_STATE; }
+    if (!h->has_topology || h->n_protein <= 0 || !h->d_map_rowptr) { h->set_error("vb_forward_protein: topology / protein map not set"); return VB_ERR_STATE; }
     if (int rc = need_derivative(h, "vb_forward_protein")) return rc;
     if (!pos_dev || !ef_prot_dev) { h->set_error("vb_forward_protein: null buffer"); return VB_ERR_ARG; }
     CUDA_TRY(h, cudaSetDevice(h->device));
@@ -1512,10 +1521,15 @@ int vb_forward_protein(vb_handle* h, const float* pos_dev, float* ef_prot_dev, v
 namespace {
 StepIO md_io(vb_handle* h) {
     StepIO io = internal_io(h, false);
+    if (h->md_unfrag) {          // one graph over the protein: its forces and energy are ef itself, no reduction
+        io.forces = h->md_ef;
+        io.energy = h->md_ef + 3 * (size_t)h->n_protein;
+        return io;
+    }
     io.ef = h->md_ef;
     return io;
 }
-// fragment placement [+ restraints into rf, one more CTA] -> evaluation + signed whole-protein reduction
+// fragment placement (un-fragmented: the fp32 cast of x) [+ restraints into rf, one more CTA] -> evaluation + signed whole-protein reduction
 // [-> non-bonded term], all on st.  Every rank of a sharded run holds the same state and the whole term set, so each
 // computes the same rf; only ef goes through the all-reduce.
 int md_eval_enqueue(vb_handle* h, cudaStream_t st) {
@@ -1557,6 +1571,45 @@ int md_check(vb_handle* h, const char* who, bool stepping = true) {
     if (!h->md_ready) { h->set_error("%s: call vb_md_setup first", who); return VB_ERR_STATE; }
     return stepping ? comm_check(h, who) : VB_OK;
 }
+
+// vb_md_setup with real_host == NULL: the topology is the protein itself, one graph in protein atom order (the
+// reference's ViSNetCalculator, visnet_calculator.py:138-155).  Called with h->mu held.
+int md_setup_unfragmented(vb_handle* h, int64_t n_protein_atoms, const double* masses_host, double dt, double kT,
+                          double friction, uint64_t seed, float* ef_prot_dev) {
+    auto fail = [&](int rc, const char* what) { h->set_error("vb_md_setup (un-fragmented, real_host = NULL): %s", what); return rc; };
+    if (!h->has_topology) return fail(VB_ERR_STATE, "call vb_set_topology first");
+    if (int rc = need_derivative(h, "vb_md_setup")) return rc;
+    if (h->d_map_rowptr) return fail(VB_ERR_STATE, "a protein map is set, and the un-fragmented step uses none; call vb_set_topology again");
+    if (h->caph_ready) return fail(VB_ERR_STATE, "hydrogen refinement is set (vb_set_caph), and one graph has no added hydrogens");
+    if (h->comm_ready && h->comm.world > 1) return fail(VB_ERR_STATE, "connected to several ranks: one graph cannot be sharded");
+    if (h->ws.G != 1) return fail(VB_ERR_ARG, "the topology must be ONE graph (n_graphs == 1)");
+    if (n_protein_atoms != h->ws.N) return fail(VB_ERR_ARG, "n_protein_atoms must equal the topology's atom count");
+    if (!masses_host || !ef_prot_dev) return fail(VB_ERR_ARG, "null masses or force buffer");
+    if (!(dt > 0.0) || kT < 0.0 || friction < 0.0) return fail(VB_ERR_ARG, "dt must be positive, kT and friction non-negative");
+    const int P = h->ws.N;
+    for (int i = 0; i < P; i++)
+        if (!(masses_host[i] > 0.0)) { h->set_error("vb_md_setup: non-positive mass at atom %d", i); return VB_ERR_ARG; }
+    CUDA_TRY(h, cudaSetDevice(h->device));
+    h->drop_graph();
+    h->free_md();
+    CUDA_TRY(h, cudaMalloc(&h->d_mx, sizeof(double) * 3 * P));
+    CUDA_TRY(h, cudaMalloc(&h->d_mv, sizeof(double) * 3 * P));
+    CUDA_TRY(h, cudaMalloc(&h->d_mmass, sizeof(double) * P));
+    CUDA_TRY(h, cudaMalloc(&h->d_ehist, sizeof(double) * h->ehist_cap));
+    CUDA_TRY(h, cudaMalloc(&h->d_step, sizeof(long long)));
+    CUDA_TRY(h, cudaMemcpy(h->d_mmass, masses_host, sizeof(double) * P, cudaMemcpyHostToDevice));
+    CUDA_TRY(h, cudaMemset(h->d_mx, 0, sizeof(double) * 3 * P));
+    CUDA_TRY(h, cudaMemset(h->d_mv, 0, sizeof(double) * 3 * P));
+    CUDA_TRY(h, cudaMemset(h->d_ehist, 0, sizeof(double) * h->ehist_cap));
+    CUDA_TRY(h, cudaMemset(h->d_step, 0, sizeof(long long)));
+    h->n_protein = P;             // no recipe arrays: md_place_kernel reads real == NULL as the identity
+    h->md_unfrag = true;
+    h->md = MdParams{P, dt, kT, friction, (unsigned long long)seed, nullptr, 0};
+    h->md_ef = ef_prot_dev;
+    h->md_step_enq = 0;
+    h->md_ready = true;
+    return VB_OK;
+}
 }  // namespace
 
 int vb_md_setup(vb_handle* h, int64_t n_protein_atoms, const double* masses_host, const int32_t* real_host,
@@ -1564,7 +1617,8 @@ int vb_md_setup(vb_handle* h, int64_t n_protein_atoms, const double* masses_host
                 double friction, uint64_t seed, float* ef_prot_dev) {
     if (!h) return VB_ERR_ARG;
     std::lock_guard<std::mutex> lk(h->mu);
-    if (!h->has_topology || h->n_protein <= 0) { h->set_error("vb_md_setup: topology / protein map not set"); return VB_ERR_STATE; }
+    if (!real_host) return md_setup_unfragmented(h, n_protein_atoms, masses_host, dt, kT, friction, seed, ef_prot_dev);
+    if (!h->has_topology || h->n_protein <= 0 || !h->d_map_rowptr) { h->set_error("vb_md_setup: topology / protein map not set"); return VB_ERR_STATE; }
     if (int rc = need_derivative(h, "vb_md_setup")) return rc;
     if (n_protein_atoms != h->n_protein || !masses_host || !real_host || !acc_host || !rem_host || !blen_host || !ef_prot_dev ||
         !(dt > 0.0) || kT < 0.0 || friction < 0.0) {
@@ -2023,6 +2077,11 @@ int vb_set_caph(vb_handle* h, const vb_caph_problem* pr) {
     if (!h) return VB_ERR_ARG;
     std::lock_guard<std::mutex> lk(h->mu);
     if (!h->has_topology) { h->set_error("vb_set_caph: call vb_set_topology first"); return VB_ERR_STATE; }
+    if (h->md_unfrag) {
+        h->set_error("vb_set_caph: the MD step is set up un-fragmented (vb_md_setup with real_host = NULL): one graph has "
+                     "no added hydrogens to refine");
+        return VB_ERR_STATE;
+    }
     if (!pr) { h->set_error("vb_set_caph: null problem"); return VB_ERR_ARG; }
     const int64_t N = h->ws.N;
     auto bad = [&](const char* what) { h->set_error("vb_set_caph: %s", what); return VB_ERR_ARG; };
@@ -2158,6 +2217,11 @@ int vb_comm_connect(vb_handle* h, const void* all_handles) {
     if (!h) return VB_ERR_ARG;
     std::lock_guard<std::mutex> lk(h->mu);
     if (!h->comm_base || !all_handles) { h->set_error("vb_comm_connect: call vb_comm_init first"); return VB_ERR_STATE; }
+    if (h->md_unfrag && h->comm.world > 1) {
+        h->set_error("vb_comm_connect: the MD step is set up un-fragmented (vb_md_setup with real_host = NULL): one graph "
+                     "cannot be sharded over %d ranks", h->comm.world);
+        return VB_ERR_STATE;
+    }
     CUDA_TRY(h, cudaSetDevice(h->device));
     const int world = h->comm.world;
     const size_t flag_bytes = ((size_t)2 * world * sizeof(int) + 255) & ~(size_t)255;
@@ -2322,6 +2386,7 @@ int64_t vb_get_option(const vb_handle* h, const char* key) {
     if (k == "derivative") return h->derivative;
     if (k == "arena_bytes") return (int64_t)h->arena_bytes;
     if (k == "caph_ready") return h->caph_ready ? 1 : 0;
+    if (k == "md_unfragmented") return h->md_unfrag ? 1 : 0;
     if (k == "caph_evals") {           // energy evaluations of the last refinement (synchronises)
         int v = 0;
         if (!h->caph_ready || cudaDeviceSynchronize() != cudaSuccess ||

@@ -345,6 +345,16 @@ class Engine:
                     "vb_md_setup")
         self._md_n = len(m)
 
+    def md_setup_unfragmented(self, masses, dt, kT, friction, seed, ef_ptr: int):
+        """The un-fragmented step (``vb_md_setup`` with no placement recipe): the topology is the input as one graph,
+        n_protein = its atom count, and the evaluation writes forces and energy straight into ``ef_ptr``."""
+        m = np.ascontiguousarray(masses, dtype=np.float64)
+        self._md_keep = [m]
+        self._check(self.lib.vb_md_setup(self.h, len(m), m.ctypes.data, None, None, None, None, float(dt), float(kT),
+                                         float(friction), int(seed), ef_ptr), "vb_md_setup")
+        self._md_n = len(m)
+        self.n_protein = len(m)
+
     def md_set_normals(self, pool_ptr: int, pool_steps: int):
         self._check(self.lib.vb_md_set_normals(self.h, pool_ptr, int(pool_steps)), "vb_md_set_normals")
 

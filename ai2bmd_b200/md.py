@@ -16,6 +16,7 @@ from __future__ import annotations
 
 import numpy as np
 
+from .elements import MASSES, masses_of   # noqa: F401  (MASSES: z -> amu, every z the model accepts)
 from .engine import Engine
 from .fragment_data import FragmentData
 from .pdbfrag import FragmentRecipe, ProteinMap
@@ -23,7 +24,6 @@ from .restraints import KCALMOL_EV, PREEQ_SCHEDULE
 
 FS = 0.09822694788464063        # 1 fs in ASE time units
 KB = 8.617330337217213e-05      # eV / K
-MASSES = {1: 1.008, 6: 12.011, 7: 14.007, 8: 15.999, 16: 32.06}
 
 
 class BondedForceField:
@@ -83,7 +83,7 @@ class Langevin:
         self.normal_source, self.noise = normal_source, noise
         self.nsteps = 0
         self.x = np.array(positions, dtype=np.float64)
-        self.m = np.array([MASSES[int(z)] for z in numbers], dtype=np.float64)[:, None]
+        self.m = masses_of(numbers)[:, None]
         self.force_fn = force_fn
         self.dt = dt_fs * FS
         self.T = temperature_K * KB
@@ -216,7 +216,7 @@ class DeviceLangevin:
         import torch
         self.torch, self.group = torch, group
         self.n = pm.n_protein
-        self.masses = np.array([MASSES[int(z)] for z in numbers], dtype=np.float64)
+        self.masses = masses_of(numbers)
         self.kT = temperature_K * KB
         self.fr = friction_per_fs / FS
         dev = torch.device("cuda", device)
@@ -233,6 +233,51 @@ class DeviceLangevin:
         self.stream = torch.cuda.current_stream(dev)
         engine.md_setup(self.masses, recipe.real, recipe.acc, recipe.rem, recipe.blen, dt_fs * FS, self.kT, self.fr,
                         seed, self.ef.data_ptr())
+        self._start(positions, velocities, seed, step, noise, noise_state, zero_com_momentum)
+
+    @classmethod
+    def unfragmented(cls, state_dict, numbers, positions, *, dt_fs=1.0, temperature_K=300.0, friction_per_fs=0.001,
+                     seed=0, device: int = 0, velocities=None, step: int = 0, noise: str = "philox",
+                     noise_state: int = None, chunk_atoms: int = 0, zero_com_momentum=False, group=None):
+        """The reference's ``--mode visnet`` run on the device: the whole input is ONE ViSNet graph
+        (``ViSNetCalculator``, ``src/Calculators/visnet_calculator.py:138-155``) -- no fragments, no cap hydrogens, no
+        protein map, no MM term -- inside the same device step (``vb_md_setup`` with no placement recipe).  The
+        reference sends every input of three or fewer residues (caps counted) here, e.g. an ACE-X-NME dipeptide.
+
+        ``numbers`` / ``positions`` are the input's atoms in file order (:func:`ai2bmd_b200.pdbfrag.whole_input`).  The
+        other arguments and the run protocol (``run``, ``run_observed``, ``preequilibrate``, ``set_restraints``,
+        ``state``, ``noise_state``, ``temperature``, ``set_normals``) are those of the fragment step.  One graph is not
+        sharded: ``group`` raises."""
+        if group is not None:
+            raise ValueError("DeviceLangevin.unfragmented runs one graph on one GPU: it cannot be sharded over a process group")
+        if noise not in ("philox", "reference"):
+            raise ValueError(f"noise must be 'philox' or 'reference', not {noise!r}")
+        z = np.asarray(numbers, dtype=np.int64).reshape(-1)
+        x = np.asarray(positions, dtype=np.float64)
+        if x.shape != (len(z), 3):
+            raise ValueError(f"positions must be [{len(z)}, 3], one row per atom of numbers")
+        import torch
+        self = cls.__new__(cls)
+        self.torch, self.group = torch, None
+        self.n = len(z)
+        self.masses = masses_of(z)
+        self.kT = temperature_K * KB
+        self.fr = friction_per_fs / FS
+        dev = torch.device("cuda", device)
+        engine = Engine(state_dict, device, chunk_atoms=chunk_atoms)
+        engine.set_topology(z, np.zeros(len(z), dtype=np.int64), n_graphs=1)
+        engine.forward_host(x.astype(np.float32))           # start geometry: real edge count for the tile plan
+        engine.set_option("calibrate", 1)
+        self.engine = engine
+        self.ef = torch.zeros(3 * self.n + 1, dtype=torch.float32, device=dev)
+        self.stream = torch.cuda.current_stream(dev)
+        engine.md_setup_unfragmented(self.masses, dt_fs * FS, self.kT, self.fr, seed, self.ef.data_ptr())
+        self._start(x, velocities, seed, step, noise, noise_state, zero_com_momentum)
+        return self
+
+    def _start(self, positions, velocities, seed, step, noise, noise_state, zero_com_momentum):
+        """Noise source, start state and the forces of the start positions (after ``md_setup``)."""
+        engine = self.engine
         if noise == "reference":
             from . import refnoise
             s0, inc = refnoise.pcg_state(seed)

@@ -152,7 +152,8 @@ def fragment_protein(prot: CappedProtein, with_recipe: bool = False):
     assert len(set(prot.resnums.tolist())) == R, "residue numbers are not continuous"
     nd, na = R - 2, R - 3
     if nd < 2:
-        raise NotImplementedError("3 or fewer residues (incl. caps): run un-fragmented (--mode visnet)")
+        raise NotImplementedError("3 or fewer residues (incl. caps) cannot be fragmented: run the input as one graph "
+                                  "(--mode visnet): pdbfrag.whole_input(prot), or md.DeviceLangevin.unfragmented for MD")
     by_res = {r: [i for i in range(len(prot)) if prot.resnums[i] == r] for r in range(1, R + 1)}
 
     def pick(r, pred):
@@ -234,6 +235,15 @@ def fragment_protein(prot: CappedProtein, with_recipe: bool = False):
     pm = ProteinMap(len(prot), np.asarray(src, dtype=np.int32), np.asarray(dst, dtype=np.int32),
                     np.asarray(sgn, dtype=np.float32), np.asarray(fsgn, dtype=np.float32))
     return (fd, pm, recipe) if with_recipe else (fd, pm)
+
+
+def whole_input(prot: CappedProtein) -> FragmentData:
+    """The reference's ``--mode visnet`` input: every atom of ``prot`` in file order as ONE graph (the work partition
+    ``start, end = [0], [len(atoms)]`` of ``initialize_fragcalc``, ``src/AIMD/simulator.py:53-63``, and the graph
+    ``ViSNetCalculator.calculate`` builds, ``visnet_calculator.py:138-155``).  No cap hydrogens, no protein map: the
+    graph's forces are the protein's."""
+    from .elements import atomic_number
+    return single_graph([atomic_number(e) for e in prot.elements], prot.positions)
 
 
 def single_graph(z, pos) -> FragmentData:

@@ -147,7 +147,20 @@ int vb_chunk_fragments(int64_t n_graphs, const int64_t* frag_start_host, int64_t
  * vb_md_setup: recipe per FRAGMENT atom a (arrays of length N): real[a] = protein index, or -1 for an added
  * hydrogen placed at P[acc[a]] + unit(P[rem[a]] - P[acc[a]]) * blen[a].  ef_prot_dev[3*n_protein + 1] is the
  * caller-owned force/energy buffer (must hold forces of the current positions before the first kick1: call
- * vb_md_eval after vb_md_set_state).  Requires vb_set_protein_map with the same n_protein_atoms. */
+ * vb_md_eval after vb_md_set_state).  Requires vb_set_protein_map with the same n_protein_atoms.
+ *
+ * Un-fragmented step (real_host == NULL): the reference's --mode visnet, which feeds the whole input to ViSNet as ONE
+ * graph (ViSNetCalculator.calculate, src/Calculators/visnet_calculator.py:138-155; chosen at src/AIMD/simulator.py:74-79,
+ * work partition [0, n) at simulator.py:53-63) instead of fragments.  The topology of vb_set_topology is then the
+ * protein itself: n_graphs == 1 and N == n_protein_atoms, in protein atom order; no protein map (VB_ERR_STATE while one
+ * is set), no hydrogen refinement, at most one rank.  acc_host, rem_host and blen_host are ignored and may be NULL.  The
+ * evaluation writes the forces straight into ef_prot_dev[0 .. 3n) and the graph's energy into ef_prot_dev[3n]: no
+ * placement recipe (the fp32 cast of x is the graph's positions) and no signed reduction.  Restraints, the frame
+ * recorder, both noise kinds, the normals pool, option "chunk_atoms" (one graph is one chunk) and the non-bonded term
+ * (added after the evaluation) work as in the fragment step.  While this mode is set, vb_set_protein_map and
+ * vb_set_caph fail with VB_ERR_STATE, and so does vb_comm_connect with world > 1; vb_set_topology (or a new
+ * vb_md_setup) ends it.  vb_get_option("md_unfragmented") answers 1 while it is set.  Other failed conditions
+ * (n_graphs != 1, N != n_protein_atoms, bad numbers) are VB_ERR_ARG, and the message names the condition. */
 int vb_md_setup(vb_handle* h, int64_t n_protein_atoms, const double* masses_host, const int32_t* real_host,
                 const int32_t* acc_host, const int32_t* rem_host, const float* blen_host, double dt, double kT,
                 double friction, uint64_t seed, float* ef_prot_dev);
