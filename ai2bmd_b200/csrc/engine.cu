@@ -4,6 +4,7 @@
 #include <cxxabi.h>
 
 #include <algorithm>
+#include <atomic>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
@@ -191,6 +192,7 @@ struct vb_handle {
     // graph cache: one instantiated graph per (kind, I/O pointer set); pointers are baked into the captured launches
     struct GraphEntry { int kind; StepIO io; cudaGraphExec_t exec; };
     std::vector<GraphEntry> graphs;
+    long long graph_captures = 0;   // graphs instantiated so far (every kind, the device loop's included)
     int launches = 0;
     bool accum_dirty = false;    // a truncated vb_debug_run left accumulators (XA, VA, GQKV, ...) un-consumed
     std::vector<std::string> stage_names;
@@ -213,6 +215,14 @@ struct vb_handle {
     // host mirrors of the step counter and the frame count once all enqueued MD work has run (a guard that fires makes
     // the device fall behind them); exact again at every call that synchronises
     long long md_step_enq = 0, rec_frames_enq = 0;
+    // device loop (vb_md_run_loop): after a loop launch the mirrors above are stale until md_resync re-reads them
+    bool md_stale = false;
+    int loop_pdl = 0;                    // the cached loop body carries programmatic-dependent-launch edges
+    long long* d_loop = nullptr;         // [MD_LOOP_WORDS] (k_md.cuh)
+    unsigned long long* stop_word = nullptr;        // mapped pinned host memory: the latest launch a stop was asked for
+    unsigned long long* d_stop = nullptr;           // ... and its device address
+    std::atomic<unsigned long long> loop_gen{0};    // number of the latest loop launch
+    std::atomic<int> comm_world{0};                 // comm.world, readable without the mutex (vb_md_request_stop)
     // Hookean restraints (k_md.cuh MdRestraints): term CSR + rf [3*n_protein + 1] in one allocation
     bool rs_ready = false;
     MdRestraints rs{};
@@ -254,6 +264,7 @@ struct vb_handle {
             if (comm_peer[r] && r != comm.rank) cudaIpcCloseMemHandle(comm_peer[r]);
         cudaFree(comm_base); cudaFree(comm.counters);
         comm_base = nullptr; comm = CommParams{}; comm_ready = false;
+        comm_world.store(0);
         for (auto& p : comm_peer) p = nullptr;
     }
     void free_nb() {
@@ -986,11 +997,17 @@ int clean_accumulators(vb_handle* h, cudaStream_t st) {
     return VB_OK;
 }
 
-enum { K_EVAL = 0, K_HOST = 1, K_MD_EVAL = 2, K_MD_STEP = 3, K_ENERGY = 4, K_ENERGY_HOST = 5 };
+enum { K_EVAL = 0, K_HOST = 1, K_MD_EVAL = 2, K_MD_STEP = 3, K_ENERGY = 4, K_ENERGY_HOST = 5, K_MD_LOOP = 6 };
 
 // Run `enqueue(stream)` -- a sequence of launches / async copies that depends only on (kind, io) and the handle's
 // configuration -- either directly or as a replay of its cached CUDA graph.  A failed capture always ends the capture
 // (the stream stays usable) and is retried once without programmatic-dependent-launch edges.
+void cache_graph(vb_handle* h, int kind, const StepIO& io, cudaGraphExec_t exec) {
+    if (h->graphs.size() >= 8) { cudaGraphExecDestroy(h->graphs.front().exec); h->graphs.erase(h->graphs.begin()); }
+    h->graphs.push_back({kind, io, exec});
+    h->graph_captures++;
+}
+
 template <typename F>
 int run_cached(vb_handle* h, cudaStream_t st, int kind, const StepIO& io, F&& enqueue) {
     if (h->accum_dirty) { if (int rc = clean_accumulators(h, st)) return rc; }
@@ -1013,8 +1030,7 @@ int run_cached(vb_handle* h, cudaStream_t st, int kind, const StepIO& io, F&& en
         if (rc == VB_OK) h->set_error("graph capture failed: %s / %s", cudaGetErrorString(e_end), cudaGetErrorString(e_inst));
         return VB_ERR_CUDA;
     }
-    if (h->graphs.size() >= 8) { cudaGraphExecDestroy(h->graphs.front().exec); h->graphs.erase(h->graphs.begin()); }
-    h->graphs.push_back({kind, io, exec});
+    cache_graph(h, kind, io, exec);
     CUDA_TRY(h, cudaGraphLaunch(exec, st));
     return VB_OK;
 }
@@ -1221,6 +1237,14 @@ int vb_create(const float* weights_host, size_t n_floats, const vb_hparams* hp, 
     h->mw.cutoff = hp->cutoff;
     if (cudaStreamCreateWithFlags(&h->own_stream, cudaStreamNonBlocking) != cudaSuccess) { h->set_error("stream create failed"); return fail(VB_ERR_CUDA); }
     if (configure_kernels(h) != VB_OK) return fail(VB_ERR_CUDA);
+    if (cudaMalloc(&h->d_loop, sizeof(long long) * MD_LOOP_WORDS) != cudaSuccess ||
+        cudaMemset(h->d_loop, 0, sizeof(long long) * MD_LOOP_WORDS) != cudaSuccess ||
+        cudaHostAlloc(&h->stop_word, sizeof(unsigned long long), cudaHostAllocMapped) != cudaSuccess ||
+        cudaHostGetDevicePointer(&h->d_stop, h->stop_word, 0) != cudaSuccess) {
+        h->set_error("device loop words: allocation failed");
+        return fail(VB_ERR_ALLOC);
+    }
+    *h->stop_word = 0;
     if (const char* s = getenv("VB_USE_GRAPH")) h->use_graph = atoi(s);
     if (const char* s = getenv("VB_NPW")) h->npw_opt = atoi(s);
     if (const char* s = getenv("VB_TE_FWD")) h->te_fwd_opt = atoi(s);
@@ -1247,6 +1271,8 @@ void vb_destroy(vb_handle* h) {
     cudaFree(h->arena);
     h->free_map();
     cudaFree(h->d_flags);
+    cudaFree(h->d_loop);
+    cudaFreeHost(h->stop_word);
     cudaFreeHost(h->h_pos); cudaFreeHost(h->h_forces);
     delete h;
 }
@@ -1550,9 +1576,12 @@ void md_kick1_enqueue(vb_handle* h, cudaStream_t st) {
     md_kick1_kernel<<<1, MD_K1_THREADS, 0, st>>>(h->md, h->d_step, h->d_mmass, h->md_ef, h->rs.rf, h->d_mx, h->d_mv,
                                                  h->rec.ctl, h->nz);
 }
-void md_kick2_enqueue(vb_handle* h, cudaStream_t st) {
-    md_kick2_kernel<<<1, MD_K2_THREADS, 0, st>>>(h->md, h->d_step, h->d_mmass, h->md_ef, h->rs.rf, h->d_mx, h->d_mv,
-                                                 h->d_ehist, h->ehist_cap, h->rec);
+// `lp`: the device loop's decision after the step (MD_LOOP_BODY), or kick2 as the one-thread node ahead of the loop
+// (MD_LOOP_AHEAD: no step); off everywhere else
+void md_kick2_enqueue(vb_handle* h, cudaStream_t st, const MdLoop& lp = MdLoop{}) {
+    const int threads = lp.mode == MD_LOOP_AHEAD ? 1 : MD_K2_THREADS;
+    md_kick2_kernel<<<1, threads, 0, st>>>(h->md, h->d_step, h->d_mmass, h->md_ef, h->rs.rf, h->d_mx, h->d_mv,
+                                           h->d_ehist, h->ehist_cap, h->rec, lp);
 }
 // host mirrors after enqueueing n more steps
 void md_count_steps(vb_handle* h, long long n) {
@@ -1563,7 +1592,14 @@ void md_count_steps(vb_handle* h, long long n) {
 int md_resync(vb_handle* h) {
     CUDA_TRY(h, cudaMemcpy(&h->md_step_enq, h->d_step, sizeof(long long), cudaMemcpyDeviceToHost));
     if (h->rec.ctl) CUDA_TRY(h, cudaMemcpy(&h->rec_frames_enq, h->rec.ctl + MD_REC_FRAMES, sizeof(long long), cudaMemcpyDeviceToHost));
+    h->md_stale = false;
     return VB_OK;
+}
+// before the mirrors are used: after a device loop, wait for it and re-read them
+int md_fresh(vb_handle* h) {
+    if (!h->md_stale) return VB_OK;
+    CUDA_TRY(h, cudaDeviceSynchronize());
+    return md_resync(h);
 }
 // `stepping`: the call enqueues or changes MD work, which a broken all-reduce would corrupt; reading the state stays
 // allowed, so a failed run can still be inspected
@@ -1607,6 +1643,7 @@ int md_setup_unfragmented(vb_handle* h, int64_t n_protein_atoms, const double* m
     h->md = MdParams{P, dt, kT, friction, (unsigned long long)seed, nullptr, 0};
     h->md_ef = ef_prot_dev;
     h->md_step_enq = 0;
+    h->md_stale = false;
     h->md_ready = true;
     return VB_OK;
 }
@@ -1660,6 +1697,7 @@ int vb_md_setup(vb_handle* h, int64_t n_protein_atoms, const double* masses_host
     h->md = MdParams{P, dt, kT, friction, (unsigned long long)seed, nullptr, 0};
     h->md_ef = ef_prot_dev;
     h->md_step_enq = 0;
+    h->md_stale = false;
     h->md_ready = true;
     return VB_OK;
 }
@@ -1818,6 +1856,8 @@ int vb_md_read_frames(vb_handle* h, int64_t first, int64_t n, int64_t* step_host
     std::lock_guard<std::mutex> lk(h->mu);
     if (int rc = md_check(h, "vb_md_read_frames", false)) return rc;
     if (!h->rec.ctl) { h->set_error("vb_md_read_frames: the recorder is off (vb_md_set_recorder)"); return VB_ERR_STATE; }
+    CUDA_TRY(h, cudaSetDevice(h->device));
+    if (int rc = md_fresh(h)) return rc;
     const long long written = h->rec_frames_enq, C = h->rec.capacity;
     if (first < 0 || n < 0 || first + n > written || first < written - C) {
         h->set_error("vb_md_read_frames: frames [%lld, %lld) are not in the ring: %lld written or enqueued, the last %lld kept",
@@ -1950,6 +1990,7 @@ int vb_md_kick2(vb_handle* h, void* stream) {
     std::lock_guard<std::mutex> lk(h->mu);
     if (int rc = md_check(h, "vb_md_kick2")) return rc;
     CUDA_TRY(h, cudaSetDevice(h->device));
+    if (int rc = md_fresh(h)) return rc;
     md_kick2_enqueue(h, (cudaStream_t)stream);
     CUDA_TRY(h, cudaGetLastError());
     md_count_steps(h, 1);
@@ -1964,6 +2005,7 @@ int vb_md_run(vb_handle* h, int64_t n_steps, void* stream) {
     if (n_steps < 0) { h->set_error("vb_md_run: negative step count"); return VB_ERR_ARG; }
     cudaStream_t st = (cudaStream_t)stream;
     CUDA_TRY(h, cudaSetDevice(h->device));
+    if (int rc = md_fresh(h)) return rc;
     for (int64_t s = 0; s < n_steps; s++) {          // one graph replay per step
         int rc = run_cached(h, st, K_MD_STEP, md_io(h), [&](cudaStream_t cs) -> int {
             md_kick1_enqueue(h, cs);
@@ -1975,6 +2017,126 @@ int vb_md_run(vb_handle* h, int64_t n_steps, void* stream) {
         if (rc != VB_OK) return rc;
         md_count_steps(h, 1);
     }
+    return VB_OK;
+}
+
+namespace {
+// The loop graph: kick2 in "ahead" mode (one thread: starts the launch, decides the first iteration) -> WHILE node.  Its
+// body is the step exactly as vb_md_run captures it, with kick2 deciding the next iteration after its step; both are
+// captured on own_stream, the body into the conditional node's graph.  With option use_pdl the body is first captured
+// with programmatic edges; if the conditional body refused them it would be captured again without (h->loop_pdl says
+// which), and only the loop graph would go without them.
+int md_loop_capture_once(vb_handle* h, cudaGraphExec_t* out) {
+    cudaGraph_t g = nullptr, captured = nullptr;
+    cudaGraphExec_t exec = nullptr;
+    int rc = VB_OK;
+    cudaError_t e = cudaGraphCreate(&g, 0), e_end = cudaSuccess;
+    cudaStream_t cs = h->own_stream;
+    MdLoop lp{MD_LOOP_AHEAD, 0, h->d_loop, h->d_stop};
+    if (e == cudaSuccess) e = cudaGraphConditionalHandleCreate(&lp.cond, g, 0, cudaGraphCondAssignDefault);
+    if (e == cudaSuccess) e = cudaStreamBeginCaptureToGraph(cs, g, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal);
+    if (e == cudaSuccess) {
+        md_kick2_enqueue(h, cs, lp);
+        e = cudaGetLastError();
+        e_end = cudaStreamEndCapture(cs, &captured);
+    }
+    cudaGraphNode_t ahead = nullptr, loop = nullptr;
+    size_t n_nodes = 1;
+    if (e == cudaSuccess && e_end == cudaSuccess) e = cudaGraphGetNodes(g, &ahead, &n_nodes);
+    cudaGraphNodeParams cp = {};
+    cp.type = cudaGraphNodeTypeConditional;
+    cp.conditional.handle = lp.cond;
+    cp.conditional.type = cudaGraphCondTypeWhile;
+    cp.conditional.size = 1;
+    if (e == cudaSuccess && e_end == cudaSuccess) e = cudaGraphAddNode(&loop, g, &ahead, 1, &cp);
+    if (e == cudaSuccess && e_end == cudaSuccess)
+        e = cudaStreamBeginCaptureToGraph(cs, cp.conditional.phGraph_out[0], nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal);
+    if (e == cudaSuccess && e_end == cudaSuccess) {
+        lp.mode = MD_LOOP_BODY;
+        md_kick1_enqueue(h, cs);
+        rc = md_eval_enqueue(h, cs);
+        md_kick2_enqueue(h, cs, lp);
+        e = cudaGetLastError();
+        e_end = cudaStreamEndCapture(cs, &captured);
+    }
+    if (rc == VB_OK && e == cudaSuccess && e_end == cudaSuccess) e = cudaGraphInstantiate(&exec, g, 0);
+    if (g) cudaGraphDestroy(g);
+    if (rc == VB_OK && e == cudaSuccess && e_end == cudaSuccess) { *out = exec; return VB_OK; }
+    (void)cudaGetLastError();
+    if (rc == VB_OK) h->set_error("vb_md_run_loop: loop graph capture failed: %s / %s", cudaGetErrorString(e), cudaGetErrorString(e_end));
+    return rc != VB_OK ? rc : VB_ERR_CUDA;
+}
+int md_loop_capture(vb_handle* h, cudaGraphExec_t* out) {
+    const int pdl_opt = h->use_pdl;
+    int rc = md_loop_capture_once(h, out);
+    h->loop_pdl = rc == VB_OK ? pdl_opt : 0;
+    if (rc != VB_OK && pdl_opt) {
+        h->use_pdl = 0;
+        rc = md_loop_capture_once(h, out);
+        h->use_pdl = pdl_opt;
+    }
+    return rc;
+}
+}  // namespace
+
+int vb_md_run_loop(vb_handle* h, int64_t max_steps, void* stream) {
+    NvtxRange nvtx_("vb_md_run_loop");
+    if (!h) return VB_ERR_ARG;
+    std::lock_guard<std::mutex> lk(h->mu);
+    if (int rc = md_check(h, "vb_md_run_loop")) return rc;
+    if (max_steps < 0) { h->set_error("vb_md_run_loop: negative step count"); return VB_ERR_ARG; }
+    if (h->comm_ready && !h->comm_auto) {
+        h->set_error("vb_md_run_loop: the all-reduce of the step is the caller's (option comm_auto = 0), and a host "
+                     "all-reduce between the kicks cannot run inside a device loop; use vb_md_kick1 / vb_md_eval / vb_md_kick2");
+        return VB_ERR_STATE;
+    }
+    cudaStream_t st = (cudaStream_t)stream;
+    CUDA_TRY(h, cudaSetDevice(h->device));
+    if (h->accum_dirty) { if (int rc = clean_accumulators(h, st)) return rc; }
+    const StepIO io = md_io(h);
+    cudaGraphExec_t exec = nullptr;
+    for (auto& g : h->graphs)
+        if (g.kind == K_MD_LOOP && g.io == io) exec = g.exec;
+    if (!exec) {
+        if (int rc = md_loop_capture(h, &exec)) return rc;
+        cache_graph(h, K_MD_LOOP, io, exec);
+    }
+    // this launch's step count and number; a copy from pageable memory is staged before the call returns
+    const long long words[2] = {(long long)max_steps, (long long)++h->loop_gen};
+    static_assert(MD_LOOP_STEPS == 0 && MD_LOOP_GEN == 1, "loop word order");
+    CUDA_TRY(h, cudaMemcpyAsync(h->d_loop, words, sizeof(words), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(h, cudaGraphLaunch(exec, st));
+    h->md_stale = true;              // how many steps ran is known on the device only
+    return VB_OK;
+}
+
+int vb_md_request_stop(vb_handle* h) {
+    if (!h) return VB_ERR_ARG;
+    const int world = h->comm_world.load();   // not comm.world: another thread may hold the mutex in vb_comm_init
+    if (world > 1) {                 // no mutex wait while a loop runs: the message only if nobody holds it
+        if (h->mu.try_lock()) {
+            h->set_error("vb_md_request_stop: the handle is one rank of %d, and the ranks would see a host stop request at "
+                         "different steps", world);
+            h->mu.unlock();
+        }
+        return VB_ERR_STATE;
+    }
+    // every launch enqueued so far stops; a later one does not see this request (the word only grows)
+    const unsigned long long gen = h->loop_gen.load();
+    unsigned long long cur = __atomic_load_n(h->stop_word, __ATOMIC_SEQ_CST);
+    while (cur < gen && !__atomic_compare_exchange_n(h->stop_word, &cur, gen, false, __ATOMIC_SEQ_CST, __ATOMIC_SEQ_CST)) {}
+    return VB_OK;
+}
+
+int vb_md_loop_iterations(vb_handle* h, int64_t* out) {
+    if (!h) return VB_ERR_ARG;
+    std::lock_guard<std::mutex> lk(h->mu);
+    if (!out) { h->set_error("vb_md_loop_iterations: null output"); return VB_ERR_ARG; }
+    long long v = 0;
+    CUDA_TRY(h, cudaSetDevice(h->device));
+    CUDA_TRY(h, cudaDeviceSynchronize());
+    CUDA_TRY(h, cudaMemcpy(&v, h->d_loop + MD_LOOP_ITERS, sizeof(v), cudaMemcpyDeviceToHost));
+    *out = v;
     return VB_OK;
 }
 
@@ -2207,6 +2369,7 @@ int vb_comm_init(vb_handle* h, int rank, int world, int64_t max_floats, void* ip
     CUDA_TRY(h, cudaMalloc(&h->comm.counters, 4 * sizeof(unsigned int)));
     CUDA_TRY(h, cudaMemset(h->comm.counters, 0, 4 * sizeof(unsigned int)));
     h->comm.rank = rank; h->comm.world = world; h->comm.max_floats = max_floats;
+    h->comm_world.store(world);
     cudaIpcMemHandle_t hd;
     CUDA_TRY(h, cudaIpcGetMemHandle(&hd, h->comm_base));
     memcpy(ipc_handle_out, &hd, sizeof(hd));
@@ -2387,6 +2550,8 @@ int64_t vb_get_option(const vb_handle* h, const char* key) {
     if (k == "arena_bytes") return (int64_t)h->arena_bytes;
     if (k == "caph_ready") return h->caph_ready ? 1 : 0;
     if (k == "md_unfragmented") return h->md_unfrag ? 1 : 0;
+    if (k == "graph_captures") return h->graph_captures;
+    if (k == "md_loop_pdl") return h->loop_pdl;
     if (k == "caph_evals") {           // energy evaluations of the last refinement (synchronises)
         int v = 0;
         if (!h->caph_ready || cudaDeviceSynchronize() != cudaSuccess ||

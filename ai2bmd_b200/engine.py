@@ -40,6 +40,7 @@ EXPORTED_SYMBOLS = [
     "vb_forward_host", "vb_set_protein_map", "vb_forward_protein", "vb_forward_energy", "vb_forward_energy_host", "vb_get_edges", "vb_launches_per_forward",
     "vb_set_option", "vb_get_option", "vb_num_stages", "vb_stage_name", "vb_stage_kernel", "vb_debug_run", "vb_debug_read", "vb_profile_stages", "vb_tc_selftest", "vb_tc_selftest_rows",
     "vb_md_setup", "vb_md_set_normals", "vb_md_set_state", "vb_md_kick1", "vb_md_eval", "vb_md_kick2", "vb_md_run", "vb_md_get_state",
+    "vb_md_run_loop", "vb_md_request_stop", "vb_md_loop_iterations",
     "vb_md_set_restraints", "vb_md_set_recorder", "vb_md_read_frames", "vb_md_set_noise", "vb_md_get_noise_state", "vb_md_get_noise",
     "vb_set_nonbonded", "vb_nonbonded",
     "vb_comm_init", "vb_comm_connect", "vb_comm_allreduce",
@@ -121,6 +122,12 @@ def load_library(path: Optional[str] = None):
         getattr(lib, name).argtypes = [vp, vp]
     lib.vb_md_run.restype = C.c_int
     lib.vb_md_run.argtypes = [vp, i64, vp]
+    lib.vb_md_run_loop.restype = C.c_int
+    lib.vb_md_run_loop.argtypes = [vp, i64, vp]
+    lib.vb_md_request_stop.restype = C.c_int
+    lib.vb_md_request_stop.argtypes = [vp]
+    lib.vb_md_loop_iterations.restype = C.c_int
+    lib.vb_md_loop_iterations.argtypes = [vp, vp]
     lib.vb_md_set_restraints.restype = C.c_int
     lib.vb_md_set_restraints.argtypes = [vp, i64, vp, C.c_double, i64, vp, vp, vp]
     lib.vb_md_set_recorder.restype = C.c_int
@@ -403,6 +410,21 @@ class Engine:
 
     def md_run(self, n_steps: int, stream_ptr: int = 0):
         self._check(self.lib.vb_md_run(self.h, int(n_steps), stream_ptr), "vb_md_run")
+
+    def md_run_loop(self, max_steps: int, stream_ptr: int = 0):
+        """One launch of the device loop: at most ``max_steps`` steps, ending early at a runaway halt or a stop request
+        (vb_md_run_loop); asynchronous."""
+        self._check(self.lib.vb_md_run_loop(self.h, int(max_steps), stream_ptr), "vb_md_run_loop")
+
+    def md_request_stop(self):
+        """Stop every loop launch enqueued so far at its next step boundary (vb_md_request_stop); takes no lock."""
+        self._check(self.lib.vb_md_request_stop(self.h), "vb_md_request_stop")
+
+    def md_loop_iterations(self) -> int:
+        """Steps the last loop launch ran (synchronises)."""
+        out = C.c_int64(0)
+        self._check(self.lib.vb_md_loop_iterations(self.h, C.byref(out)), "vb_md_loop_iterations")
+        return int(out.value)
 
     def md_set_restraints(self, tether_atoms=(), tether_k: float = 0.0, spring_ij=None, spring_k=(), spring_rt=()):
         """Hookean restraints in eV/A^2 and A (vb_md_set_restraints): tethers anchored at the current device positions,

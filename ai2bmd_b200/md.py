@@ -331,6 +331,46 @@ class DeviceLangevin:
             self._eval()
             self.engine.md_kick2(sp)
 
+    def run_segment(self, n_steps: int) -> int:
+        """Up to ``n_steps`` steps as ONE launch of the device loop (``vb_md_run_loop``), waited for; returns the steps
+        actually run.  The loop ends by itself at the step the recorder's runaway guard halts on (a recorder set with
+        ``engine.md_set_recorder``), which raises :class:`TemperatureRunawayError` as ``run_observed`` does, and at the
+        next step boundary after :meth:`request_stop`.  While the engine stays halted (until ``engine.md_set_state``)
+        every call runs no step and raises again.  A ``KeyboardInterrupt`` during the wait asks the loop to stop, waits
+        for it and re-raises, so the state is that of a whole step; in a sharded run, where the ranks could not agree on
+        a stop step, it only waits for the launch to end (at ``n_steps`` or a halt) and re-raises.  Frames are not drained during the launch: read them
+        afterwards with ``engine.md_read_frames``.  A sharded run needs the engine's own all-reduce: with the
+        ``torch.distributed`` all-reduce between the kicks the step cannot loop on the device."""
+        n_steps = int(n_steps)
+        if n_steps < 0:
+            raise ValueError(f"n_steps must be >= 0, not {n_steps}")
+        if self.group is not None and not self._native_comm:
+            raise ValueError("run_segment needs the engine's own all-reduce inside the step graph: this run all-reduces "
+                             "with torch.distributed between the kicks, which cannot run inside a device loop; use run()")
+        import time
+        torch = self.torch
+        done = torch.cuda.Event()
+        try:
+            self.engine.md_run_loop(n_steps, self.stream.cuda_stream)
+            done.record(self.stream)
+            while not done.query():              # a sleep-poll, not synchronize(): a KeyboardInterrupt gets through
+                time.sleep(2e-4)
+        except KeyboardInterrupt:
+            if self.group is None:               # a launch already enqueued ends at its next step boundary
+                self.request_stop()
+            self.stream.synchronize()            # sharded: no stop step is agreed between ranks, the launch runs out
+            raise
+        ran = self.engine.md_loop_iterations()
+        halt = self.engine.get_option("md_halt_step")
+        if halt >= 0:
+            raise TemperatureRunawayError(f"temperature runaway at step {halt}: {self.temperature():.1f} K")
+        return ran
+
+    def request_stop(self):
+        """Stop a running :meth:`run_segment` (or ``engine.md_run_loop``) at its next step boundary.  Safe to call from
+        another thread while it waits; a sharded run refuses it (the ranks would stop at different steps)."""
+        self.engine.md_request_stop()
+
     def state(self, n_hist: int = 0):
         """(positions, velocities, step, potential energies of the last n_hist steps); synchronises."""
         return self.engine.md_get_state(n_hist)

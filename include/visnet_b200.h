@@ -205,6 +205,29 @@ int vb_md_set_restraints(vb_handle* h, int64_t n_tether, const int32_t* tether_a
                          const double* spring_rt);
 /* Single GPU: n_steps whole steps, each one replay of a captured CUDA graph, no host synchronisation. */
 int vb_md_run(vb_handle* h, int64_t n_steps, void* stream);
+/* Device loop: ONE asynchronous launch on `stream` that runs at most max_steps whole steps and ends earlier, at a step
+ * boundary, when the frame recorder's runaway guard fires (the halting step is the last one run) or after
+ * vb_md_request_stop.  The launch is a cached CUDA graph: a WHILE conditional node whose body is the step vb_md_run
+ * replays, whose kick2 counts the iteration and decides the next, with that decision also made once ahead of the node
+ * (a one-thread kick2 launch), so max_steps = 0 or a halted handle runs no step.  max_steps is not part of the graph: calls
+ * with any step count replay the same graph (vb_get_option "graph_captures" counts instantiations), and the loop graph
+ * is captured again exactly when vb_md_run's step graph would be.  After the call the host does not know how many steps
+ * ran: the next vb_md_run, vb_md_kick2 or vb_md_read_frames first waits for the device and re-reads the step counter.
+ * A sharded handle with the engine's own all-reduce loops as well: every rank holds the same state, so all ranks leave
+ * the loop at the same step.  VB_ERR_STATE when the caller all-reduces the step's buffer itself (option comm_auto = 0
+ * after vb_comm_connect), VB_ERR_ARG for max_steps < 0.  The library cannot tell a shard whose caller all-reduces with
+ * its own transport (NCCL) and never called vb_comm_init from a single-GPU handle: such a shard must not call this
+ * entry (nor vb_md_run), since its loop would integrate partial forces; DeviceLangevin.run_segment refuses it.  With option use_pdl the body is captured with programmatic edges if the conditional
+ * body accepts them, else without them (vb_get_option "md_loop_pdl" says which; vb_md_run's graph keeps them). */
+int vb_md_run_loop(vb_handle* h, int64_t max_steps, void* stream);
+/* Ask every loop launch enqueued so far on this handle to stop at its next step boundary; a launch enqueued after this
+ * call does not see the request.  Thread-safe, takes no lock and never waits: it may be called while another thread
+ * waits for the loop.  The request is an atomic store into a word of mapped pinned host memory that the loop reads at
+ * system scope after every step.  A sharded handle (vb_comm_init with world > 1) refuses it with VB_ERR_STATE: the ranks
+ * would see the request at different steps and leave the loop apart, and no stop step is agreed between them. */
+int vb_md_request_stop(vb_handle* h);
+/* Synchronises; *out = the steps the last vb_md_run_loop launch ran (0 before any). */
+int vb_md_loop_iterations(vb_handle* h, int64_t* out);
 /* Synchronises; any of x_host / v_host / step_out may be NULL.  epot_hist_host[n_hist] receives the potential
  * energies recorded at the end of the last n_hist steps (oldest first). */
 int vb_md_get_state(vb_handle* h, double* x_host, double* v_host, int64_t* step_out, double* epot_hist_host,
