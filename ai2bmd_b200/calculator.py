@@ -7,6 +7,7 @@ Mirrors, name for name, the classes of ``/root/reference/src/Calculators`` that 
 * :class:`ViSNetCalculator`   <- ``visnet_calculator.py:121-155`` (un-fragmented ``--mode visnet``)
 * :class:`DipeptideBondedCombiner` <- ``combiner.py:11-41``
 * :class:`DLBondedCalculator` <- ``bonded.py:19-123`` (fragment-batch evaluation + combine)
+* :class:`FragmentCalculator` <- ``fragment.py:16-68`` (placement, hydrogen refinement, bonded + MM term in one device call)
 
 ASE is not a dependency: calculators expose ``calculate(atoms, ...)`` / ``get_potential_energy`` /
 ``get_forces`` with ASE semantics (results cached while positions are unchanged,
@@ -222,3 +223,80 @@ class DLBondedCalculator:
         dip_e, dip_f, an_e, an_f = self.calculate(fragments)
         return (self.combiner.energy_combine(dip_e, an_e),
                 self.combiner.forces_combine(num_atoms, dip_f, an_f, select_index, origin_index))
+
+
+def _check_nbcalc_type(nbcalc_type: str):
+    if nbcalc_type == "pme":
+        raise NotImplementedError("nbcalc_type='pme': the smooth-PME non-bonded term is not implemented on the device "
+                                  "(DESIGN.md section 9); use 'mm'")
+    if nbcalc_type != "mm":
+        raise ValueError(f"nbcalc_type must be 'mm' or 'pme', not {nbcalc_type!r}")
+
+
+class FragmentCalculator(_CalculatorBase):
+    """The reference's whole per-step calculator call (``FragmentCalculator.calculate``, ``src/Calculators/fragment.py:50-68``)
+    as ONE engine call: protein positions in, the bonded (fragment) energy and forces plus the non-bonded MM term out,
+    in eV and eV/A.  Everything between runs on the device in one graph replay (``vb_forward_fragments_host``): the
+    fragment placement with the cap hydrogens (``DistanceFragment.get_fragments``), their LBFGS refinement, the model on
+    every fragment, the signed dipeptide / ACE-NME combination (``DLBondedCalculator.__call__``) and
+    ``MMNonBondedCalculator``, added as ``DipeptideCombiner`` does.  For any loop that keeps its own integrator: ASE's
+    ``Langevin``, the QM/MM solvent mode (``AsyncQMMM``'s ``qmcalc``), or :class:`ai2bmd_b200.md.Langevin`.
+
+    ``frags``, ``pm``, ``recipe``: the fragment batch, protein map and placement recipe of
+    :func:`ai2bmd_b200.pdbfrag.fragment_protein` (``with_recipe=True``); :meth:`from_protein` builds them.  ``caph``: a
+    :class:`ai2bmd_b200.caph.CapHProblem` turns the hydrogen refinement on.  ``nonbonded = (charges [e], sigmas [nm],
+    epsilons [kJ/mol])`` per protein atom turns the MM term on, with the reference's exclusions (atoms sharing a
+    dipeptide); without it the calculator is the reference's ``DLBondedCalculator.__call__``.  ``nbcalc_type`` is the
+    reference's ``--fragment-longrange-calc``: ``"mm"`` only, ``"pme"`` raises ``NotImplementedError``.  ``chunk_size`` is
+    the reference's ``--chunk-size`` (``Engine(chunk_atoms=...)``).  Arguments are checked before any engine is made."""
+
+    def __init__(self, ckpt_path: str, ckpt_type: str, frags: FragmentData, pm, recipe, caph=None, nonbonded=None,
+                 nbcalc_type: str = "mm", device: str = "cuda:0", chunk_size: Optional[int] = None, **kwargs):
+        super().__init__()
+        _check_nbcalc_type(nbcalc_type)
+        from .engine import check_recipe
+        real, acc, rem, blen = check_recipe(recipe.real, recipe.acc, recipe.rem, recipe.blen)
+        if len(real) != len(frags.z):
+            raise ValueError(f"recipe arrays must have one entry per fragment atom ({len(frags.z)}), not {len(real)}")
+        if nonbonded is not None:
+            from .nonbonded import dipeptide_atom_sets, exclusion_table
+            nonbonded = [np.asarray(a, dtype=np.float32).reshape(-1) for a in nonbonded]
+            if len(nonbonded) != 3 or any(len(a) != pm.n_protein for a in nonbonded):
+                raise ValueError(f"nonbonded must be (charges, sigmas_nm, epsilons_kj), {pm.n_protein} entries each")
+            excl = exclusion_table(pm.n_protein, dipeptide_atom_sets(frags, recipe, pm))
+        model_path = osp.join(ckpt_path, f"visnet-uni-{ckpt_type}.ckpt") if ckpt_type else ckpt_path
+        sd, ckpt_derivative = load_checkpoint(model_path)
+        if not resolve_derivative(ckpt_derivative, None):
+            raise ValueError(f"{model_path}: the fragment calculator needs forces, and the checkpoint has derivative=False")
+        self.device, self.n_protein = device, int(pm.n_protein)
+        self.engine = eng = Engine(sd, _device_index(device), chunk_atoms=int(chunk_size or 0))
+        eng.set_topology(frags.z, frags.batch, n_graphs=len(frags))
+        eng.set_protein_map(pm.n_protein, pm.src_atom, pm.dst_atom, pm.sign, pm.frag_sign)
+        eng.forward_host(np.asarray(frags.pos, dtype=np.float32))    # start geometry: real edge count for the tile plan
+        eng.set_option("calibrate", 1)
+        eng.set_fragment_recipe(real, acc, rem, blen)
+        if caph is not None:
+            eng.set_caph(caph)
+        if nonbonded is not None:
+            eng.set_nonbonded(*nonbonded, *excl)
+
+    @classmethod
+    def from_protein(cls, ckpt_path: str, ckpt_type: str, prot, caph_tables=None, nonbonded=None, nbcalc_type: str = "mm",
+                     device: str = "cuda:0", chunk_size: Optional[int] = None, **kwargs):
+        """From a :class:`ai2bmd_b200.pdbfrag.CappedProtein`: fragmentation, protein map and recipe
+        (``fragment_protein``), and with ``caph_tables`` (the per-dipeptide prmtop tables of
+        :func:`ai2bmd_b200.caph.build_problem`) the hydrogen refinement."""
+        _check_nbcalc_type(nbcalc_type)
+        from .pdbfrag import fragment_protein
+        frags, pm, recipe = fragment_protein(prot, with_recipe=True)
+        caph = None
+        if caph_tables is not None:
+            from .caph import build_problem
+            caph = build_problem(prot, frags, recipe, caph_tables)
+        return cls(ckpt_path, ckpt_type, frags, pm, recipe, caph=caph, nonbonded=nonbonded, nbcalc_type=nbcalc_type,
+                   device=device, chunk_size=chunk_size, **kwargs)
+
+    def calculate(self, atoms, properties=("energy", "forces"), system_changes=("positions",)):
+        energy, forces = self.engine.forward_fragments_host(atoms.positions)
+        self.results = {"energy": energy, "forces": forces}
+        return forces

@@ -122,7 +122,10 @@ struct StepIO {
     float* energy = nullptr;      // [G]
     float* forces = nullptr;      // [N][3]
     float* ef = nullptr;          // [3*n_protein + 1] or nullptr (no whole-protein reduction)
-    bool operator==(const StepIO& o) const { return pos == o.pos && energy == o.energy && forces == o.forces && ef == o.ef; }
+    const double* x = nullptr;    // [n_protein][3] protein positions the placement reads (vb_forward_fragments)
+    bool operator==(const StepIO& o) const {
+        return pos == o.pos && energy == o.energy && forces == o.forces && ef == o.ef && x == o.x;
+    }
 };
 
 struct vb_handle {
@@ -149,7 +152,9 @@ struct vb_handle {
     int n_protein = 0, n_map = 0;
     int *d_map_rowptr = nullptr, *d_map_src = nullptr;
     float *d_map_sign = nullptr, *d_frag_sign = nullptr;
-    float* d_ef = nullptr;       // [3*n_protein + 1] internal whole-protein buffer (diagnostic runs)
+    float* d_ef = nullptr;       // [3*n_protein + 1] internal whole-protein buffer (diagnostic runs, vb_forward_fragments_host)
+    double *d_fx = nullptr, *h_fx = nullptr;   // [n_protein][3] vb_forward_fragments_host's positions, pinned staging
+    float* h_fef = nullptr;                    // [3*n_protein + 1] ... and its pinned result
     int* d_flags = nullptr;      // [0]: set by the neighbour stage when a step produced more edges than the workspace holds
     // cap-hydrogen refinement (k_caph.cuh): flat term arrays + scratch in one device allocation
     bool caph_ready = false;
@@ -252,7 +257,9 @@ struct vb_handle {
     }
     void free_map() {
         cudaFree(d_map_rowptr); cudaFree(d_map_src); cudaFree(d_map_sign); cudaFree(d_frag_sign); cudaFree(d_ef);
+        cudaFree(d_fx); cudaFreeHost(h_fx); cudaFreeHost(h_fef);
         d_map_rowptr = d_map_src = nullptr; d_map_sign = d_frag_sign = d_ef = nullptr;
+        d_fx = h_fx = nullptr; h_fef = nullptr;
         n_protein = n_map = 0;
     }
     void free_caph() {
@@ -284,13 +291,17 @@ struct vb_handle {
         cudaFree(nz_mem);
         nz_mem = nullptr; nz = MdNoise{};
     }
+    void free_recipe() {
+        cudaFree(d_real); cudaFree(d_acc); cudaFree(d_rem); cudaFree(d_blen);
+        d_real = d_acc = d_rem = nullptr; d_blen = nullptr;
+    }
     void free_md() {
         free_rs();                       // the restraints index the MD state
         free_rec();                      // ... and so does the frame ring
         free_nz();                       // ... and the noise buffers
-        cudaFree(d_mx); cudaFree(d_mv); cudaFree(d_mmass); cudaFree(d_ehist);
-        cudaFree(d_real); cudaFree(d_acc); cudaFree(d_rem); cudaFree(d_blen); cudaFree(d_step);
-        d_mx = d_mv = d_mmass = d_ehist = nullptr; d_real = d_acc = d_rem = nullptr; d_blen = nullptr; d_step = nullptr;
+        free_recipe();                   // the recipe indexes the protein of the map: whoever set it, it goes with it
+        cudaFree(d_mx); cudaFree(d_mv); cudaFree(d_mmass); cudaFree(d_ehist); cudaFree(d_step);
+        d_mx = d_mv = d_mmass = d_ehist = nullptr; d_step = nullptr;
         md_ready = false;
         if (md_unfrag) { md_unfrag = false; n_protein = 0; }   // that n_protein came from vb_md_setup, not from a map
     }
@@ -997,7 +1008,8 @@ int clean_accumulators(vb_handle* h, cudaStream_t st) {
     return VB_OK;
 }
 
-enum { K_EVAL = 0, K_HOST = 1, K_MD_EVAL = 2, K_MD_STEP = 3, K_ENERGY = 4, K_ENERGY_HOST = 5, K_MD_LOOP = 6 };
+enum { K_EVAL = 0, K_HOST = 1, K_MD_EVAL = 2, K_MD_STEP = 3, K_ENERGY = 4, K_ENERGY_HOST = 5, K_MD_LOOP = 6, K_FRAG = 7,
+       K_FRAG_HOST = 8 };
 
 // Run `enqueue(stream)` -- a sequence of launches / async copies that depends only on (kind, io) and the handle's
 // configuration -- either directly or as a replay of its cached CUDA graph.  A failed capture always ends the capture
@@ -1545,31 +1557,35 @@ int vb_forward_protein(vb_handle* h, const float* pos_dev, float* ef_prot_dev, v
 
 // ---- device-resident MD (k_md.cuh) ---------------------------------------------------------------------
 namespace {
-StepIO md_io(vb_handle* h) {
+// the evaluation's buffers when it ends in the protein buffer ef [3*n_protein + 1]
+StepIO eval_io(vb_handle* h, float* ef) {
     StepIO io = internal_io(h, false);
     if (h->md_unfrag) {          // one graph over the protein: its forces and energy are ef itself, no reduction
-        io.forces = h->md_ef;
-        io.energy = h->md_ef + 3 * (size_t)h->n_protein;
+        io.forces = ef;
+        io.energy = ef + 3 * (size_t)h->n_protein;
         return io;
     }
-    io.ef = h->md_ef;
+    io.ef = ef;
     return io;
 }
-// fragment placement (un-fragmented: the fp32 cast of x) [+ restraints into rf, one more CTA] -> evaluation + signed whole-protein reduction
-// [-> non-bonded term], all on st.  Every rank of a sharded run holds the same state and the whole term set, so each
-// computes the same rf; only ef goes through the all-reduce.
-int md_eval_enqueue(vb_handle* h, cudaStream_t st) {
+StepIO md_io(vb_handle* h) { return eval_io(h, h->md_ef); }
+// fragment placement from the protein positions x (un-fragmented: the fp32 cast of x) [+ restraints into rf, one more
+// CTA, with `restrain`] -> evaluation + signed whole-protein reduction into ef [-> non-bonded term at x], all on st.  The
+// MD step passes its own state (d_mx, md_ef, restrain); vb_forward_fragments the caller's buffers and no restraints.
+// Every rank of a sharded run holds the same state and the whole term set, so each computes the same rf; only ef goes
+// through the all-reduce.
+int md_eval_enqueue(vb_handle* h, cudaStream_t st, const double* x, float* ef, bool restrain) {
     const int N = h->ws.N;
-    md_place_kernel<<<(N + 255) / 256 + (h->rs_ready ? 1 : 0), 256, 0, st>>>(N, h->d_real, h->d_acc, h->d_rem, h->d_blen,
-                                                                            h->d_mx, h->d_pos, h->rs);
+    md_place_kernel<<<(N + 255) / 256 + (restrain && h->rs_ready ? 1 : 0), 256, 0, st>>>(N, h->d_real, h->d_acc, h->d_rem,
+                                                                                        h->d_blen, x, h->d_pos, h->rs);
     if (h->caph_ready) caph_relax_kernel<<<1, CAPH_THREADS, 0, st>>>(h->caph, h->d_pos);   // hydrogen refinement, in place
-    if (int rc = enqueue_eval(h, st, md_io(h))) return rc;
+    if (int rc = enqueue_eval(h, st, eval_io(h, ef))) return rc;
     if (h->nb_ready && h->nb.hi > h->nb.lo) {      // non-bonded MM term on the same protein coordinates
-        nonbonded_kernel<double><<<(h->nb.hi - h->nb.lo + 7) / 8, 256, 0, st>>>(h->nb, h->d_mx, h->md_ef, h->d_nb_eatom);
-        nonbonded_energy_kernel<<<1, 256, 0, st>>>(h->nb, h->d_nb_eatom, h->md_ef);
+        nonbonded_kernel<double><<<(h->nb.hi - h->nb.lo + 7) / 8, 256, 0, st>>>(h->nb, x, ef, h->d_nb_eatom);
+        nonbonded_energy_kernel<<<1, 256, 0, st>>>(h->nb, h->d_nb_eatom, ef);
     }
     CUDA_TRY(h, cudaGetLastError());
-    if (h->comm_ready && h->comm_auto) return enqueue_allreduce(h, st, h->md_ef, 3LL * h->n_protein + 1);
+    if (h->comm_ready && h->comm_auto) return enqueue_allreduce(h, st, ef, 3LL * h->n_protein + 1);
     return VB_OK;
 }
 void md_kick1_enqueue(vb_handle* h, cudaStream_t st) {
@@ -1647,6 +1663,40 @@ int md_setup_unfragmented(vb_handle* h, int64_t n_protein_atoms, const double* m
     h->md_ready = true;
     return VB_OK;
 }
+
+// The placement recipe of the fragment atoms, as vb_md_setup and vb_set_fragment_recipe take it: the handle must have a
+// topology and a protein map of n_protein_atoms atoms, and every index must address that protein.  Called with h->mu held.
+int check_recipe(vb_handle* h, const char* who, int64_t n_protein_atoms, const int32_t* real, const int32_t* acc,
+                 const int32_t* rem, const float* blen) {
+    if (!h->has_topology || h->n_protein <= 0 || !h->d_map_rowptr) { h->set_error("%s: topology / protein map not set", who); return VB_ERR_STATE; }
+    if (n_protein_atoms != h->n_protein || !real || !acc || !rem || !blen) {
+        h->set_error("%s: bad arguments (null recipe array, or n_protein differs from the protein map's %d)", who, h->n_protein);
+        return VB_ERR_ARG;
+    }
+    const int N = h->ws.N, P = h->n_protein;
+    for (int a = 0; a < N; a++) {
+        const bool cap = real[a] < 0;
+        if ((!cap && real[a] >= P) || (cap && (acc[a] < 0 || acc[a] >= P || rem[a] < 0 || rem[a] >= P || acc[a] == rem[a]))) {
+            h->set_error("%s: recipe index out of range at fragment atom %d", who, a);
+            return VB_ERR_ARG;
+        }
+    }
+    return VB_OK;
+}
+// ... and its upload in place of the handle's recipe (the caller has dropped the graphs that hold the old pointers)
+int upload_recipe(vb_handle* h, const int32_t* real, const int32_t* acc, const int32_t* rem, const float* blen) {
+    const int N = h->ws.N;
+    h->free_recipe();
+    CUDA_TRY(h, cudaMalloc(&h->d_real, sizeof(int) * N));
+    CUDA_TRY(h, cudaMalloc(&h->d_acc, sizeof(int) * N));
+    CUDA_TRY(h, cudaMalloc(&h->d_rem, sizeof(int) * N));
+    CUDA_TRY(h, cudaMalloc(&h->d_blen, sizeof(float) * N));
+    CUDA_TRY(h, cudaMemcpy(h->d_real, real, sizeof(int) * N, cudaMemcpyHostToDevice));
+    CUDA_TRY(h, cudaMemcpy(h->d_acc, acc, sizeof(int) * N, cudaMemcpyHostToDevice));
+    CUDA_TRY(h, cudaMemcpy(h->d_rem, rem, sizeof(int) * N, cudaMemcpyHostToDevice));
+    CUDA_TRY(h, cudaMemcpy(h->d_blen, blen, sizeof(float) * N, cudaMemcpyHostToDevice));
+    return VB_OK;
+}
 }  // namespace
 
 int vb_md_setup(vb_handle* h, int64_t n_protein_atoms, const double* masses_host, const int32_t* real_host,
@@ -1657,39 +1707,24 @@ int vb_md_setup(vb_handle* h, int64_t n_protein_atoms, const double* masses_host
     if (!real_host) return md_setup_unfragmented(h, n_protein_atoms, masses_host, dt, kT, friction, seed, ef_prot_dev);
     if (!h->has_topology || h->n_protein <= 0 || !h->d_map_rowptr) { h->set_error("vb_md_setup: topology / protein map not set"); return VB_ERR_STATE; }
     if (int rc = need_derivative(h, "vb_md_setup")) return rc;
-    if (n_protein_atoms != h->n_protein || !masses_host || !real_host || !acc_host || !rem_host || !blen_host || !ef_prot_dev ||
-        !(dt > 0.0) || kT < 0.0 || friction < 0.0) {
-        h->set_error("vb_md_setup: bad arguments (n_protein must equal the protein map's)");
+    if (!masses_host || !ef_prot_dev || !(dt > 0.0) || kT < 0.0 || friction < 0.0) {
+        h->set_error("vb_md_setup: bad arguments");
         return VB_ERR_ARG;
     }
-    const int N = h->ws.N, P = h->n_protein;
-    for (int a = 0; a < N; a++) {
-        const bool cap = real_host[a] < 0;
-        if ((!cap && real_host[a] >= P) || (cap && (acc_host[a] < 0 || acc_host[a] >= P || rem_host[a] < 0 || rem_host[a] >= P ||
-                                                     acc_host[a] == rem_host[a]))) {
-            h->set_error("vb_md_setup: recipe index out of range at fragment atom %d", a);
-            return VB_ERR_ARG;
-        }
-    }
+    if (int rc = check_recipe(h, "vb_md_setup", n_protein_atoms, real_host, acc_host, rem_host, blen_host)) return rc;
+    const int P = h->n_protein;
     for (int i = 0; i < P; i++)
         if (!(masses_host[i] > 0.0)) { h->set_error("vb_md_setup: non-positive mass at atom %d", i); return VB_ERR_ARG; }
     CUDA_TRY(h, cudaSetDevice(h->device));
     h->drop_graph();
     h->free_md();
+    if (int rc = upload_recipe(h, real_host, acc_host, rem_host, blen_host)) return rc;
     CUDA_TRY(h, cudaMalloc(&h->d_mx, sizeof(double) * 3 * P));
     CUDA_TRY(h, cudaMalloc(&h->d_mv, sizeof(double) * 3 * P));
     CUDA_TRY(h, cudaMalloc(&h->d_mmass, sizeof(double) * P));
     CUDA_TRY(h, cudaMalloc(&h->d_ehist, sizeof(double) * h->ehist_cap));
-    CUDA_TRY(h, cudaMalloc(&h->d_real, sizeof(int) * N));
-    CUDA_TRY(h, cudaMalloc(&h->d_acc, sizeof(int) * N));
-    CUDA_TRY(h, cudaMalloc(&h->d_rem, sizeof(int) * N));
-    CUDA_TRY(h, cudaMalloc(&h->d_blen, sizeof(float) * N));
     CUDA_TRY(h, cudaMalloc(&h->d_step, sizeof(long long)));
     CUDA_TRY(h, cudaMemcpy(h->d_mmass, masses_host, sizeof(double) * P, cudaMemcpyHostToDevice));
-    CUDA_TRY(h, cudaMemcpy(h->d_real, real_host, sizeof(int) * N, cudaMemcpyHostToDevice));
-    CUDA_TRY(h, cudaMemcpy(h->d_acc, acc_host, sizeof(int) * N, cudaMemcpyHostToDevice));
-    CUDA_TRY(h, cudaMemcpy(h->d_rem, rem_host, sizeof(int) * N, cudaMemcpyHostToDevice));
-    CUDA_TRY(h, cudaMemcpy(h->d_blen, blen_host, sizeof(float) * N, cudaMemcpyHostToDevice));
     CUDA_TRY(h, cudaMemset(h->d_mx, 0, sizeof(double) * 3 * P));
     CUDA_TRY(h, cudaMemset(h->d_mv, 0, sizeof(double) * 3 * P));
     CUDA_TRY(h, cudaMemset(h->d_ehist, 0, sizeof(double) * h->ehist_cap));
@@ -1972,7 +2007,8 @@ int vb_md_eval(vb_handle* h, void* stream) {
     std::lock_guard<std::mutex> lk(h->mu);
     if (int rc = md_check(h, "vb_md_eval")) return rc;
     CUDA_TRY(h, cudaSetDevice(h->device));
-    return run_cached(h, (cudaStream_t)stream, K_MD_EVAL, md_io(h), [&](cudaStream_t s) -> int { return md_eval_enqueue(h, s); });
+    return run_cached(h, (cudaStream_t)stream, K_MD_EVAL, md_io(h),
+                      [&](cudaStream_t s) -> int { return md_eval_enqueue(h, s, h->d_mx, h->md_ef, true); });
 }
 
 int vb_md_kick1(vb_handle* h, void* stream) {
@@ -2009,7 +2045,7 @@ int vb_md_run(vb_handle* h, int64_t n_steps, void* stream) {
     for (int64_t s = 0; s < n_steps; s++) {          // one graph replay per step
         int rc = run_cached(h, st, K_MD_STEP, md_io(h), [&](cudaStream_t cs) -> int {
             md_kick1_enqueue(h, cs);
-            if (int r = md_eval_enqueue(h, cs)) return r;
+            if (int r = md_eval_enqueue(h, cs, h->d_mx, h->md_ef, true)) return r;
             md_kick2_enqueue(h, cs);
             CUDA_TRY(h, cudaGetLastError());
             return (int)VB_OK;
@@ -2054,7 +2090,7 @@ int md_loop_capture_once(vb_handle* h, cudaGraphExec_t* out) {
     if (e == cudaSuccess && e_end == cudaSuccess) {
         lp.mode = MD_LOOP_BODY;
         md_kick1_enqueue(h, cs);
-        rc = md_eval_enqueue(h, cs);
+        rc = md_eval_enqueue(h, cs, h->d_mx, h->md_ef, true);
         md_kick2_enqueue(h, cs, lp);
         e = cudaGetLastError();
         e_end = cudaStreamEndCapture(cs, &captured);
@@ -2161,6 +2197,84 @@ int vb_md_get_state(vb_handle* h, double* x_host, double* v_host, int64_t* step_
             epot_hist_host[i] = sidx >= 0 ? ring[sidx % h->ehist_cap] : 0.0;
         }
     }
+    return VB_OK;
+}
+
+// ---- the whole FragmentCalculator call on the caller's protein positions -----------------------------------------------
+int vb_set_fragment_recipe(vb_handle* h, int64_t n_protein_atoms, const int32_t* real_host, const int32_t* acc_host,
+                           const int32_t* rem_host, const float* blen_host) {
+    NvtxRange nvtx_("vb_set_fragment_recipe");
+    if (!h) return VB_ERR_ARG;
+    std::lock_guard<std::mutex> lk(h->mu);
+    if (int rc = check_recipe(h, "vb_set_fragment_recipe", n_protein_atoms, real_host, acc_host, rem_host, blen_host)) return rc;
+    CUDA_TRY(h, cudaSetDevice(h->device));
+    CUDA_TRY(h, cudaDeviceSynchronize());      // no enqueued placement may still read the old recipe
+    h->drop_graph();                           // the captured placements hold its pointers
+    return upload_recipe(h, real_host, acc_host, rem_host, blen_host);
+}
+
+namespace {
+int fragments_check(vb_handle* h, const char* who) {
+    if (h->md_unfrag) {
+        h->set_error("%s: the MD step is set up un-fragmented (vb_md_setup with real_host = NULL): there are no fragments "
+                     "to place; call vb_set_topology again for a fragment batch", who);
+        return VB_ERR_STATE;
+    }
+    if (!h->has_topology) { h->set_error("%s: call vb_set_topology first", who); return VB_ERR_STATE; }
+    if (h->n_protein <= 0 || !h->d_map_rowptr) { h->set_error("%s: no protein map: call vb_set_protein_map", who); return VB_ERR_STATE; }
+    if (!h->d_real) {
+        h->set_error("%s: no placement recipe: call vb_set_fragment_recipe (or vb_md_setup)", who);
+        return VB_ERR_STATE;
+    }
+    if (int rc = need_derivative(h, who)) return rc;
+    return comm_check(h, who);
+}
+}  // namespace
+
+int vb_forward_fragments(vb_handle* h, const double* prot_pos_dev, float* ef_prot_dev, void* stream) {
+    NvtxRange nvtx_("vb_forward_fragments");
+    if (!h) return VB_ERR_ARG;
+    std::lock_guard<std::mutex> lk(h->mu);
+    if (int rc = fragments_check(h, "vb_forward_fragments")) return rc;
+    if (!prot_pos_dev || !ef_prot_dev) { h->set_error("vb_forward_fragments: null buffer"); return VB_ERR_ARG; }
+    CUDA_TRY(h, cudaSetDevice(h->device));
+    StepIO io = eval_io(h, ef_prot_dev);
+    io.x = prot_pos_dev;
+    return run_cached(h, (cudaStream_t)stream, K_FRAG, io,
+                      [&](cudaStream_t s) -> int { return md_eval_enqueue(h, s, prot_pos_dev, ef_prot_dev, false); });
+}
+
+int vb_forward_fragments_host(vb_handle* h, const double* prot_pos_host, float* ef_prot_host) {
+    NvtxRange nvtx_("vb_forward_fragments_host");
+    if (!h) return VB_ERR_ARG;
+    std::lock_guard<std::mutex> lk(h->mu);
+    if (int rc = fragments_check(h, "vb_forward_fragments_host")) return rc;
+    if (!prot_pos_host || !ef_prot_host) { h->set_error("vb_forward_fragments_host: null buffer"); return VB_ERR_ARG; }
+    const size_t n3 = 3 * (size_t)h->n_protein;
+    cudaStream_t st = h->own_stream;
+    CUDA_TRY(h, cudaSetDevice(h->device));
+    // MD steps enqueued on the caller's stream (vb_md_run, vb_md_run_loop, ...) may still be running, and they use the
+    // same workspace; own_stream is non-blocking, so nothing orders the replay after them but this wait
+    if (h->md_ready) CUDA_TRY(h, cudaDeviceSynchronize());
+    if (!h->d_fx) {                  // staging of the first call, kept with the protein map
+        CUDA_TRY(h, cudaMalloc(&h->d_fx, sizeof(double) * n3));
+        CUDA_TRY(h, cudaMallocHost(&h->h_fx, sizeof(double) * n3));
+        CUDA_TRY(h, cudaMallocHost(&h->h_fef, sizeof(float) * (n3 + 1)));
+    }
+    memcpy(h->h_fx, prot_pos_host, sizeof(double) * n3);
+    // H2D of the positions, every launch of vb_forward_fragments, D2H of forces and energy: one graph replay
+    StepIO io = eval_io(h, h->d_ef);
+    io.x = h->d_fx;
+    int rc = run_cached(h, st, K_FRAG_HOST, io, [&](cudaStream_t s) -> int {
+        CUDA_TRY(h, cudaMemcpyAsync(h->d_fx, h->h_fx, sizeof(double) * n3, cudaMemcpyHostToDevice, s));
+        if (int r = md_eval_enqueue(h, s, h->d_fx, h->d_ef, false)) return r;
+        CUDA_TRY(h, cudaMemcpyAsync(h->h_fef, h->d_ef, sizeof(float) * (n3 + 1), cudaMemcpyDeviceToHost, s));
+        return (int)VB_OK;
+    });
+    if (rc != VB_OK) return rc;
+    CUDA_TRY(h, cudaStreamSynchronize(st));
+    if (int r = check_edge_overflow(h, "vb_forward_fragments_host")) return r;
+    memcpy(ef_prot_host, h->h_fef, sizeof(float) * (n3 + 1));
     return VB_OK;
 }
 

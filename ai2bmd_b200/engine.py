@@ -45,6 +45,7 @@ EXPORTED_SYMBOLS = [
     "vb_set_nonbonded", "vb_nonbonded",
     "vb_comm_init", "vb_comm_connect", "vb_comm_allreduce",
     "vb_set_caph", "vb_caph_relax", "vb_chunk_fragments",
+    "vb_set_fragment_recipe", "vb_forward_fragments", "vb_forward_fragments_host",
 ]
 
 
@@ -152,9 +153,25 @@ def load_library(path: Optional[str] = None):
     lib.vb_md_get_state.argtypes = [vp, vp, vp, vp, vp, i64]
     lib.vb_chunk_fragments.restype = C.c_int
     lib.vb_chunk_fragments.argtypes = [i64, vp, i64, vp]
+    lib.vb_set_fragment_recipe.restype = C.c_int
+    lib.vb_set_fragment_recipe.argtypes = [vp, i64, vp, vp, vp, vp]
+    lib.vb_forward_fragments.restype = C.c_int
+    lib.vb_forward_fragments.argtypes = [vp, vp, vp, vp]
+    lib.vb_forward_fragments_host.restype = C.c_int
+    lib.vb_forward_fragments_host.argtypes = [vp, vp, vp]
     if path == _build.LIB_PATH:
         _lib = lib
     return lib
+
+
+def check_recipe(real, acc, rem, blen):
+    """The four arrays of a fragment placement recipe as the C ABI takes them (int32, int32, int32, float32), one entry
+    per fragment atom each; raises ``ValueError`` before anything reaches the engine."""
+    r, a, q = (np.ascontiguousarray(v, dtype=np.int32) for v in (real, acc, rem))
+    b = np.ascontiguousarray(blen, dtype=np.float32)
+    if not (r.ndim == a.ndim == q.ndim == b.ndim == 1 and len(r) == len(a) == len(q) == len(b)):
+        raise ValueError("recipe arrays must be 1-D with one entry per fragment atom")
+    return r, a, q, b
 
 
 def weight_manifest() -> str:
@@ -306,6 +323,35 @@ class Engine:
     def caph_relax(self, pos_ptr: int, stream_ptr: int = 0):
         """Refine the added hydrogens of a packed fragment position buffer (device pointer) in place; asynchronous."""
         self._check(self.lib.vb_caph_relax(self.h, pos_ptr, stream_ptr), "vb_caph_relax")
+
+    # ---- the whole FragmentCalculator call (include/visnet_b200.h: vb_set_fragment_recipe / vb_forward_fragments*) ----
+    def set_fragment_recipe(self, real, acc, rem, blen):
+        """The placement recipe of every fragment atom (a :class:`ai2bmd_b200.pdbfrag.FragmentRecipe`'s arrays) for the
+        protein of the protein map, without any MD setup; replaces the recipe of an earlier call or ``md_setup``."""
+        r, a, q, b = check_recipe(real, acc, rem, blen)
+        if len(r) != self.n_atoms:
+            raise ValueError(f"recipe arrays must have one entry per fragment atom ({self.n_atoms}), not {len(r)}")
+        self._check(self.lib.vb_set_fragment_recipe(self.h, self.n_protein, r.ctypes.data, a.ctypes.data, q.ctypes.data,
+                                                    b.ctypes.data), "vb_set_fragment_recipe")
+
+    def forward_fragments_host(self, prot_pos: np.ndarray) -> Tuple[float, np.ndarray]:
+        """Protein positions [n_protein, 3] (A) in, (energy [eV], forces [n_protein, 3] float32 eV/A) out: placement,
+        hydrogen refinement, evaluation, signed reduction and the non-bonded term in one graph replay, synchronous.
+        After ``md_setup`` it first waits for the device, so MD steps still running on any stream finish before it."""
+        x = np.ascontiguousarray(prot_pos, dtype=np.float64)
+        if x.shape != (self.n_protein, 3):
+            raise ValueError(f"prot_pos must be [{self.n_protein},3]")
+        ef = np.empty(3 * self.n_protein + 1, dtype=np.float32)
+        rc = self.lib.vb_forward_fragments_host(self.h, x.__array_interface__["data"][0], ef.__array_interface__["data"][0])
+        if rc < 0:
+            self._check(rc, "vb_forward_fragments_host")
+        return float(ef[-1]), ef[:-1].reshape(-1, 3)
+
+    def forward_fragments_device(self, prot_pos_ptr: int, ef_ptr: int, stream_ptr: int = 0):
+        """Raw device pointers: fp64 protein positions [n_protein, 3] -> ef [3 n_protein + 1] (forces, then the energy);
+        asynchronous on ``stream_ptr``.  It shares the workspace with the MD step: order it after MD work of this engine
+        (the same stream, or a wait on an event of it)."""
+        self._check(self.lib.vb_forward_fragments(self.h, prot_pos_ptr, ef_ptr, stream_ptr), "vb_forward_fragments")
 
     # ---- NVLink peer-memory all-reduce (include/visnet_b200.h: vb_comm_*) ----
     def comm_init(self, rank: int, world: int, max_floats: int) -> bytes:

@@ -294,6 +294,40 @@ int vb_set_caph(vb_handle* h, const vb_caph_problem* problem);          /* host 
 /* Refine a packed fragment position buffer in place (device pointer), asynchronous on `stream`. */
 int vb_caph_relax(vb_handle* h, float* pos_dev, void* stream);
 
+/* ---- The whole FragmentCalculator call: protein positions in, combined energy and forces out ----------------------
+ * For a caller that keeps its own integrator loop (ASE's Langevin, the QM/MM solvent mode, a user's driver): everything
+ * the MD step evaluates, on the caller's positions and force buffer instead of the MD state.  One call enqueues, in order,
+ * the placement of every fragment atom from the fp64 protein positions (the recipe below), the hydrogen refinement (if
+ * vb_set_caph was called), the evaluation with its signed reduction into ef, the non-bonded term at the same positions
+ * (if vb_set_nonbonded was called; on top of the bonded values), and the engine's all-reduce of ef (after vb_comm_connect
+ * with option comm_auto = 1) -- exactly the launches of vb_md_eval, without its restraint forces.  It writes no MD state:
+ * positions, velocities, the step counter, restraints, the frame recorder, the noise stream and vb_md_setup's buffer stay
+ * as they are.  It does use the workspace the MD step uses (fragment positions, model buffers, refinement and MM scratch),
+ * so it must not run while MD work of the same handle runs: the host entry waits for the device first when vb_md_setup
+ * was called (MD steps enqueued on any stream finish before its replay starts, and it returns synchronised); the device
+ * entry is ordered like every asynchronous entry, by the caller, on the stream the MD work uses or after an event of it.
+ * Replaces: FragmentCalculator.calculate, src/Calculators/fragment.py:50-68 (DLBondedCalculator.__call__, bonded.py:102-123,
+ *           with DistanceFragment.get_fragments, distancefrag.py:56-92, and MMNonBondedCalculator, nonbonded.py:24-63,
+ *           added by DipeptideCombiner, combiner.py:44-55). */
+
+/* The placement recipe of the fragment atoms without any MD setup, the arrays of vb_md_setup: real[a] = protein index,
+ * or -1 for an added hydrogen at P[acc[a]] + unit(P[rem[a]] - P[acc[a]]) * blen[a].  Requires vb_set_topology and
+ * vb_set_protein_map with the same n_protein_atoms (VB_ERR_STATE; VB_ERR_ARG for a null array, another n_protein_atoms or
+ * an index out of range).  A handle holds one recipe: this call and vb_md_setup each replace it, and the MD step places
+ * with whichever came last.  vb_set_topology and vb_set_protein_map drop it.  Synchronises. */
+int vb_set_fragment_recipe(vb_handle* h, int64_t n_protein_atoms, const int32_t* real_host, const int32_t* acc_host,
+                           const int32_t* rem_host, const float* blen_host);
+/* prot_pos_dev[3*n_protein] (fp64, Angstrom) -> ef_prot_dev[3*n_protein + 1] (forces, then the energy; overwritten),
+ * device buffers, asynchronous on `stream`: one replay of a CUDA graph cached per buffer pair.  VB_ERR_STATE without a
+ * topology, protein map or recipe, on a derivative = 0 handle, on a handle whose MD step is un-fragmented, and after an
+ * all-reduce timed out (option comm_timeouts); VB_ERR_ARG for a null buffer.  Like vb_forward, an edge overflow of a
+ * trimmed max_edges is only seen by the host entry. */
+int vb_forward_fragments(vb_handle* h, const double* prot_pos_dev, float* ef_prot_dev, void* stream);
+/* The same with HOST buffers, synchronous: one graph replay with the H2D of the positions into pinned staging and the
+ * D2H of [3*n_protein + 1] inside; fails with VB_ERR_STATE when a step produced more edges than a trimmed max_edges.
+ * After vb_md_setup it first synchronises the device, so it may follow MD work enqueued on any stream without a wait. */
+int vb_forward_fragments_host(vb_handle* h, const double* prot_pos_host, float* ef_prot_host);
+
 /* ---- One-shot all-reduce over NVLink peer memory (SURVEY section 8e) ---------------------------------------------
  * One process per GPU.  vb_comm_init allocates this rank's window (2 parities x world slots of max_floats) and returns
  * its 64-byte CUDA IPC handle; the caller exchanges the handles of all ranks (any host transport: torch.distributed,
