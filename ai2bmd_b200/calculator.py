@@ -255,14 +255,10 @@ class FragmentCalculator(_CalculatorBase):
         super().__init__()
         _check_nbcalc_type(nbcalc_type)
         from .engine import check_recipe
-        real, acc, rem, blen = check_recipe(recipe.real, recipe.acc, recipe.rem, recipe.blen)
-        if len(real) != len(frags.z):
-            raise ValueError(f"recipe arrays must have one entry per fragment atom ({len(frags.z)}), not {len(real)}")
+        real, acc, rem, blen = check_recipe(recipe.real, recipe.acc, recipe.rem, recipe.blen, len(frags.z))
         if nonbonded is not None:
-            from .nonbonded import dipeptide_atom_sets, exclusion_table
-            nonbonded = [np.asarray(a, dtype=np.float32).reshape(-1) for a in nonbonded]
-            if len(nonbonded) != 3 or any(len(a) != pm.n_protein for a in nonbonded):
-                raise ValueError(f"nonbonded must be (charges, sigmas_nm, epsilons_kj), {pm.n_protein} entries each")
+            from .nonbonded import check_parameters, dipeptide_atom_sets, exclusion_table
+            nonbonded = check_parameters(nonbonded, pm.n_protein)
             excl = exclusion_table(pm.n_protein, dipeptide_atom_sets(frags, recipe, pm))
         model_path = osp.join(ckpt_path, f"visnet-uni-{ckpt_type}.ckpt") if ckpt_type else ckpt_path
         sd, ckpt_derivative = load_checkpoint(model_path)

@@ -156,6 +156,10 @@ struct vb_handle {
     double *d_fx = nullptr, *h_fx = nullptr;   // [n_protein][3] vb_forward_fragments_host's positions, pinned staging
     float* h_fef = nullptr;                    // [3*n_protein + 1] ... and its pinned result
     int* d_flags = nullptr;      // [0]: set by the neighbour stage when a step produced more edges than the workspace holds
+    // batch window (vb_set_batch_window): the topology is atoms [win_first, win_first + N) of a packed batch of win_batch
+    // atoms, which the placement and the hydrogen refinement fill whole in d_bpos; the evaluation reads its window of it
+    int64_t win_batch = 0, win_first = 0;   // win_batch = 0: no window
+    float* d_bpos = nullptr;                // [win_batch][3]
     // cap-hydrogen refinement (k_caph.cuh): flat term arrays + scratch in one device allocation
     bool caph_ready = false;
     CaphDev caph{};
@@ -243,6 +247,10 @@ struct vb_handle {
     double* d_nb_eatom = nullptr;
 
     bool has_topology_sizes() const { return ws.N > 0; }
+    // the packed batch the placement recipe, the refinement terms and vb_debug_read("pos") address: the window's batch,
+    // else the topology itself
+    int batch_atoms() const { return win_batch ? (int)win_batch : ws.N; }
+    float* batch_pos() const { return win_batch ? d_bpos : d_pos; }
     void set_error(const char* fmt, ...) {
         char buf[1024];
         va_list ap;
@@ -295,6 +303,10 @@ struct vb_handle {
         cudaFree(d_real); cudaFree(d_acc); cudaFree(d_rem); cudaFree(d_blen);
         d_real = d_acc = d_rem = nullptr; d_blen = nullptr;
     }
+    void free_window() {
+        cudaFree(d_bpos);
+        d_bpos = nullptr; win_batch = win_first = 0;
+    }
     void free_md() {
         free_rs();                       // the restraints index the MD state
         free_rec();                      // ... and so does the frame ring
@@ -311,6 +323,7 @@ struct vb_handle {
         free_md();                 // the MD recipe indexes the fragment atoms of the old topology
         free_map();                // ... and so does the protein map: it must be set again
         free_caph();               // ... and the hydrogen-refinement terms
+        free_window();             // ... and the batch window around it
         has_topology = false;
         cudaFree(arena); arena = nullptr; arena_bytes = 0;
         d_pos = d_energy = d_forces = nullptr;
@@ -1280,6 +1293,7 @@ void vb_destroy(vb_handle* h) {
     h->free_nb();
     h->free_comm();
     h->free_caph();
+    h->free_window();
     cudaFree(h->arena);
     h->free_map();
     cudaFree(h->d_flags);
@@ -1560,6 +1574,7 @@ namespace {
 // the evaluation's buffers when it ends in the protein buffer ef [3*n_protein + 1]
 StepIO eval_io(vb_handle* h, float* ef) {
     StepIO io = internal_io(h, false);
+    io.pos = h->batch_pos() + 3 * h->win_first;     // a window evaluates its atoms of the placed batch where they lie
     if (h->md_unfrag) {          // one graph over the protein: its forces and energy are ef itself, no reduction
         io.forces = ef;
         io.energy = ef + 3 * (size_t)h->n_protein;
@@ -1573,12 +1588,14 @@ StepIO md_io(vb_handle* h) { return eval_io(h, h->md_ef); }
 // CTA, with `restrain`] -> evaluation + signed whole-protein reduction into ef [-> non-bonded term at x], all on st.  The
 // MD step passes its own state (d_mx, md_ef, restrain); vb_forward_fragments the caller's buffers and no restraints.
 // Every rank of a sharded run holds the same state and the whole term set, so each computes the same rf; only ef goes
-// through the all-reduce.
+// through the all-reduce.  On a windowed handle the placement and the refinement cover the whole batch, exactly as a
+// handle of the whole batch runs them, and the evaluation reads the window.
 int md_eval_enqueue(vb_handle* h, cudaStream_t st, const double* x, float* ef, bool restrain) {
-    const int N = h->ws.N;
+    const int N = h->batch_atoms();
+    float* pos = h->batch_pos();
     md_place_kernel<<<(N + 255) / 256 + (restrain && h->rs_ready ? 1 : 0), 256, 0, st>>>(N, h->d_real, h->d_acc, h->d_rem,
-                                                                                        h->d_blen, x, h->d_pos, h->rs);
-    if (h->caph_ready) caph_relax_kernel<<<1, CAPH_THREADS, 0, st>>>(h->caph, h->d_pos);   // hydrogen refinement, in place
+                                                                                        h->d_blen, x, pos, h->rs);
+    if (h->caph_ready) caph_relax_kernel<<<1, CAPH_THREADS, 0, st>>>(h->caph, pos);   // hydrogen refinement, in place
     if (int rc = enqueue_eval(h, st, eval_io(h, ef))) return rc;
     if (h->nb_ready && h->nb.hi > h->nb.lo) {      // non-bonded MM term on the same protein coordinates
         nonbonded_kernel<double><<<(h->nb.hi - h->nb.lo + 7) / 8, 256, 0, st>>>(h->nb, x, ef, h->d_nb_eatom);
@@ -1633,6 +1650,7 @@ int md_setup_unfragmented(vb_handle* h, int64_t n_protein_atoms, const double* m
     if (int rc = need_derivative(h, "vb_md_setup")) return rc;
     if (h->d_map_rowptr) return fail(VB_ERR_STATE, "a protein map is set, and the un-fragmented step uses none; call vb_set_topology again");
     if (h->caph_ready) return fail(VB_ERR_STATE, "hydrogen refinement is set (vb_set_caph), and one graph has no added hydrogens");
+    if (h->win_batch) return fail(VB_ERR_STATE, "a batch window is set (vb_set_batch_window), and one graph is no window of a batch");
     if (h->comm_ready && h->comm.world > 1) return fail(VB_ERR_STATE, "connected to several ranks: one graph cannot be sharded");
     if (h->ws.G != 1) return fail(VB_ERR_ARG, "the topology must be ONE graph (n_graphs == 1)");
     if (n_protein_atoms != h->ws.N) return fail(VB_ERR_ARG, "n_protein_atoms must equal the topology's atom count");
@@ -1665,7 +1683,8 @@ int md_setup_unfragmented(vb_handle* h, int64_t n_protein_atoms, const double* m
 }
 
 // The placement recipe of the fragment atoms, as vb_md_setup and vb_set_fragment_recipe take it: the handle must have a
-// topology and a protein map of n_protein_atoms atoms, and every index must address that protein.  Called with h->mu held.
+// topology and a protein map of n_protein_atoms atoms, and every index must address that protein.  The arrays have one
+// entry per atom of the batch (of the window, when one is set).  Called with h->mu held.
 int check_recipe(vb_handle* h, const char* who, int64_t n_protein_atoms, const int32_t* real, const int32_t* acc,
                  const int32_t* rem, const float* blen) {
     if (!h->has_topology || h->n_protein <= 0 || !h->d_map_rowptr) { h->set_error("%s: topology / protein map not set", who); return VB_ERR_STATE; }
@@ -1673,7 +1692,7 @@ int check_recipe(vb_handle* h, const char* who, int64_t n_protein_atoms, const i
         h->set_error("%s: bad arguments (null recipe array, or n_protein differs from the protein map's %d)", who, h->n_protein);
         return VB_ERR_ARG;
     }
-    const int N = h->ws.N, P = h->n_protein;
+    const int N = h->batch_atoms(), P = h->n_protein;
     for (int a = 0; a < N; a++) {
         const bool cap = real[a] < 0;
         if ((!cap && real[a] >= P) || (cap && (acc[a] < 0 || acc[a] >= P || rem[a] < 0 || rem[a] >= P || acc[a] == rem[a]))) {
@@ -1685,7 +1704,7 @@ int check_recipe(vb_handle* h, const char* who, int64_t n_protein_atoms, const i
 }
 // ... and its upload in place of the handle's recipe (the caller has dropped the graphs that hold the old pointers)
 int upload_recipe(vb_handle* h, const int32_t* real, const int32_t* acc, const int32_t* rem, const float* blen) {
-    const int N = h->ws.N;
+    const int N = h->batch_atoms();
     h->free_recipe();
     CUDA_TRY(h, cudaMalloc(&h->d_real, sizeof(int) * N));
     CUDA_TRY(h, cudaMalloc(&h->d_acc, sizeof(int) * N));
@@ -2213,6 +2232,40 @@ int vb_set_fragment_recipe(vb_handle* h, int64_t n_protein_atoms, const int32_t*
     return upload_recipe(h, real_host, acc_host, rem_host, blen_host);
 }
 
+int vb_set_batch_window(vb_handle* h, int64_t n_batch_atoms, int64_t first_atom) {
+    NvtxRange nvtx_("vb_set_batch_window");
+    if (!h) return VB_ERR_ARG;
+    std::lock_guard<std::mutex> lk(h->mu);
+    auto fail = [&](int rc, const char* what) { h->set_error("vb_set_batch_window: %s", what); return rc; };
+    if (!h->has_topology) return fail(VB_ERR_STATE, "call vb_set_topology first");
+    if (h->md_unfrag)
+        return fail(VB_ERR_STATE, "the MD step is set up un-fragmented (vb_md_setup with real_host = NULL): one graph is "
+                                  "not a window of a fragment batch");
+    if (h->md_ready || h->d_real || h->caph_ready)
+        return fail(VB_ERR_STATE, "a placement recipe (vb_md_setup / vb_set_fragment_recipe) or the hydrogen refinement "
+                                  "(vb_set_caph) is set and indexes the topology: set the window first, then those");
+    const int64_t N = h->ws.N;
+    if (n_batch_atoms > (1 << 26) || first_atom < 0 || first_atom + N > n_batch_atoms) {
+        h->set_error("vb_set_batch_window: the topology's %lld atoms from atom %lld do not lie in a batch of %lld atoms",
+                     (long long)N, (long long)first_atom, (long long)n_batch_atoms);
+        return VB_ERR_ARG;
+    }
+    CUDA_TRY(h, cudaSetDevice(h->device));
+    CUDA_TRY(h, cudaDeviceSynchronize());      // no enqueued evaluation may still read the old batch buffer
+    h->drop_graph();
+    h->free_window();
+    if (n_batch_atoms == N) return VB_OK;      // the window (N, 0) is the topology itself: no window
+    if (cudaMalloc(&h->d_bpos, sizeof(float) * 3 * (size_t)n_batch_atoms) != cudaSuccess) {
+        (void)cudaGetLastError();
+        h->d_bpos = nullptr;
+        return fail(VB_ERR_ALLOC, "allocation of the batch positions failed");
+    }
+    CUDA_TRY(h, cudaMemset(h->d_bpos, 0, sizeof(float) * 3 * (size_t)n_batch_atoms));
+    h->win_batch = n_batch_atoms;
+    h->win_first = first_atom;
+    return VB_OK;
+}
+
 namespace {
 int fragments_check(vb_handle* h, const char* who) {
     if (h->md_unfrag) {
@@ -2359,7 +2412,7 @@ int vb_set_caph(vb_handle* h, const vb_caph_problem* pr) {
         return VB_ERR_STATE;
     }
     if (!pr) { h->set_error("vb_set_caph: null problem"); return VB_ERR_ARG; }
-    const int64_t N = h->ws.N;
+    const int64_t N = h->batch_atoms();
     auto bad = [&](const char* what) { h->set_error("vb_set_caph: %s", what); return VB_ERR_ARG; };
     if (pr->n_h < 0 || pr->n_bonds < 0 || pr->n_angles < 0 || pr->n_dih < 0 || pr->n_pairs < 0 || pr->n_mirror < 0) return bad("negative count");
     if (pr->max_iter < 1 || pr->max_iter > 64) return bad("max_iter must be in [1, 64]");
@@ -2666,6 +2719,8 @@ int64_t vb_get_option(const vb_handle* h, const char* key) {
     if (k == "md_unfragmented") return h->md_unfrag ? 1 : 0;
     if (k == "graph_captures") return h->graph_captures;
     if (k == "md_loop_pdl") return h->loop_pdl;
+    if (k == "batch_atoms") return h->batch_atoms();
+    if (k == "batch_first_atom") return h->win_first;
     if (k == "caph_evals") {           // energy evaluations of the last refinement (synchronises)
         int v = 0;
         if (!h->caph_ready || cudaDeviceSynchronize() != cudaSuccess ||
@@ -2903,7 +2958,7 @@ int64_t vb_debug_read(vb_handle* h, const char* name, int layer, void* host_dst,
     else BUF("eatom", ws.eatom, N, 4)
     else BUF("energy", h->d_energy, G, 4)
     else BUF("forces", h->d_forces, N * 3, 4)
-    else BUF("pos", h->d_pos, N * 3, 4)
+    else BUF("pos", h->batch_pos(), (size_t)h->batch_atoms() * 3, 4)
     else if (k == "RF" && h->rs_ready) { src = h->rs.rf; bytes = (3 * (size_t)h->n_protein + 1) * 8; }
 #undef BUF
     if (!src) { h->set_error("vb_debug_read: unknown buffer %s[%d]", name, layer); return VB_ERR_ARG; }

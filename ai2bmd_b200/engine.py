@@ -45,7 +45,7 @@ EXPORTED_SYMBOLS = [
     "vb_set_nonbonded", "vb_nonbonded",
     "vb_comm_init", "vb_comm_connect", "vb_comm_allreduce",
     "vb_set_caph", "vb_caph_relax", "vb_chunk_fragments",
-    "vb_set_fragment_recipe", "vb_forward_fragments", "vb_forward_fragments_host",
+    "vb_set_fragment_recipe", "vb_forward_fragments", "vb_forward_fragments_host", "vb_set_batch_window",
 ]
 
 
@@ -159,18 +159,23 @@ def load_library(path: Optional[str] = None):
     lib.vb_forward_fragments.argtypes = [vp, vp, vp, vp]
     lib.vb_forward_fragments_host.restype = C.c_int
     lib.vb_forward_fragments_host.argtypes = [vp, vp, vp]
+    lib.vb_set_batch_window.restype = C.c_int
+    lib.vb_set_batch_window.argtypes = [vp, i64, i64]
     if path == _build.LIB_PATH:
         _lib = lib
     return lib
 
 
-def check_recipe(real, acc, rem, blen):
+def check_recipe(real, acc, rem, blen, n_atoms: Optional[int] = None):
     """The four arrays of a fragment placement recipe as the C ABI takes them (int32, int32, int32, float32), one entry
-    per fragment atom each; raises ``ValueError`` before anything reaches the engine."""
+    per fragment atom each -- ``n_atoms`` of them when given (the batch's atoms, on a windowed engine); raises
+    ``ValueError`` before anything reaches the engine."""
     r, a, q = (np.ascontiguousarray(v, dtype=np.int32) for v in (real, acc, rem))
     b = np.ascontiguousarray(blen, dtype=np.float32)
     if not (r.ndim == a.ndim == q.ndim == b.ndim == 1 and len(r) == len(a) == len(q) == len(b)):
         raise ValueError("recipe arrays must be 1-D with one entry per fragment atom")
+    if n_atoms is not None and len(r) != n_atoms:
+        raise ValueError(f"recipe arrays must have one entry per fragment atom ({n_atoms}), not {len(r)}")
     return r, a, q, b
 
 
@@ -189,6 +194,8 @@ class Engine:
     ``chunk_atoms=C > 0`` (option ``"chunk_atoms"``) evaluates the batch in contiguous fragment chunks of about C atoms
     (:func:`ai2bmd_b200.parallel.chunk_fragments`) on one workspace sized for the largest chunk: the reference's
     ``--chunk-size``, a bound on the engine's device memory.  0 evaluates the batch in one pass."""
+
+    _window = None          # (n_batch_atoms, first_atom) of set_batch_window, while one is set
 
     def __init__(self, state_dict: Dict[str, np.ndarray], device: int = 0, cutoff: float = 5.0, derivative: bool = True,
                  chunk_atoms: int = 0):
@@ -239,6 +246,21 @@ class Engine:
         self._check(self.lib.vb_set_topology(self.h, z.size, g, z.ctypes.data, batch.ctypes.data, int(max_edges)),
                     "vb_set_topology")
         self.n_atoms, self.n_graphs = int(z.size), g
+        self._window = None
+
+    def set_batch_window(self, n_batch_atoms: int, first_atom: int):
+        """Declare the topology to be atoms ``[first_atom, first_atom + n_atoms)`` of a packed batch of ``n_batch_atoms``
+        (``vb_set_batch_window``): the placement recipe, the refinement problem and ``debug_read("pos")`` then address the
+        batch, which every evaluation places and refines whole before it evaluates this window.  Call it before
+        ``set_fragment_recipe``, ``md_setup`` and ``set_caph``; ``(n_atoms, 0)`` removes the window."""
+        self._check(self.lib.vb_set_batch_window(self.h, int(n_batch_atoms), int(first_atom)), "vb_set_batch_window")
+        self._window = (int(n_batch_atoms), int(first_atom)) if int(n_batch_atoms) != self.n_atoms else None
+
+    @property
+    def batch_atoms(self) -> int:
+        """Atoms of the packed batch the placement recipe and the refinement address: the window's batch, else the
+        topology's."""
+        return self._window[0] if self._window else self.n_atoms
 
     def set_protein_map(self, n_protein, src_atom, dst_atom, sign, frag_sign):
         src_atom = np.ascontiguousarray(src_atom, dtype=np.int32)
@@ -257,6 +279,7 @@ class Engine:
         if key in ("derivative", "chunk_atoms"):      # the library dropped the topology: set_topology again
             setattr(self, key, bool(value) if key == "derivative" else int(value))
             self.n_atoms = self.n_graphs = self.n_protein = 0
+            self._window = None
 
     def get_option(self, key: str) -> int:
         return int(self.lib.vb_get_option(self.h, key.encode()))
@@ -328,9 +351,7 @@ class Engine:
     def set_fragment_recipe(self, real, acc, rem, blen):
         """The placement recipe of every fragment atom (a :class:`ai2bmd_b200.pdbfrag.FragmentRecipe`'s arrays) for the
         protein of the protein map, without any MD setup; replaces the recipe of an earlier call or ``md_setup``."""
-        r, a, q, b = check_recipe(real, acc, rem, blen)
-        if len(r) != self.n_atoms:
-            raise ValueError(f"recipe arrays must have one entry per fragment atom ({self.n_atoms}), not {len(r)}")
+        r, a, q, b = check_recipe(real, acc, rem, blen, self.batch_atoms)
         self._check(self.lib.vb_set_fragment_recipe(self.h, self.n_protein, r.ctypes.data, a.ctypes.data, q.ctypes.data,
                                                     b.ctypes.data), "vb_set_fragment_recipe")
 
@@ -387,12 +408,8 @@ class Engine:
 
     # ---- device-resident MD (include/visnet_b200.h: vb_md_*) ----
     def md_setup(self, masses, real, acc, rem, blen, dt, kT, friction, seed, ef_ptr: int):
-        self._md_keep = [np.ascontiguousarray(masses, dtype=np.float64), np.ascontiguousarray(real, dtype=np.int32),
-                         np.ascontiguousarray(acc, dtype=np.int32), np.ascontiguousarray(rem, dtype=np.int32),
-                         np.ascontiguousarray(blen, dtype=np.float32)]
+        self._md_keep = [np.ascontiguousarray(masses, dtype=np.float64), *check_recipe(real, acc, rem, blen, self.batch_atoms)]
         m, r, a, q, b = self._md_keep
-        if not (len(r) == len(a) == len(q) == len(b)):
-            raise ValueError("recipe arrays must have one entry per fragment atom")
         self._check(self.lib.vb_md_setup(self.h, len(m), m.ctypes.data, r.ctypes.data, a.ctypes.data, q.ctypes.data,
                                          b.ctypes.data, float(dt), float(kT), float(friction), int(seed), ef_ptr),
                     "vb_md_setup")

@@ -236,6 +236,37 @@ class DeviceLangevin:
         self._start(positions, velocities, seed, step, noise, noise_state, zero_com_momentum)
 
     @classmethod
+    def sharded(cls, state_dict, frags: FragmentData, pm: ProteinMap, recipe: FragmentRecipe, positions, numbers, group, *,
+                caph=None, nonbonded=None, chunk_atoms: int = 0, native_comm: bool = True, device: int = None, **kwargs):
+        """This rank's part of a step sharded over ``group`` (one rank per GPU) with the hydrogen refinement and the MM
+        term: the reference's step on several devices.  The rank's :class:`ai2bmd_b200.parallel.DeviceShard` evaluates
+        its block of fragments (``partition_fragments``), but places and refines the WHOLE batch first
+        (``DeviceShard.set_window``), so every rank refines exactly what one GPU would; ``caph`` is the whole batch's
+        :class:`ai2bmd_b200.caph.CapHProblem` and ``recipe`` the whole batch's.  ``nonbonded = (charges, sigmas,
+        epsilons)`` adds the MM term, each rank computing an even split of its rows (``parallel.mm_rows``).  The ranks
+        combine the force buffer with the engine's own all-reduce inside the step graph (``native_comm``; NCCL between
+        the kicks where peer memory is unavailable).  ``device`` defaults to the current CUDA device; the other keyword
+        arguments are the constructor's.  A recipe or MM parameters of the wrong length, or more ranks than blocks,
+        raise ``ValueError`` before any engine is made."""
+        from .engine import check_recipe
+        from .nonbonded import check_parameters
+        from .parallel import DeviceShard, check_shardable
+        check_recipe(recipe.real, recipe.acc, recipe.rem, recipe.blen, len(frags.z))
+        if nonbonded is not None:
+            check_parameters(nonbonded, pm.n_protein)
+        import torch
+        import torch.distributed as dist
+        world = dist.get_world_size(group)
+        check_shardable(frags, world)
+        device = torch.cuda.current_device() if device is None else int(device)
+        sh = DeviceShard(state_dict, frags, pm, dist.get_rank(group), world, device, native_comm=native_comm,
+                         chunk_atoms=chunk_atoms)
+        sh.set_window(frags, pm, recipe, caph=caph, nonbonded=nonbonded)
+        self = cls(None, None, pm, recipe, positions, numbers, device=device, group=group, engine=sh.engine, **kwargs)
+        self.shard = sh
+        return self
+
+    @classmethod
     def unfragmented(cls, state_dict, numbers, positions, *, dt_fs=1.0, temperature_K=300.0, friction_per_fs=0.001,
                      seed=0, device: int = 0, velocities=None, step: int = 0, noise: str = "philox",
                      noise_state: int = None, chunk_atoms: int = 0, zero_com_momentum=False, group=None):

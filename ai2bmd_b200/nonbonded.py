@@ -26,6 +26,15 @@ def dipeptide_atom_sets(frags, recipe, pm) -> list:
     return sets
 
 
+def check_parameters(nonbonded, n_protein: int):
+    """``(charges [e], sigmas [nm], epsilons [kJ/mol])``, one entry per protein atom each, as float32 arrays; raises
+    ``ValueError`` otherwise."""
+    nonbonded = [np.asarray(a, dtype=np.float32).reshape(-1) for a in nonbonded]
+    if len(nonbonded) != 3 or any(len(a) != n_protein for a in nonbonded):
+        raise ValueError(f"nonbonded must be (charges, sigmas_nm, epsilons_kj), {n_protein} entries each")
+    return nonbonded
+
+
 def exclusion_table(n_atoms: int, groups: Sequence[np.ndarray]) -> Tuple[np.ndarray, np.ndarray]:
     """CSR table (rowptr [n+1], col) of excluded partners: j is listed under i iff i != j share a group
     (``distancefrag.py:355-361``: every combination inside a dipeptide, both orders).  Rows are ascending."""

@@ -79,6 +79,20 @@ def chunk_fragments(start: Sequence[int], end: Sequence[int], chunk_atoms: int) 
     return [(int(bounds[c]), int(bounds[c + 1])) for c in range(n)]
 
 
+def mm_rows(n_protein: int, rank: int, world_size: int) -> Tuple[int, int]:
+    """The destination atoms [lo, hi) of the MM term one rank computes: an even split of the protein atoms."""
+    return n_protein * rank // world_size, n_protein * (rank + 1) // world_size
+
+
+def check_shardable(frags: FragmentData, world_size: int):
+    """Every rank needs a block of fragments to hold an engine; raises ``ValueError`` when
+    :func:`partition_fragments` leaves a rank without one."""
+    parts = partition_fragments(frags.start, frags.end, world_size)
+    empty = [r for r, (lo, hi) in enumerate(parts) if hi <= lo]
+    if empty:
+        raise ValueError(f"{len(frags)} fragments over {world_size} ranks leave rank(s) {empty} without a block")
+
+
 def shard_protein_map(pm: ProteinMap, frags: FragmentData, lo: int, hi: int) -> ProteinMap:
     """Restrict the signed force map to fragments [lo, hi), re-basing fragment-atom indices to the shard."""
     if hi <= lo:
@@ -191,6 +205,24 @@ class DeviceShard:
             self.native = bool(int(flag.item()))
             if not self.native:
                 self.comm_engine.set_option("comm_auto", 0)
+
+    def set_window(self, frags: FragmentData, pm: ProteinMap, recipe, caph=None, nonbonded=None):
+        """Make this rank place and refine the WHOLE batch, as the reference does on one device before it splits the
+        fragments (``bonded.py:64-110``), and evaluate its own block of it (``vb_set_batch_window``): the window, then the
+        whole placement ``recipe`` and the whole :class:`ai2bmd_b200.caph.CapHProblem` ``caph`` (optional).  Every rank's
+        placed and refined batch is bit-identical to a single-GPU handle's.  ``nonbonded = (charges, sigmas, epsilons)``
+        (optional) sets this rank's rows of the MM term, :func:`mm_rows`, with the exclusions ``FragmentCalculator`` uses.
+        A rank without fragments has no engine and cannot take part: :func:`check_shardable` refuses that case."""
+        from .nonbonded import check_parameters, dipeptide_atom_sets, exclusion_table
+        eng = self.engine
+        eng.set_batch_window(len(frags.z), self.plan.atom_lo)
+        eng.set_fragment_recipe(recipe.real, recipe.acc, recipe.rem, recipe.blen)
+        if caph is not None:
+            eng.set_caph(caph)
+        if nonbonded is not None:
+            q, sg, ep = check_parameters(nonbonded, pm.n_protein)
+            rowptr, col = exclusion_table(pm.n_protein, dipeptide_atom_sets(frags, recipe, pm))
+            eng.set_nonbonded(q, sg, ep, rowptr, col, *mm_rows(pm.n_protein, self.plan.rank, self.plan.world_size))
 
     @property
     def collective(self) -> str:

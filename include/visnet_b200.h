@@ -144,7 +144,7 @@ int vb_chunk_fragments(int64_t n_graphs, const int64_t* frag_start_host, int64_t
  * velocity Verlet (no random numbers, no centre-of-mass correction).  Normals come from Philox4x32-10 keyed by
  * (seed; step, component): every rank of a sharded run draws the same numbers.
  *
- * vb_md_setup: recipe per FRAGMENT atom a (arrays of length N): real[a] = protein index, or -1 for an added
+ * vb_md_setup: recipe per FRAGMENT atom a (arrays of length N, or of the batch after vb_set_batch_window): real[a] = protein index, or -1 for an added
  * hydrogen placed at P[acc[a]] + unit(P[rem[a]] - P[acc[a]]) * blen[a].  ef_prot_dev[3*n_protein + 1] is the
  * caller-owned force/energy buffer (must hold forces of the current positions before the first kick1: call
  * vb_md_eval after vb_md_set_state).  Requires vb_set_protein_map with the same n_protein_atoms.
@@ -271,7 +271,7 @@ int vb_nonbonded(vb_handle* h, const float* prot_pos_dev, float* ef_prot_dev, vo
  * One LBFGS call (lr, max_iter, tolerance_grad, tolerance_change; no line search, fresh state) on the Amber energy of all
  * dipeptides, moving only the added hydrogens -- what the reference runs every MD step between placing them and the
  * ViSNet evaluation.  The problem is given as flat term arrays whose atom indices address the PACKED FRAGMENT position
- * buffer [N][3] of vb_set_topology: every term that contains an optimised hydrogen, with its own parameters (Amber
+ * buffer [N][3] of vb_set_topology (of the batch after vb_set_batch_window): every term that contains an optimised hydrogen, with its own parameters (Amber
  * units: kcal/mol, Angstrom, radians; qq = product of prmtop charges).  mirror_dst/mirror_src: fragment atoms that are
  * copies of relaxed ones (the ACE-NME fragments take their hydrogens from the neighbouring dipeptides,
  * src/Fragmentation/distancefrag.py:286-307) and are re-copied after the relaxation.
@@ -327,6 +327,25 @@ int vb_forward_fragments(vb_handle* h, const double* prot_pos_dev, float* ef_pro
  * D2H of [3*n_protein + 1] inside; fails with VB_ERR_STATE when a step produced more edges than a trimmed max_edges.
  * After vb_md_setup it first synchronises the device, so it may follow MD work enqueued on any stream without a wait. */
 int vb_forward_fragments_host(vb_handle* h, const double* prot_pos_host, float* ef_prot_host);
+
+/* ---- A window of a fragment batch: one rank's shard that places and refines the whole batch ---------------------------
+ * Declares the topology of vb_set_topology, N atoms, to be atoms [first_atom, first_atom + N) of a packed fragment batch of
+ * n_batch_atoms atoms.  From then on the placement recipe (vb_md_setup, vb_set_fragment_recipe: arrays of n_batch_atoms
+ * entries), every atom index of vb_set_caph, the buffer vb_caph_relax refines and vb_debug_read("pos") address the BATCH,
+ * while the protein map, the evaluation and its chunks stay the topology's.  The evaluation of the MD step and of
+ * vb_forward_fragments* (md_eval_enqueue) places every batch atom into a batch-sized buffer of the handle, refines the
+ * added hydrogens of the whole batch -- one CTA with fixed-order sums, so the buffer is bit-identical to that of a handle
+ * of the whole batch -- and then evaluates its window where it lies in that buffer (no copy): the same launches as a
+ * handle without a window.  This is the sharded form of the reference's step, which relaxes the hydrogens of all
+ * dipeptides in one LBFGS before it splits the fragments over devices (DLBondedCalculator.__call__,
+ * src/Calculators/bonded.py:64-110).  Each rank sets the window of its shard, then the whole recipe and the whole
+ * refinement problem, and the ranks all-reduce ef as before.
+ * Set the window before the recipe, vb_md_setup and vb_set_caph: VB_ERR_STATE once any of them is set, without a
+ * topology, and on an un-fragmented MD handle (and vb_md_setup with real_host == NULL refuses a windowed handle).
+ * VB_ERR_ARG for a window outside the batch.  (N, 0) is the handle without a window; vb_set_topology, and the options
+ * that drop the topology, drop the window.  vb_get_option answers "batch_atoms" (n_batch_atoms, or N without a window)
+ * and "batch_first_atom".  Synchronises. */
+int vb_set_batch_window(vb_handle* h, int64_t n_batch_atoms, int64_t first_atom);
 
 /* ---- One-shot all-reduce over NVLink peer memory (SURVEY section 8e) ---------------------------------------------
  * One process per GPU.  vb_comm_init allocates this rank's window (2 parities x world slots of max_floats) and returns
@@ -385,7 +404,8 @@ int vb_tc_selftest(int device, const float* a_host, const float* img_host, float
 int vb_tc_selftest_rows(int device, int rows, const float* a_host, const float* img_host, float* d_host, int reps, float* ms_out);
 /* Copy an internal buffer to the host.  name: "X","V","F","VN","QKV","V123","VDOT","TU","O" (per layer),
  * "XA","VA","GX","GVEC","GF","GXA","GQKV","GVNMSG","GTU","geom","rbf","eacc","grbf","esrc","edst","rowptr",
- * "eatom","energy","forces","pos" (the packed fragment positions [N*3] the MD placement and hydrogen refinement write),
+ * "eatom","energy","forces","pos" (the packed fragment positions [N*3] the MD placement and hydrogen refinement write;
+ * with vb_set_batch_window those of the whole batch),
  * and "RF" (fp64 restraint forces then energy [3*n_protein + 1], while restraints are set).
  * Returns the number of bytes copied (<= cap_bytes) or a negative status. */
 int64_t vb_debug_read(vb_handle* h, const char* name, int layer, void* host_dst, int64_t cap_bytes);
