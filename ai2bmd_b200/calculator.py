@@ -7,7 +7,8 @@ Mirrors, name for name, the classes of ``/root/reference/src/Calculators`` that 
 * :class:`ViSNetCalculator`   <- ``visnet_calculator.py:121-155`` (un-fragmented ``--mode visnet``)
 * :class:`DipeptideBondedCombiner` <- ``combiner.py:11-41``
 * :class:`DLBondedCalculator` <- ``bonded.py:19-123`` (fragment-batch evaluation + combine)
-* :class:`FragmentCalculator` <- ``fragment.py:16-68`` (placement, hydrogen refinement, bonded + MM term in one device call)
+* :class:`FragmentCalculator` <- ``fragment.py:16-68`` (placement, hydrogen refinement, bonded + MM term in one device call,
+  on one GPU or, with ``devices``, on a group of them: ``bonded.py:64-89``)
 
 ASE is not a dependency: calculators expose ``calculate(atoms, ...)`` / ``get_potential_energy`` /
 ``get_forces`` with ASE semantics (results cached while positions are unchanged,
@@ -17,7 +18,8 @@ All compute goes through the C-ABI library; nothing here falls back to PyTorch o
 from __future__ import annotations
 
 import os.path as osp
-from typing import Dict, Optional, Tuple
+from concurrent.futures import ThreadPoolExecutor
+from typing import Dict, List, Optional, Tuple
 
 import numpy as np
 
@@ -32,6 +34,20 @@ def _device_index(device: str) -> int:
     if not device.startswith("cuda"):
         raise ValueError(f"Unrecognized device {device!r}")   # device_strategy.py:24-35
     return int(device.split(":")[1]) if ":" in device else 0
+
+
+def _device_list(devices) -> Optional[List[str]]:
+    """The ``devices`` argument of the multi-device calculators: a list or tuple of devices (duplicates allowed, e.g.
+    ``["cuda:0", "cuda:0"]``; the reference's ``DeviceStrategy.get_bonded_devices()``) is returned as a list of strings,
+    each checked as a device; None or one device is None, the single-device path."""
+    if devices is None or not isinstance(devices, (list, tuple)):
+        return None
+    devs = [str(d) for d in devices]
+    if not devs:
+        raise ValueError("devices must name at least one device")
+    for d in devs:
+        _device_index(d)
+    return devs
 
 
 class ViSNetModel:
@@ -203,18 +219,38 @@ class DLBondedCalculator:
     whole-protein reduction can also run on the device through ``Engine.set_protein_map`` /
     ``forward_protein_device`` (used by ``parallel.ShardedBondedCalculator`` for the multi-GPU path).
     ``chunk_size`` is the reference's ``--chunk-size`` (``DeviceStrategy._chunk_size``): the engine evaluates the batch
-    in fragment chunks of about that many atoms, one after the other on one bounded workspace (None: one pass)."""
+    in fragment chunks of about that many atoms, one after the other on one bounded workspace (None: one pass).
+    ``devices`` is the reference's multi-device ``calculate`` (``bonded.py:64-89``): a list of devices (duplicates
+    allowed) gets one engine per entry, each evaluates its block of :func:`ai2bmd_b200.parallel.partition_fragments`
+    from a thread pool (the engine calls release the GIL), and the results are concatenated in fragment order.  None or
+    one device is the single-device path."""
 
     def __init__(self, ckpt_path: str, ckpt_type: str = "", device: str = "cuda:0", chunk_size: Optional[int] = None,
-                 **kwargs):
+                 devices=None, **kwargs):
         model_path = osp.join(ckpt_path, f"visnet-uni-{ckpt_type}.ckpt") if ckpt_type else ckpt_path
-        self.models = [get_visnet_model(model_path, device, chunk_size=chunk_size)]
+        devs = _device_list(devices)
+        if devs is None:
+            self.models = [get_visnet_model(model_path, device if devices is None else str(devices), chunk_size=chunk_size)]
+        else:            # one engine per entry, also for a device named twice: each keeps its own block's topology
+            sd, ckpt_derivative = load_checkpoint(model_path)
+            derivative = resolve_derivative(ckpt_derivative, None)
+            self.models = [ViSNetModel(sd, device=d, derivative=derivative, chunk_size=chunk_size) for d in devs]
         if not self.models[0].derivative:
             raise ValueError(f"{model_path}: the bonded calculator needs forces, and the checkpoint has derivative=False")
         self.combiner = DipeptideBondedCombiner()
 
+    def _evaluate(self, fragments: FragmentData):
+        if len(self.models) == 1:
+            return self.models[0].dl_potential_loader(fragments)
+        from .parallel import partition_fragments
+        parts = partition_fragments(fragments.start, fragments.end, len(self.models))
+        jobs = [(m, fragments[lo:hi]) for m, (lo, hi) in zip(self.models, parts) if hi > lo]
+        with ThreadPoolExecutor(len(jobs)) as pool:
+            out = list(pool.map(lambda job: job[0].dl_potential_loader(job[1]), jobs))
+        return np.concatenate([e for e, _ in out]), np.concatenate([f for _, f in out])
+
     def calculate(self, fragments: FragmentData):
-        energy, forces = self.models[0].dl_potential_loader(fragments)
+        energy, forces = self._evaluate(fragments)
         dip_e, an_e = (energy[s] for s in fragments.scalar_split())
         dip_f, an_f = (forces[s] for s in fragments.vector_split())
         return dip_e, dip_f, an_e, an_f
@@ -248,23 +284,53 @@ class FragmentCalculator(_CalculatorBase):
     epsilons [kJ/mol])`` per protein atom turns the MM term on, with the reference's exclusions (atoms sharing a
     dipeptide); without it the calculator is the reference's ``DLBondedCalculator.__call__``.  ``nbcalc_type`` is the
     reference's ``--fragment-longrange-calc``: ``"mm"`` only, ``"pme"`` raises ``NotImplementedError``.  ``chunk_size`` is
-    the reference's ``--chunk-size`` (``Engine(chunk_atoms=...)``).  Arguments are checked before any engine is made."""
+    the reference's ``--chunk-size`` (``Engine(chunk_atoms=...)``).  Arguments are checked before any engine is made.
+
+    ``devices`` spreads the call over several GPUs of this process, as the reference's bonded devices do
+    (``DeviceStrategy.get_bonded_devices()``, ``bonded.py:64-89``; the default ``--solvent`` run calls it from
+    ``AsyncQMMM``'s worker thread): a list of devices (duplicates allowed, e.g. ``["cuda:0", "cuda:0"]``) builds one
+    window engine per entry on its block of :func:`ai2bmd_b200.parallel.partition_fragments`, set up as a rank of the
+    sharded path (:meth:`ai2bmd_b200.parallel.DeviceShard.set_window`: the whole placement and refinement, its own
+    fragments, its rows of the MM term) and calibrated on the start geometry, joined by an
+    :class:`ai2bmd_b200.engine.EngineGroup` that sums their buffers on the first device.  A list that leaves an entry
+    without fragments is refused (:func:`ai2bmd_b200.parallel.check_shardable`).  None or one device is the
+    single-device path; ``calculate`` is the same either way."""
 
     def __init__(self, ckpt_path: str, ckpt_type: str, frags: FragmentData, pm, recipe, caph=None, nonbonded=None,
-                 nbcalc_type: str = "mm", device: str = "cuda:0", chunk_size: Optional[int] = None, **kwargs):
+                 nbcalc_type: str = "mm", device: str = "cuda:0", chunk_size: Optional[int] = None, devices=None,
+                 **kwargs):
         super().__init__()
         _check_nbcalc_type(nbcalc_type)
         from .engine import check_recipe
         real, acc, rem, blen = check_recipe(recipe.real, recipe.acc, recipe.rem, recipe.blen, len(frags.z))
+        devs = _device_list(devices)
+        if devs is None:
+            device = device if devices is None else str(devices)
+        else:
+            from .parallel import check_shardable
+            check_shardable(frags, len(devs))
         if nonbonded is not None:
             from .nonbonded import check_parameters, dipeptide_atom_sets, exclusion_table
             nonbonded = check_parameters(nonbonded, pm.n_protein)
-            excl = exclusion_table(pm.n_protein, dipeptide_atom_sets(frags, recipe, pm))
+            excl = exclusion_table(pm.n_protein, dipeptide_atom_sets(frags, recipe, pm)) if devs is None else None
         model_path = osp.join(ckpt_path, f"visnet-uni-{ckpt_type}.ckpt") if ckpt_type else ckpt_path
         sd, ckpt_derivative = load_checkpoint(model_path)
         if not resolve_derivative(ckpt_derivative, None):
             raise ValueError(f"{model_path}: the fragment calculator needs forces, and the checkpoint has derivative=False")
-        self.device, self.n_protein = device, int(pm.n_protein)
+        self.n_protein = int(pm.n_protein)
+        self.devices, self.shards, self.group = devs, None, None
+        if devs is not None:
+            from .engine import EngineGroup
+            from .parallel import DeviceShard
+            self.device, self.engine = devs[0], None
+            self.shards = [DeviceShard(sd, frags, pm, r, len(devs), _device_index(d), native_comm=False,
+                                       chunk_atoms=int(chunk_size or 0)) for r, d in enumerate(devs)]
+            for sh in self.shards:
+                sh.set_window(frags, pm, recipe, caph=caph, nonbonded=nonbonded)
+            self.group = EngineGroup([sh.engine for sh in self.shards])
+            self._target = self.group
+            return
+        self.device = device
         self.engine = eng = Engine(sd, _device_index(device), chunk_atoms=int(chunk_size or 0))
         eng.set_topology(frags.z, frags.batch, n_graphs=len(frags))
         eng.set_protein_map(pm.n_protein, pm.src_atom, pm.dst_atom, pm.sign, pm.frag_sign)
@@ -275,14 +341,16 @@ class FragmentCalculator(_CalculatorBase):
             eng.set_caph(caph)
         if nonbonded is not None:
             eng.set_nonbonded(*nonbonded, *excl)
+        self._target = eng
 
     @classmethod
     def from_protein(cls, ckpt_path: str, ckpt_type: str, prot, caph_tables=None, nonbonded=None, nbcalc_type: str = "mm",
-                     device: str = "cuda:0", chunk_size: Optional[int] = None, **kwargs):
+                     device: str = "cuda:0", chunk_size: Optional[int] = None, devices=None, **kwargs):
         """From a :class:`ai2bmd_b200.pdbfrag.CappedProtein`: fragmentation, protein map and recipe
         (``fragment_protein``), and with ``caph_tables`` (the per-dipeptide prmtop tables of
-        :func:`ai2bmd_b200.caph.build_problem`) the hydrogen refinement."""
+        :func:`ai2bmd_b200.caph.build_problem`) the hydrogen refinement; ``devices`` as in the constructor."""
         _check_nbcalc_type(nbcalc_type)
+        _device_list(devices)
         from .pdbfrag import fragment_protein
         frags, pm, recipe = fragment_protein(prot, with_recipe=True)
         caph = None
@@ -290,9 +358,9 @@ class FragmentCalculator(_CalculatorBase):
             from .caph import build_problem
             caph = build_problem(prot, frags, recipe, caph_tables)
         return cls(ckpt_path, ckpt_type, frags, pm, recipe, caph=caph, nonbonded=nonbonded, nbcalc_type=nbcalc_type,
-                   device=device, chunk_size=chunk_size, **kwargs)
+                   device=device, chunk_size=chunk_size, devices=devices, **kwargs)
 
     def calculate(self, atoms, properties=("energy", "forces"), system_changes=("positions",)):
-        energy, forces = self.engine.forward_fragments_host(atoms.positions)
+        energy, forces = self._target.forward_fragments_host(atoms.positions)
         self.results = {"energy": energy, "forces": forces}
         return forces

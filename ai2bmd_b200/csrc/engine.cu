@@ -259,9 +259,14 @@ struct vb_handle {
         va_end(ap);
         err = buf;
     }
+    // configuration generation: every call that drops the cached graphs (a topology, window, map, recipe, refinement, MM
+    // term, MD or comm setup, any option) changes what an evaluation computes, so a group (vb_group_*) that checked this
+    // handle at vb_group_create compares it before every call
+    unsigned long long gen = 0;
     void drop_graph() {
         for (auto& g : graphs) cudaGraphExecDestroy(g.exec);
         graphs.clear();
+        gen++;
     }
     void free_map() {
         cudaFree(d_map_rowptr); cudaFree(d_map_src); cudaFree(d_map_sign); cudaFree(d_frag_sign); cudaFree(d_ef);
@@ -2282,6 +2287,15 @@ int fragments_check(vb_handle* h, const char* who) {
     if (int rc = need_derivative(h, who)) return rc;
     return comm_check(h, who);
 }
+// the positions buffer and pinned staging of vb_forward_fragments_host, allocated at its first use and kept with the map
+int fragments_staging(vb_handle* h) {
+    if (h->d_fx) return VB_OK;
+    const size_t n3 = 3 * (size_t)h->n_protein;
+    CUDA_TRY(h, cudaMalloc(&h->d_fx, sizeof(double) * n3));
+    CUDA_TRY(h, cudaMallocHost(&h->h_fx, sizeof(double) * n3));
+    CUDA_TRY(h, cudaMallocHost(&h->h_fef, sizeof(float) * (n3 + 1)));
+    return VB_OK;
+}
 }  // namespace
 
 int vb_forward_fragments(vb_handle* h, const double* prot_pos_dev, float* ef_prot_dev, void* stream) {
@@ -2309,11 +2323,7 @@ int vb_forward_fragments_host(vb_handle* h, const double* prot_pos_host, float* 
     // MD steps enqueued on the caller's stream (vb_md_run, vb_md_run_loop, ...) may still be running, and they use the
     // same workspace; own_stream is non-blocking, so nothing orders the replay after them but this wait
     if (h->md_ready) CUDA_TRY(h, cudaDeviceSynchronize());
-    if (!h->d_fx) {                  // staging of the first call, kept with the protein map
-        CUDA_TRY(h, cudaMalloc(&h->d_fx, sizeof(double) * n3));
-        CUDA_TRY(h, cudaMallocHost(&h->h_fx, sizeof(double) * n3));
-        CUDA_TRY(h, cudaMallocHost(&h->h_fef, sizeof(float) * (n3 + 1)));
-    }
+    if (int r = fragments_staging(h)) return r;
     memcpy(h->h_fx, prot_pos_host, sizeof(double) * n3);
     // H2D of the positions, every launch of vb_forward_fragments, D2H of forces and energy: one graph replay
     StepIO io = eval_io(h, h->d_ef);
@@ -2328,6 +2338,319 @@ int vb_forward_fragments_host(vb_handle* h, const double* prot_pos_host, float* 
     CUDA_TRY(h, cudaStreamSynchronize(st));
     if (int r = check_edge_overflow(h, "vb_forward_fragments_host")) return r;
     memcpy(ef_prot_host, h->h_fef, sizeof(float) * (n3 + 1));
+    return VB_OK;
+}
+
+// ---- an in-process group of window handles: one FragmentCalculator call over several GPUs of one process ---------------
+// Every member places and refines the whole batch and evaluates its own window into its own partial buffer (its d_ef, on
+// its device), as a rank of the one-process-per-GPU path does; the leader (member 0) then sums the partials in rank order
+// with comm_allreduce_kernel's gather mode.  Members run their cached K_FRAG graphs on their own streams, joined to the
+// leader's stream by events: no flags, no spin waits, no host synchronisation between them.
+struct vb_group {
+    std::vector<vb_handle*> m;               // members in rank order; m[0] leads
+    std::vector<int> dev;                    // their devices (kept for vb_group_destroy, which must not touch members)
+    std::vector<unsigned long long> gen;     // each member's configuration generation at vb_group_create
+    std::vector<char> peer;                  // member r's partial is read in place on dev[0] (same device or peer access)
+    std::vector<cudaEvent_t> done;           // per member, on its device: its partial is complete
+    std::string err;
+    std::mutex mu;
+    int n_protein = 0;
+    float* d_stage = nullptr;                // [k][3n+1] on dev[0]: copies of the partials the leader cannot read in place
+    float* d_ef = nullptr;                   // [3n+1] on dev[0]: the host entry's result
+    double* h_x = nullptr;                   // [3n] pinned, portable: the host entry's positions, copied to every member
+    float* h_ef = nullptr;                   // [3n+1] pinned: the host entry's result
+    cudaStream_t st = nullptr;               // dev[0]: the host entry's leader stream
+    cudaEvent_t ev_start = nullptr;          // dev[0]: the call's positions are ready
+    cudaEvent_t ev_join = nullptr;           // dev[0]: the last join has read the partials
+    CommParams join{};                       // comm_allreduce_kernel in gather mode over the partials
+    void set_error(const char* fmt, ...) {
+        char buf[1024];
+        va_list ap;
+        va_start(ap, fmt);
+        vsnprintf(buf, sizeof(buf), fmt, ap);
+        va_end(ap);
+        err = buf;
+    }
+};
+
+namespace {
+std::string g_group_create_error;
+
+// the calling thread's current device, restored when the entry returns
+struct DeviceRestore {
+    int dev = -1;
+    DeviceRestore() { if (cudaGetDevice(&dev) != cudaSuccess) { dev = -1; (void)cudaGetLastError(); } }
+    ~DeviceRestore() { if (dev >= 0) cudaSetDevice(dev); }
+};
+
+// the member mutexes, taken in rank order
+std::vector<std::unique_lock<std::mutex>> lock_members(vb_handle* const* m, int k) {
+    std::vector<std::unique_lock<std::mutex>> locks;
+    locks.reserve(k);
+    for (int r = 0; r < k; r++) locks.emplace_back(m[r]->mu);
+    return locks;
+}
+
+// a member's failure, named, as the group's error
+int member_fail(vb_group* g, int r, int rc) {
+    g->set_error("member %d: %s", r, g->m[r]->err.c_str());
+    return rc;
+}
+
+// vb_group_create's checks of the members, with their mutexes held; 0 or a status with the message in `err`
+int group_check_members(vb_handle* const* m, int k, std::string& err) {
+    char buf[512];
+    auto fail = [&](int rc, const char* fmt, auto... a) { snprintf(buf, sizeof(buf), fmt, a...); err = buf; return rc; };
+    for (int r = 0; r < k; r++) {
+        const vb_handle* h = m[r];
+        if (!h->derivative) return fail(VB_ERR_STATE, "vb_group_create: member %d has option derivative = 0 (no forces)", r);
+        if (h->md_unfrag) return fail(VB_ERR_STATE, "vb_group_create: member %d is set up un-fragmented (vb_md_setup with real_host = NULL)", r);
+        if (!h->has_topology || h->n_protein <= 0 || !h->d_map_rowptr)
+            return fail(VB_ERR_STATE, "vb_group_create: member %d has no topology or protein map", r);
+        if (!h->d_real) return fail(VB_ERR_STATE, "vb_group_create: member %d has no placement recipe (vb_set_fragment_recipe)", r);
+        if (h->comm_ready)
+            return fail(VB_ERR_STATE, "vb_group_create: member %d is connected through vb_comm_connect; a group joins its members itself", r);
+    }
+    const int P = m[0]->n_protein, B = m[0]->batch_atoms();
+    for (int r = 1; r < k; r++) {
+        if (m[r]->n_protein != P)
+            return fail(VB_ERR_ARG, "vb_group_create: member %d has %d protein atoms, member 0 has %d", r, m[r]->n_protein, P);
+        if (m[r]->batch_atoms() != B)
+            return fail(VB_ERR_ARG, "vb_group_create: member %d has a batch of %d atoms, member 0 one of %d", r, m[r]->batch_atoms(), B);
+    }
+    long long next = 0;                     // the windows [first, first + N) tile the batch in rank order
+    for (int r = 0; r < k; r++) {
+        if (m[r]->win_first != next)
+            return fail(VB_ERR_ARG, "vb_group_create: member %d's window starts at batch atom %lld, not at %lld: the windows must "
+                        "tile the batch contiguously in rank order", r, (long long)m[r]->win_first, next);
+        next += m[r]->ws.N;
+    }
+    if (next != B)
+        return fail(VB_ERR_ARG, "vb_group_create: member %d's window ends at batch atom %lld, and the batch has %d atoms", k - 1, next, B);
+    int with_mm = 0;                        // the MM rows: unset everywhere, or a tiling of [0, n_protein) in rank order
+    for (int r = 0; r < k; r++) with_mm += m[r]->nb_ready ? 1 : 0;
+    if (with_mm == 0) return VB_OK;
+    int lo = 0;
+    for (int r = 0; r < k; r++) {
+        if (!m[r]->nb_ready)
+            return fail(VB_ERR_ARG, "vb_group_create: member %d has no MM rows (vb_set_nonbonded) while other members have", r);
+        if (m[r]->nb.lo != lo || m[r]->nb.hi < lo)
+            return fail(VB_ERR_ARG, "vb_group_create: member %d's MM rows [%d, %d) do not start at row %d: they must tile "
+                        "[0, %d) in rank order", r, m[r]->nb.lo, m[r]->nb.hi, lo, P);
+        lo = m[r]->nb.hi;
+    }
+    if (lo != P)
+        return fail(VB_ERR_ARG, "vb_group_create: member %d's MM rows end at row %d, and the protein has %d atoms", k - 1, lo, P);
+    return VB_OK;
+}
+
+// every member as vb_group_create found it, and ready for the call
+int group_check_call(vb_group* g, const char* who) {
+    for (int r = 0; r < (int)g->m.size(); r++) {
+        vb_handle* h = g->m[r];
+        if (h->gen != g->gen[r]) {
+            g->set_error("%s: member %d was reconfigured after vb_group_create (topology, window, map, recipe, refinement, MM "
+                         "term, MD or comm setup, or an option); create the group again", who, r);
+            return VB_ERR_STATE;
+        }
+        if (int rc = fragments_check(h, who)) return member_fail(g, r, rc);
+    }
+    return VB_OK;
+}
+
+// members with an MD step set up may have MD work running on any stream, over the workspace the call uses: wait for it,
+// as vb_forward_fragments_host does
+int group_md_sync(vb_group* g, const char* who) {
+    for (int r = 0; r < (int)g->m.size(); r++) {
+        if (!g->m[r]->md_ready) continue;
+        const cudaError_t e = cudaSetDevice(g->dev[r]) == cudaSuccess ? cudaDeviceSynchronize() : cudaGetLastError();
+        if (e != cudaSuccess) { g->set_error("%s: member %d: %s", who, r, cudaGetErrorString(e)); return VB_ERR_CUDA; }
+    }
+    return VB_OK;
+}
+
+// One group call enqueued, members locked: positions to every member (host_x: from pinned host memory; else dev_x on
+// dev[0], read in place by the members there and copied peer-to-peer to the others), each member's evaluation into its
+// partial on its own stream, then, on `leader` (dev[0]), the wait for every member and the rank-order join into ef.
+int group_enqueue(vb_group* g, const double* host_x, const double* dev_x, float* ef, cudaStream_t leader) {
+    const int k = (int)g->m.size();
+    const size_t n3 = 3 * (size_t)g->n_protein;
+    vb_handle* h0 = g->m[0];
+    CUDA_TRY(h0, cudaSetDevice(g->dev[0]));
+    CUDA_TRY(h0, cudaStreamWaitEvent(leader, g->ev_join, 0));   // the last join, on whichever stream, has read the partials
+    CUDA_TRY(h0, cudaEventRecord(g->ev_start, leader));
+    for (int r = 0; r < k; r++) {
+        vb_handle* h = g->m[r];
+        const cudaStream_t s = h->own_stream;
+        int rc = VB_OK;
+        auto member = [&]() -> int {
+            CUDA_TRY(h, cudaSetDevice(h->device));
+            CUDA_TRY(h, cudaStreamWaitEvent(s, g->ev_start, 0));
+            const double* x = h->d_fx;
+            if (host_x) CUDA_TRY(h, cudaMemcpyAsync(h->d_fx, host_x, sizeof(double) * n3, cudaMemcpyHostToDevice, s));
+            else if (h->device == g->dev[0]) x = dev_x;
+            else CUDA_TRY(h, cudaMemcpyPeerAsync(h->d_fx, h->device, dev_x, g->dev[0], sizeof(double) * n3, s));
+            StepIO io = eval_io(h, h->d_ef);
+            io.x = x;
+            if (int r2 = run_cached(h, s, K_FRAG, io, [&](cudaStream_t q) -> int { return md_eval_enqueue(h, q, x, h->d_ef, false); }))
+                return r2;
+            CUDA_TRY(h, cudaEventRecord(g->done[r], s));
+            return VB_OK;
+        };
+        if ((rc = member())) return member_fail(g, r, rc);
+    }
+    CUDA_TRY(h0, cudaSetDevice(g->dev[0]));
+    for (int r = 0; r < k; r++) {
+        CUDA_TRY(h0, cudaStreamWaitEvent(leader, g->done[r], 0));
+        if (!g->peer[r])
+            CUDA_TRY(h0, cudaMemcpyPeerAsync(g->d_stage + r * (n3 + 1), g->dev[0], g->m[r]->d_ef, g->dev[r], sizeof(float) * (n3 + 1), leader));
+    }
+    const long long n = (long long)n3 + 1;
+    const int ctas = (int)std::max<long long>(1, std::min<long long>((n + COMM_THREADS - 1) / COMM_THREADS, COMM_MAX_CTAS));
+    comm_allreduce_kernel<<<ctas, COMM_THREADS, 0, leader>>>(g->join, ef, n);
+    CUDA_TRY(h0, cudaGetLastError());
+    CUDA_TRY(h0, cudaEventRecord(g->ev_join, leader));
+    return VB_OK;
+}
+}  // namespace
+
+const char* vb_group_last_error(const vb_group* g) { return g ? g->err.c_str() : g_group_create_error.c_str(); }
+
+void vb_group_destroy(vb_group* g) {
+    if (!g) return;
+    DeviceRestore restore;
+    {
+        std::lock_guard<std::mutex> lk(g->mu);
+        if (!g->dev.empty() && cudaSetDevice(g->dev[0]) == cudaSuccess) {
+            if (g->ev_join) cudaEventSynchronize(g->ev_join);     // a device-entry join may still read the staging
+            if (g->st) cudaStreamSynchronize(g->st);
+            cudaFree(g->d_stage); cudaFree(g->d_ef);
+            cudaFreeHost(g->h_x); cudaFreeHost(g->h_ef);
+            if (g->st) cudaStreamDestroy(g->st);
+            if (g->ev_start) cudaEventDestroy(g->ev_start);
+            if (g->ev_join) cudaEventDestroy(g->ev_join);
+        }
+        for (size_t r = 0; r < g->done.size(); r++)
+            if (g->done[r] && cudaSetDevice(g->dev[r]) == cudaSuccess) cudaEventDestroy(g->done[r]);
+        (void)cudaGetLastError();
+    }
+    delete g;
+}
+
+int vb_group_create(vb_handle* const* members, int n_members, vb_group** out) {
+    NvtxRange nvtx_("vb_group_create");
+    if (!out) { g_group_create_error = "vb_group_create: null output pointer"; return VB_ERR_ARG; }
+    *out = nullptr;
+    if (!members || n_members < 1 || n_members > COMM_MAX_WORLD) {
+        g_group_create_error = "vb_group_create: a group has 1 to " + std::to_string(COMM_MAX_WORLD) + " members";
+        return VB_ERR_ARG;
+    }
+    for (int r = 0; r < n_members; r++) {
+        if (!members[r]) { g_group_create_error = "vb_group_create: member " + std::to_string(r) + " is null"; return VB_ERR_ARG; }
+        for (int q = 0; q < r; q++)
+            if (members[q] == members[r]) {
+                g_group_create_error = "vb_group_create: member " + std::to_string(r) + " is the handle of member " + std::to_string(q);
+                return VB_ERR_ARG;
+            }
+    }
+    DeviceRestore restore;
+    auto locks = lock_members(members, n_members);
+    std::string err;
+    if (int rc = group_check_members(members, n_members, err)) { g_group_create_error = err; return rc; }
+    vb_group* g = new vb_group();
+    auto fail = [&](int rc) { g_group_create_error = g->err; locks.clear(); vb_group_destroy(g); return rc; };
+    g->n_protein = members[0]->n_protein;
+    const size_t n3 = 3 * (size_t)g->n_protein;
+    for (int r = 0; r < n_members; r++) {
+        vb_handle* h = members[r];
+        g->m.push_back(h);
+        g->dev.push_back(h->device);
+        g->done.push_back(nullptr);
+        if (cudaSetDevice(h->device) != cudaSuccess) { g->set_error("vb_group_create: member %d: cudaSetDevice failed", r); return fail(VB_ERR_CUDA); }
+        if (int rc = fragments_staging(h)) { member_fail(g, r, rc); return fail(rc); }
+        if (cudaEventCreateWithFlags(&g->done[r], cudaEventDisableTiming) != cudaSuccess) {
+            g->set_error("vb_group_create: member %d: event creation failed", r);
+            return fail(VB_ERR_CUDA);
+        }
+    }
+    const int d0 = g->dev[0];
+    if (cudaSetDevice(d0) != cudaSuccess ||
+        cudaStreamCreateWithFlags(&g->st, cudaStreamNonBlocking) != cudaSuccess ||
+        cudaEventCreateWithFlags(&g->ev_start, cudaEventDisableTiming) != cudaSuccess ||
+        cudaEventCreateWithFlags(&g->ev_join, cudaEventDisableTiming) != cudaSuccess ||
+        cudaMalloc(&g->d_ef, sizeof(float) * (n3 + 1)) != cudaSuccess ||
+        cudaHostAlloc(&g->h_x, sizeof(double) * n3, cudaHostAllocPortable) != cudaSuccess ||
+        cudaHostAlloc(&g->h_ef, sizeof(float) * (n3 + 1), cudaHostAllocPortable) != cudaSuccess) {
+        g->set_error("vb_group_create: leader resources on device %d: %s", d0, cudaGetErrorString(cudaGetLastError()));
+        return fail(VB_ERR_ALLOC);
+    }
+    // peer access from the leader's device to every other member device; where there is none, the leader copies that
+    // partial into its staging first (cudaMemcpyPeerAsync goes through the host) and sums local rows
+    bool staging = false;
+    for (int r = 0; r < n_members; r++) {
+        int can = 0;
+        bool ok = g->dev[r] == d0;
+        if (!ok && cudaDeviceCanAccessPeer(&can, d0, g->dev[r]) == cudaSuccess && can) {
+            const cudaError_t e = cudaDeviceEnablePeerAccess(g->dev[r], 0);
+            ok = e == cudaSuccess || e == cudaErrorPeerAccessAlreadyEnabled;
+        }
+        (void)cudaGetLastError();
+        g->peer.push_back(ok ? 1 : 0);
+        staging = staging || !ok;
+    }
+    if (staging && cudaMalloc(&g->d_stage, sizeof(float) * (n3 + 1) * n_members) != cudaSuccess) {
+        g->set_error("vb_group_create: staging of %d partials on device %d: allocation failed", n_members, d0);
+        return fail(VB_ERR_ALLOC);
+    }
+    g->join.world = n_members;
+    g->join.gather = 1;
+    for (int r = 0; r < n_members; r++) g->join.slots[r] = g->peer[r] ? g->m[r]->d_ef : g->d_stage + r * (n3 + 1);
+    for (int r = 0; r < n_members; r++) g->gen.push_back(members[r]->gen);
+    *out = g;
+    return VB_OK;
+}
+
+int vb_group_forward_fragments(vb_group* g, const double* prot_pos_dev, float* ef_prot_dev, void* stream) {
+    NvtxRange nvtx_("vb_group_forward_fragments");
+    if (!g) return VB_ERR_ARG;
+    std::lock_guard<std::mutex> lk(g->mu);
+    if (!prot_pos_dev || !ef_prot_dev) { g->set_error("vb_group_forward_fragments: null buffer"); return VB_ERR_ARG; }
+    DeviceRestore restore;
+    auto locks = lock_members(g->m.data(), (int)g->m.size());
+    const char* who = "vb_group_forward_fragments";
+    if (int rc = group_check_call(g, who)) return rc;
+    if (int rc = group_md_sync(g, who)) return rc;
+    if (int rc = group_enqueue(g, nullptr, prot_pos_dev, ef_prot_dev, (cudaStream_t)stream)) return rc;
+    return VB_OK;
+}
+
+int vb_group_forward_fragments_host(vb_group* g, const double* prot_pos_host, float* ef_prot_host) {
+    NvtxRange nvtx_("vb_group_forward_fragments_host");
+    if (!g) return VB_ERR_ARG;
+    std::lock_guard<std::mutex> lk(g->mu);
+    if (!prot_pos_host || !ef_prot_host) { g->set_error("vb_group_forward_fragments_host: null buffer"); return VB_ERR_ARG; }
+    DeviceRestore restore;
+    auto locks = lock_members(g->m.data(), (int)g->m.size());
+    const char* who = "vb_group_forward_fragments_host";
+    if (int rc = group_check_call(g, who)) return rc;
+    if (int rc = group_md_sync(g, who)) return rc;
+    const size_t n3 = 3 * (size_t)g->n_protein;
+    memcpy(g->h_x, prot_pos_host, sizeof(double) * n3);
+    if (int rc = group_enqueue(g, g->h_x, nullptr, g->d_ef, g->st)) return rc;
+    vb_handle* h0 = g->m[0];
+    auto finish = [&]() -> int {
+        CUDA_TRY(h0, cudaSetDevice(g->dev[0]));
+        CUDA_TRY(h0, cudaMemcpyAsync(g->h_ef, g->d_ef, sizeof(float) * (n3 + 1), cudaMemcpyDeviceToHost, g->st));
+        CUDA_TRY(h0, cudaStreamSynchronize(g->st));
+        return VB_OK;
+    };
+    if (int rc = finish()) return member_fail(g, 0, rc);
+    for (int r = 0; r < (int)g->m.size(); r++) {
+        vb_handle* h = g->m[r];
+        if (cudaSetDevice(h->device) != cudaSuccess) { g->set_error("%s: member %d: cudaSetDevice failed", who, r); return VB_ERR_CUDA; }
+        if (int rc = check_edge_overflow(h, who)) return member_fail(g, r, rc);
+    }
+    memcpy(ef_prot_host, g->h_ef, sizeof(float) * (n3 + 1));
     return VB_OK;
 }
 
@@ -2905,8 +3228,8 @@ int64_t vb_debug_read(vb_handle* h, const char* name, int layer, void* host_dst,
     const void* src = nullptr;
     size_t bytes = 0;
     const std::string k(name);
-    if (!h->chunks.empty() && k != "energy" && k != "forces" && k != "pos" && k != "RF") {
-        h->set_error("vb_debug_read: %s holds only the last chunk of a chunked handle; energy, forces, pos and RF span the batch", name);
+    if (!h->chunks.empty() && k != "energy" && k != "forces" && k != "pos" && k != "RF" && k != "ef") {
+        h->set_error("vb_debug_read: %s holds only the last chunk of a chunked handle; energy, forces, pos, RF and ef span the batch", name);
         return VB_ERR_STATE;
     }
     if (!h->derivative) {
@@ -2960,6 +3283,7 @@ int64_t vb_debug_read(vb_handle* h, const char* name, int layer, void* host_dst,
     else BUF("forces", h->d_forces, N * 3, 4)
     else BUF("pos", h->batch_pos(), (size_t)h->batch_atoms() * 3, 4)
     else if (k == "RF" && h->rs_ready) { src = h->rs.rf; bytes = (3 * (size_t)h->n_protein + 1) * 8; }
+    else if (k == "ef" && h->d_ef) { src = h->d_ef; bytes = (3 * (size_t)h->n_protein + 1) * 4; }
 #undef BUF
     if (!src) { h->set_error("vb_debug_read: unknown buffer %s[%d]", name, layer); return VB_ERR_ARG; }
     if (overwritten) {

@@ -24,6 +24,12 @@
 // The deadline bounds the skew between ranks, host side included: one rank stalled for more than 10 s between steps
 // (I/O, a checkpoint) while its peers already wait in the next all-reduce also trips it.
 // The sum starts at +0.0f, so an element that is -0.0 on every rank comes out as +0.0 (also with world = 1).
+//
+// With `gather` set the kernel is the join of an in-process group of handles (vb_group_*): one launch on the leader
+// device, ordered after every member's evaluation by stream events, runs step 4 alone over slots[0 .. world), each the
+// base of one member's complete [n] buffer (a peer pointer, a local one, or a row of a leader staging copy).  No push,
+// no flags, no wait; the same rank-order sum from +0.0f, so a group's result is bit-identical to what the one-process-
+// per-GPU path sums for the same partials.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -42,6 +48,7 @@ struct CommParams {
     int* flags[COMM_MAX_WORLD];           // flags[r]: base of rank r's flag array [2][world]
     unsigned int* counters;               // local: [0] CTAs done pushing, [1] CTAs done summing, [2] sequence number,
                                           //        [3] flag waits that ran past COMM_WAIT_NS
+    int gather;                           // 1: the group join -- buf[i] = sum over r of slots[r][i], nothing else
 };
 
 __device__ __forceinline__ unsigned long long globaltimer_ns() {
@@ -65,6 +72,14 @@ __device__ __forceinline__ float ld_relaxed_sys(const float* p) {
 }
 
 __global__ void __launch_bounds__(COMM_THREADS) comm_allreduce_kernel(CommParams c, float* __restrict__ buf, long long n) {
+    if (c.gather) {         // step 4 alone over complete member buffers (stream-ordered: plain loads)
+        for (long long i = (long long)blockIdx.x * COMM_THREADS + threadIdx.x; i < n; i += (long long)gridDim.x * COMM_THREADS) {
+            float s = 0.f;
+            for (int r = 0; r < c.world; r++) s += c.slots[r][i];
+            buf[i] = s;
+        }
+        return;
+    }
     __shared__ unsigned int s_seq, s_broken;
     __shared__ int s_last;
     const int rank = c.rank, world = c.world;

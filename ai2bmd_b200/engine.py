@@ -46,6 +46,8 @@ EXPORTED_SYMBOLS = [
     "vb_comm_init", "vb_comm_connect", "vb_comm_allreduce",
     "vb_set_caph", "vb_caph_relax", "vb_chunk_fragments",
     "vb_set_fragment_recipe", "vb_forward_fragments", "vb_forward_fragments_host", "vb_set_batch_window",
+    "vb_group_create", "vb_group_destroy", "vb_group_last_error", "vb_group_forward_fragments",
+    "vb_group_forward_fragments_host",
 ]
 
 
@@ -161,6 +163,16 @@ def load_library(path: Optional[str] = None):
     lib.vb_forward_fragments_host.argtypes = [vp, vp, vp]
     lib.vb_set_batch_window.restype = C.c_int
     lib.vb_set_batch_window.argtypes = [vp, i64, i64]
+    lib.vb_group_create.restype = C.c_int
+    lib.vb_group_create.argtypes = [vp, C.c_int, C.POINTER(vp)]
+    lib.vb_group_destroy.restype = None
+    lib.vb_group_destroy.argtypes = [vp]
+    lib.vb_group_last_error.restype = C.c_char_p
+    lib.vb_group_last_error.argtypes = [vp]
+    lib.vb_group_forward_fragments.restype = C.c_int
+    lib.vb_group_forward_fragments.argtypes = [vp, vp, vp, vp]
+    lib.vb_group_forward_fragments_host.restype = C.c_int
+    lib.vb_group_forward_fragments_host.argtypes = [vp, vp, vp]
     if path == _build.LIB_PATH:
         _lib = lib
     return lib
@@ -599,6 +611,62 @@ class Engine:
         if n != out.nbytes:
             raise RuntimeError(f"vb_debug_read({name}): got {n} bytes, wanted {out.nbytes}")
         return out
+
+
+class EngineGroup:
+    """Window engines of one process as ONE fragment calculator call over their devices (``vb_group_*``): every member
+    places and refines the whole batch, evaluates its own block into its own partial buffer, and member 0 sums the
+    partials in rank order on its device.  ``engines``: in rank order, each set up as a rank of the sharded path
+    (:meth:`ai2bmd_b200.parallel.DeviceShard.set_window`).  The group keeps them alive; reconfiguring one of them makes
+    every later call raise -- build the group again."""
+
+    def __init__(self, engines):
+        self.engines = list(engines)
+        self.lib = load_library()
+        arr = (C.c_void_p * len(self.engines))(*[e.h for e in self.engines])
+        handle = C.c_void_p()
+        rc = self.lib.vb_group_create(arr, len(self.engines), C.byref(handle))
+        if rc != 0:
+            raise RuntimeError(f"vb_group_create failed ({rc}): {self.lib.vb_group_last_error(None).decode()}")
+        self.g = handle
+        self.n_protein = self.engines[0].n_protein
+        self.device = self.engines[0].device
+
+    def last_error(self) -> str:
+        return self.lib.vb_group_last_error(self.g).decode()
+
+    def _check(self, rc, what):
+        if rc < 0:
+            raise RuntimeError(f"{what} failed ({rc}): {self.last_error()}")
+        return rc
+
+    def close(self):
+        if getattr(self, "g", None):
+            self.lib.vb_group_destroy(self.g)
+            self.g = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def forward_fragments_host(self, prot_pos: np.ndarray) -> Tuple[float, np.ndarray]:
+        """Protein positions [n_protein, 3] (A) in, (energy [eV], forces [n_protein, 3] float32 eV/A) out, synchronous;
+        the values :meth:`Engine.forward_fragments_host` computes on one engine of the whole batch."""
+        x = np.ascontiguousarray(prot_pos, dtype=np.float64)
+        if x.shape != (self.n_protein, 3):
+            raise ValueError(f"prot_pos must be [{self.n_protein},3]")
+        ef = np.empty(3 * self.n_protein + 1, dtype=np.float32)
+        rc = self.lib.vb_group_forward_fragments_host(self.g, x.__array_interface__["data"][0], ef.__array_interface__["data"][0])
+        if rc < 0:
+            self._check(rc, "vb_group_forward_fragments_host")
+        return float(ef[-1]), ef[:-1].reshape(-1, 3)
+
+    def forward_fragments_device(self, prot_pos_ptr: int, ef_ptr: int, stream_ptr: int = 0):
+        """Raw device pointers on member 0's device: fp64 protein positions [n_protein, 3] -> ef [3 n_protein + 1];
+        asynchronous on ``stream_ptr`` (a stream of member 0's device)."""
+        self._check(self.lib.vb_group_forward_fragments(self.g, prot_pos_ptr, ef_ptr, stream_ptr), "vb_group_forward_fragments")
 
 
 def tc_selftest(a: np.ndarray, w_nk: np.ndarray, reps: int = 1, device: int = 0, rows: int = 128):

@@ -347,6 +347,43 @@ int vb_forward_fragments_host(vb_handle* h, const double* prot_pos_host, float* 
  * and "batch_first_atom".  Synchronises. */
 int vb_set_batch_window(vb_handle* h, int64_t n_batch_atoms, int64_t first_atom);
 
+/* ---- A group of window handles in one process: one FragmentCalculator call over several GPUs -------------------------
+ * The reference's single-process run spreads the fragments of every calculator call over all bonded devices, one model
+ * per device from a thread pool, and joins the results on the host (DLBondedCalculator.calculate, src/Calculators/
+ * bonded.py:64-89, behind AsyncQMMM's qmcalc, src/Calculators/qmmm.py:48-83).  A group does that on the device, with no
+ * other process: each member is set up as one rank of the sharded path (the topology and shard protein map of its block of
+ * the fragment partition, vb_set_batch_window, the whole recipe and refinement problem, its MM rows), and one group call
+ * runs what vb_forward_fragments runs on every member, each into its own partial [3*n_protein + 1] (the member's internal
+ * buffer, vb_debug_read "ef"), then sums the partials on member 0's device in rank order from +0.0f: the arithmetic of the
+ * engine's all-reduce, so a group's result is bit-identical to what the one-process-per-GPU path sums for the same
+ * partials.  Members run their cached vb_forward_fragments graphs on their own streams; events order them after the
+ * call's positions and the join after every member: no host synchronisation between members and no spin wait, so members
+ * on one GPU run as well as members on several.  Member 0's device reads the other partials through peer access where
+ * cudaDeviceCanAccessPeer allows it (vb_group_create enables it), else copies them into a staging buffer of its own first.
+ *
+ * vb_group_create: members in rank order (member 0 leads), 1 to 16 of them; they are not copied, and the group must be
+ * destroyed before any of them.  VB_ERR_ARG, with a message naming the member (vb_group_last_error(NULL)): a null member,
+ * a member given twice, n_protein or the batch size differing from member 0's, windows [batch_first_atom, + N) that do not
+ * tile the batch contiguously in rank order, MM rows (vb_set_nonbonded's [atom_lo, atom_hi)) set on some members only or
+ * not tiling [0, n_protein) in rank order.  VB_ERR_STATE: a member with derivative = 0, un-fragmented, without a topology,
+ * protein map or recipe, or connected through vb_comm_connect.  Any later call on a member that drops its cached graphs (a
+ * topology, window, map, recipe, refinement, MM term, MD or comm setup, any vb_set_option) makes every later group call
+ * fail with VB_ERR_STATE: create the group again.
+ * A group call takes the member mutexes in rank order, may come from any host thread and restores the caller's current
+ * device.  It uses each member's workspace: a member with an MD step set up is synchronised first, as
+ * vb_forward_fragments_host does; other work of a member must be ordered before the call by its caller. */
+typedef struct vb_group vb_group;
+int vb_group_create(vb_handle* const* members, int n_members, vb_group** out);
+void vb_group_destroy(vb_group* g);                    /* waits for the group's work; does not destroy the members */
+const char* vb_group_last_error(const vb_group* g);    /* g may be NULL: the last vb_group_create error */
+/* prot_pos_dev[3*n_protein] (fp64) -> ef_prot_dev[3*n_protein + 1], both on member 0's device, asynchronous on `stream`
+ * (of member 0's device): the members wait for the work enqueued on `stream` so far, and the join is the last launch on
+ * it.  VB_ERR_ARG for a null buffer; a member refused by vb_forward_fragments' checks fails the call with its message. */
+int vb_group_forward_fragments(vb_group* g, const double* prot_pos_dev, float* ef_prot_dev, void* stream);
+/* The same with HOST buffers, synchronous: the positions go from one pinned staging buffer to every member; fails with
+ * VB_ERR_STATE, naming the member, when one produced more edges than its trimmed max_edges. */
+int vb_group_forward_fragments_host(vb_group* g, const double* prot_pos_host, float* ef_prot_host);
+
 /* ---- One-shot all-reduce over NVLink peer memory (SURVEY section 8e) ---------------------------------------------
  * One process per GPU.  vb_comm_init allocates this rank's window (2 parities x world slots of max_floats) and returns
  * its 64-byte CUDA IPC handle; the caller exchanges the handles of all ranks (any host transport: torch.distributed,
@@ -406,7 +443,9 @@ int vb_tc_selftest_rows(int device, int rows, const float* a_host, const float* 
  * "XA","VA","GX","GVEC","GF","GXA","GQKV","GVNMSG","GTU","geom","rbf","eacc","grbf","esrc","edst","rowptr",
  * "eatom","energy","forces","pos" (the packed fragment positions [N*3] the MD placement and hydrogen refinement write;
  * with vb_set_batch_window those of the whole batch),
- * and "RF" (fp64 restraint forces then energy [3*n_protein + 1], while restraints are set).
+ * "RF" (fp64 restraint forces then energy [3*n_protein + 1], while restraints are set), and "ef" (the internal
+ * [3*n_protein + 1] whole-protein buffer: the result of the last vb_forward_fragments_host, or the partial of the last
+ * group call; while a protein map is set).
  * Returns the number of bytes copied (<= cap_bytes) or a negative status. */
 int64_t vb_debug_read(vb_handle* h, const char* name, int layer, void* host_dst, int64_t cap_bytes);
 
