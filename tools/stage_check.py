@@ -12,6 +12,7 @@ one tile, one fragment or a few rows is not diluted by whichever fragment holds 
 Test infrastructure; not part of the product path.
 """
 import argparse
+import hashlib
 import os
 import sys
 
@@ -94,9 +95,17 @@ def energy_slot_layer(name, layer):
 _oracle_cache = {}
 
 
+def _geometry_key(z, pos, batch):
+    """Cache key of a geometry given as arrays: a hash of its atomic numbers, positions and fragment indices."""
+    h = hashlib.sha256()
+    for a in (z, pos, batch):
+        h.update(np.ascontiguousarray(a).tobytes())
+    return h.hexdigest()
+
+
 def _oracle(key, sd, z, pos, batch, ei):
-    """fp64 hand-adjoint tensors of one geometry; the last one is kept, so that runs of cases on one fixture (and one
-    case under several decoys) build it once."""
+    """fp64 hand-adjoint tensors of one geometry; the last one is kept, so that runs of cases on one geometry (one
+    case under several decoys, options or launch plans) build it once."""
     if key is not None and key in _oracle_cache:
         return _oracle_cache[key]
     adj = AdjointViSNet(O.OracleViSNet(sd, torch.float64))
@@ -109,31 +118,43 @@ def _oracle(key, sd, z, pos, batch, ei):
 
 
 def stage_report(frags="chig", weights="real", max_frags=0, opts="", calibrate=False, detail=None, decoy=None,
-                 derivative=True):
+                 derivative=True, calibrate_pos=None):
     """Run the evaluation one launch at a time and compare every buffer a stage produces with the fp64 hand-adjoint
     oracle.  Returns (lines, worst) where worst = [(stage, what, rel)] of the comparisons, rel relative to the largest
     reference entry of the buffer.
 
     frags: a fixture name (tests/golden/fragments_<name>.npz) or a (z, pos, batch) tuple.  opts: "key=value,..." for
     vb_set_option.  calibrate: evaluate once, then re-plan the edge tiles from the real edge count (the plan the host
-    entry points run).  detail: an optional dict, filled with "fragments" = [(stage, what, rel, fragment)] (the
-    per-fragment metric of every comparison, see fragment_rel), "kernels" = Engine.stage_kernels(), "options" (resolved
-    tile_rows, tc_rows, gxa_parts, node_tc, node_nb, edge_tc, npw), "n_edges", "n_atoms" and "max_degree"."""
+    entry points run).  calibrate_pos: positions [N, 3] of another geometry on the same topology (before the max_frags
+    selection, as the positions of frags); the edge tiles are then calibrated on that geometry instead, as a plan
+    calibrated earlier in a trajectory meets the geometry under test (implies calibrate).  detail: an optional dict,
+    filled with "fragments" = [(stage, what, rel, fragment)] (the per-fragment metric of every comparison, see
+    fragment_rel), "kernels" = Engine.stage_kernels(), "options" (resolved tile_rows, tc_rows, gxa_parts, node_tc,
+    node_nb, edge_tc, npw, and use_pdl / tile_rows / tc_rows again after the last evaluation, as "<key>_after"),
+    "n_edges", "n_atoms", "max_degree", and "host" = (energies, forces or None) of the last evaluation through the host
+    entry point."""
     if isinstance(frags, str):
         g = np.load(os.path.join(ROOT, "tests", "golden", f"fragments_{frags}.npz"))
         z, pos, batch = g["z"], g["pos"], g["batch"]
     else:
         z, pos, batch = (np.asarray(a) for a in frags)
         z, pos, batch = z.astype(np.int64), pos.astype(np.float32), batch.astype(np.int64)
+    if calibrate_pos is not None:
+        calibrate_pos = np.asarray(calibrate_pos, dtype=np.float32)
+        assert calibrate_pos.shape == pos.shape, "calibrate_pos must be a geometry of the same atoms"
+        calibrate = True
     if max_frags:
         keep = batch < max_frags
         z, pos, batch = z[keep], pos[keep], batch[keep]
+        if calibrate_pos is not None:
+            calibrate_pos = calibrate_pos[keep]
     sd = O.load_state_dict(os.path.join(ROOT, "tests", "golden", "weights_2ef43f29.npz")) if weights == "real" \
         else O.random_state_dict(int(weights) if str(weights).isdigit() else 0)
     slots, deg = O.radius_graph_canonical(pos, batch)
     ei = torch.from_numpy(O.slots_to_edge_index(slots, deg))
     E, N = ei.shape[1], len(z)
-    S, B = _oracle((frags, max_frags, str(weights)) if isinstance(frags, str) else None, sd, z, pos, batch, ei)
+    key = frags if isinstance(frags, str) else _geometry_key(z, pos, batch)
+    S, B = _oracle((key, max_frags, str(weights)), sd, z, pos, batch, ei)
 
     eng = Engine({k: v.numpy() for k, v in sd.items()}, 0, derivative=derivative)
     G = int(batch.max()) + 1
@@ -143,7 +164,7 @@ def stage_report(frags="chig", weights="real", max_frags=0, opts="", calibrate=F
         eng.set_option(k, int(v))
     host_eval = eng.forward_host if derivative else eng.energy_host
     if calibrate:
-        host_eval(pos)
+        host_eval(pos if calibrate_pos is None else calibrate_pos)
         eng.set_option("calibrate", 1)
     names = eng.stage_names()
     dpos = torch.from_numpy(pos).cuda()
@@ -292,9 +313,12 @@ def stage_report(frags="chig", weights="real", max_frags=0, opts="", calibrate=F
         report("forward_host", "E", e, S["E"][:, 0])
         report("forward_host", "forces", f, B["forces"])
     else:
-        report("energy_host", "E", eng.energy_host(pos), S["E"][:, 0])
+        e, f = eng.energy_host(pos), None
+        report("energy_host", "E", e, S["E"][:, 0])
     if detail is not None:
-        detail["options"]["use_pdl_after"] = eng.get_option("use_pdl")
+        for k in ("use_pdl", "tile_rows", "tc_rows"):
+            detail["options"][f"{k}_after"] = eng.get_option(k)
+        detail["host"] = (e, f)
     return lines, worst
 
 
