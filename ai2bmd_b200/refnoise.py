@@ -269,13 +269,17 @@ def normals_from_raw(raw, n: int, tab=None):
     return val[pos[:n]], last + int(cost[last])
 
 
-def window_normals(raw, n: int, tab=None, list_cap: int = WIN_LIST):
+def window_normals(raw, n: int, tab=None, list_cap: int = WIN_LIST, trace: list | None = None):
     """The device kernel's scheme (k_md.cuh ``md_refnoise_cta``) on the same stream: windows of ``window_size`` draws,
     each split into contiguous per-thread chunks that are classified independently; the non-fast positions of a window,
     in order, are walked (in runs between anchors on the device) to mark the draws consumed inside other attempts; a
     prefix count over the surviving attempts with a value numbers the normals.  A window holding more than ``list_cap``
     non-fast positions stops at the first it cannot hold, and a window that yields too few normals is followed by
-    another from where its attempts ended.  Returns (normals, draws consumed) -- equal to :func:`normals_from_raw`."""
+    another from where its attempts ended.  Returns (normals, draws consumed) -- equal to :func:`normals_from_raw`.
+
+    ``trace``, when given, gets one dict per window: ``start`` (its first draw in ``raw``), ``W``, ``T``, ``C``,
+    ``weff`` (where the window stops, relative to ``start``), ``cut`` (the list overflowed), ``rem`` (normals still
+    wanted), ``normals`` (how many of them it yielded) and ``end`` (the draw the next window or the step starts from)."""
     cost, val = attempts(raw, tab)
     out, base = [], 0
     while len(out) < n:
@@ -315,5 +319,8 @@ def window_normals(raw, n: int, tab=None, list_cap: int = WIN_LIST):
                         if got == rem - 1:
                             end = i + int(c[i])
                     got += 1
+        if trace is not None:
+            trace.append({"start": base, "W": W, "T": T, "C": C, "weff": weff, "cut": weff < W, "rem": rem,
+                          "normals": min(got, rem), "end": base + end})
         base += end
     return np.array(out), base
