@@ -8,7 +8,7 @@ Mirrors, name for name, the classes of ``/root/reference/src/Calculators`` that 
 * :class:`DipeptideBondedCombiner` <- ``combiner.py:11-41``
 * :class:`DLBondedCalculator` <- ``bonded.py:19-123`` (fragment-batch evaluation + combine)
 * :class:`FragmentCalculator` <- ``fragment.py:16-68`` (placement, hydrogen refinement, bonded + MM term in one device call,
-  on one GPU or, with ``devices``, on a group of them: ``bonded.py:64-89``)
+  on one GPU or, with ``devices``, on a group of them: ``bonded.py:64-89``; energies alone with ``derivative=False``)
 
 ASE is not a dependency: calculators expose ``calculate(atoms, ...)`` / ``get_potential_energy`` /
 ``get_forces`` with ASE semantics (results cached while positions are unchanged,
@@ -269,6 +269,11 @@ def _check_nbcalc_type(nbcalc_type: str):
         raise ValueError(f"nbcalc_type must be 'mm' or 'pme', not {nbcalc_type!r}")
 
 
+def _check_derivative(derivative):
+    if derivative is not None and not isinstance(derivative, (bool, np.bool_)):
+        raise TypeError(f"derivative must be None, True or False, not {derivative!r}")
+
+
 class FragmentCalculator(_CalculatorBase):
     """The reference's whole per-step calculator call (``FragmentCalculator.calculate``, ``src/Calculators/fragment.py:50-68``)
     as ONE engine call: protein positions in, the bonded (fragment) energy and forces plus the non-bonded MM term out,
@@ -294,13 +299,22 @@ class FragmentCalculator(_CalculatorBase):
     fragments, its rows of the MM term) and calibrated on the start geometry, joined by an
     :class:`ai2bmd_b200.engine.EngineGroup` that sums their buffers on the first device.  A list that leaves an entry
     without fragments is refused (:func:`ai2bmd_b200.parallel.check_shardable`).  None or one device is the
-    single-device path; ``calculate`` is the same either way."""
+    single-device path; ``calculate`` is the same either way.
+
+    ``derivative`` follows the reference's ``load_model(path, derivative=...)``: the checkpoint's hyper-parameter unless
+    given (an ``.npz`` counts as True).  With ``derivative=False`` the calculator serves ``get_potential_energy`` only
+    (``get_forces`` raises ``NotImplementedError``): every ``calculate`` runs the energy plan of the same call
+    (``vb_forward_fragments_energy_host``), whose energy equals the full call's bit for bit, for conformer ranking,
+    energy scans and Monte-Carlo acceptance tests.  On one device the engine is a forward-only one, with the smaller
+    workspace; with ``devices`` the group's window engines stay full ones (so the workspace is not reduced there) and
+    run the energy plan alone."""
 
     def __init__(self, ckpt_path: str, ckpt_type: str, frags: FragmentData, pm, recipe, caph=None, nonbonded=None,
                  nbcalc_type: str = "mm", device: str = "cuda:0", chunk_size: Optional[int] = None, devices=None,
-                 **kwargs):
+                 derivative: Optional[bool] = None, **kwargs):
         super().__init__()
         _check_nbcalc_type(nbcalc_type)
+        _check_derivative(derivative)
         from .engine import check_recipe
         real, acc, rem, blen = check_recipe(recipe.real, recipe.acc, recipe.rem, recipe.blen, len(frags.z))
         devs = _device_list(devices)
@@ -315,8 +329,9 @@ class FragmentCalculator(_CalculatorBase):
             excl = exclusion_table(pm.n_protein, dipeptide_atom_sets(frags, recipe, pm)) if devs is None else None
         model_path = osp.join(ckpt_path, f"visnet-uni-{ckpt_type}.ckpt") if ckpt_type else ckpt_path
         sd, ckpt_derivative = load_checkpoint(model_path)
-        if not resolve_derivative(ckpt_derivative, None):
-            raise ValueError(f"{model_path}: the fragment calculator needs forces, and the checkpoint has derivative=False")
+        self.derivative = resolve_derivative(ckpt_derivative, derivative)
+        if not self.derivative:
+            self.implemented_properties = ["energy"]
         self.n_protein = int(pm.n_protein)
         self.devices, self.shards, self.group = devs, None, None
         if devs is not None:
@@ -331,10 +346,14 @@ class FragmentCalculator(_CalculatorBase):
             self._target = self.group
             return
         self.device = device
-        self.engine = eng = Engine(sd, _device_index(device), chunk_atoms=int(chunk_size or 0))
+        self.engine = eng = Engine(sd, _device_index(device), derivative=self.derivative, chunk_atoms=int(chunk_size or 0))
         eng.set_topology(frags.z, frags.batch, n_graphs=len(frags))
         eng.set_protein_map(pm.n_protein, pm.src_atom, pm.dst_atom, pm.sign, pm.frag_sign)
-        eng.forward_host(np.asarray(frags.pos, dtype=np.float32))    # start geometry: real edge count for the tile plan
+        start = np.asarray(frags.pos, dtype=np.float32)             # start geometry: real edge count for the tile plan
+        if self.derivative:
+            eng.forward_host(start)
+        else:
+            eng.energy_host(start)
         eng.set_option("calibrate", 1)
         eng.set_fragment_recipe(real, acc, rem, blen)
         if caph is not None:
@@ -345,11 +364,14 @@ class FragmentCalculator(_CalculatorBase):
 
     @classmethod
     def from_protein(cls, ckpt_path: str, ckpt_type: str, prot, caph_tables=None, nonbonded=None, nbcalc_type: str = "mm",
-                     device: str = "cuda:0", chunk_size: Optional[int] = None, devices=None, **kwargs):
+                     device: str = "cuda:0", chunk_size: Optional[int] = None, devices=None,
+                     derivative: Optional[bool] = None, **kwargs):
         """From a :class:`ai2bmd_b200.pdbfrag.CappedProtein`: fragmentation, protein map and recipe
         (``fragment_protein``), and with ``caph_tables`` (the per-dipeptide prmtop tables of
-        :func:`ai2bmd_b200.caph.build_problem`) the hydrogen refinement; ``devices`` as in the constructor."""
+        :func:`ai2bmd_b200.caph.build_problem`) the hydrogen refinement; ``devices`` and ``derivative`` as in the
+        constructor."""
         _check_nbcalc_type(nbcalc_type)
+        _check_derivative(derivative)
         _device_list(devices)
         from .pdbfrag import fragment_protein
         frags, pm, recipe = fragment_protein(prot, with_recipe=True)
@@ -358,9 +380,12 @@ class FragmentCalculator(_CalculatorBase):
             from .caph import build_problem
             caph = build_problem(prot, frags, recipe, caph_tables)
         return cls(ckpt_path, ckpt_type, frags, pm, recipe, caph=caph, nonbonded=nonbonded, nbcalc_type=nbcalc_type,
-                   device=device, chunk_size=chunk_size, devices=devices, **kwargs)
+                   device=device, chunk_size=chunk_size, devices=devices, derivative=derivative, **kwargs)
 
     def calculate(self, atoms, properties=("energy", "forces"), system_changes=("positions",)):
+        if not self.derivative:
+            self.results = {"energy": self._target.forward_fragments_energy_host(atoms.positions)}
+            return None
         energy, forces = self._target.forward_fragments_host(atoms.positions)
         self.results = {"energy": energy, "forces": forces}
         return forces

@@ -123,8 +123,9 @@ struct StepIO {
     float* forces = nullptr;      // [N][3]
     float* ef = nullptr;          // [3*n_protein + 1] or nullptr (no whole-protein reduction)
     const double* x = nullptr;    // [n_protein][3] protein positions the placement reads (vb_forward_fragments)
+    float* e_out = nullptr;       // [1] the caller's energy buffer (vb_forward_fragments_energy)
     bool operator==(const StepIO& o) const {
-        return pos == o.pos && energy == o.energy && forces == o.forces && ef == o.ef && x == o.x;
+        return pos == o.pos && energy == o.energy && forces == o.forces && ef == o.ef && x == o.x && e_out == o.e_out;
     }
 };
 
@@ -789,22 +790,24 @@ void node_bwd_tc(Launcher& Lc, int k) {
     if (k >= 1) { snprintf(name, sizeof(name), "bwdB%d", k); if (Lc.next(name)) launch_node_bwdB_tc(Lc, k); }
 }
 
-void enqueue_finalize(Launcher& Lc, const StepIO& io) {
+// `gather` = false leaves out the force gather of the whole-protein reduction: its energy block alone writes ef[3P]
+void enqueue_finalize(Launcher& Lc, const StepIO& io, bool gather = true) {
     vb_handle* h = Lc.h;
     const Workspace& ws = h->ws;
     const bool prot = io.ef != nullptr;
     const int fb = (ws.G + FIN_THREADS / 32 - 1) / (FIN_THREADS / 32);
-    const int pb = prot ? (h->n_protein + FIN_THREADS - 1) / FIN_THREADS : 0;
+    const int pb = prot && gather ? (h->n_protein + FIN_THREADS - 1) / FIN_THREADS : 0;
     Lc.launch(finalize_kernel, dim3(fb + pb + (prot ? 1 : 0)), dim3(FIN_THREADS), 0, ws, h->mw.scalars, fb, pb, h->n_protein,
               h->d_map_rowptr, h->d_map_src, h->d_map_sign, h->d_frag_sign, io.forces, io.energy, io.ef, 0);
     Lc.check();
 }
 
 // The whole-protein reduction of a chunked evaluation, after its last chunk: forces of every fragment atom and the
-// energies every chunk's finalize wrote (h->ws is the batch-wide view here: G is every fragment)
-void enqueue_protein(Launcher& Lc, const StepIO& io) {
+// energies every chunk's finalize wrote (h->ws is the batch-wide view here: G is every fragment); without `gather`, the
+// energy alone
+void enqueue_protein(Launcher& Lc, const StepIO& io, bool gather = true) {
     vb_handle* h = Lc.h;
-    const int pb = (h->n_protein + FIN_THREADS - 1) / FIN_THREADS;
+    const int pb = gather ? (h->n_protein + FIN_THREADS - 1) / FIN_THREADS : 0;
     Lc.launch(finalize_kernel, dim3(pb + 1), dim3(FIN_THREADS), 0, h->ws, h->mw.scalars, 0, pb, h->n_protein,
               h->d_map_rowptr, h->d_map_src, h->d_map_sign, h->d_frag_sign, io.forces, io.energy, io.ef, 1);
     Lc.check();
@@ -965,6 +968,23 @@ void enqueue_energy(Launcher& Lc, const StepIO& io) {
     });
 }
 
+// The energy plan ending in the whole-protein energy ef[3 n_protein]: the signed fragment sum without the force gather,
+// in the same launch as the fragment energies, or, chunked, once after the last chunk from the energies every chunk
+// wrote -- where and in the order enqueue_all sums it, so the two plans' ef[3 n_protein] agree bit for bit.
+void enqueue_energy_protein(Launcher& Lc, const StepIO& io) {
+    vb_handle* h = Lc.h;
+    StepIO eio = io;
+    eio.forces = nullptr;
+    each_chunk(Lc, eio, [&](const StepIO& cio) {
+        const Workspace full = h->ws;
+        h->ws = energy_workspace(full);
+        enqueue_fwd(Lc, cio);
+        if (Lc.next("finalize")) enqueue_finalize(Lc, cio, false);
+        h->ws = full;
+    });
+    if (!h->chunks.empty() && Lc.next("protein")) enqueue_protein(Lc, eio, false);
+}
+
 // The plan a handle evaluates by default: the full one, or the energy plan when it was set up with derivative = 0
 void enqueue_plan(Launcher& Lc, const StepIO& io) {
     if (Lc.h->derivative) enqueue_all(Lc, io);
@@ -1027,7 +1047,7 @@ int clean_accumulators(vb_handle* h, cudaStream_t st) {
 }
 
 enum { K_EVAL = 0, K_HOST = 1, K_MD_EVAL = 2, K_MD_STEP = 3, K_ENERGY = 4, K_ENERGY_HOST = 5, K_MD_LOOP = 6, K_FRAG = 7,
-       K_FRAG_HOST = 8 };
+       K_FRAG_HOST = 8, K_FRAG_E = 9, K_FRAG_E_HOST = 10 };
 
 // Run `enqueue(stream)` -- a sequence of launches / async copies that depends only on (kind, io) and the handle's
 // configuration -- either directly or as a replay of its cached CUDA graph.  A failed capture always ends the capture
@@ -1608,6 +1628,24 @@ int md_eval_enqueue(vb_handle* h, cudaStream_t st, const double* x, float* ef, b
     }
     CUDA_TRY(h, cudaGetLastError());
     if (h->comm_ready && h->comm_auto) return enqueue_allreduce(h, st, ef, 3LL * h->n_protein + 1);
+    return VB_OK;
+}
+// The energy counterpart of md_eval_enqueue without restraints (vb_forward_fragments_energy*): the same placement and
+// refinement, the energy plan ending in the signed fragment sum ef[3 n_protein], then the MM energy without its forces.
+// Only ef[3 n_protein] is written, bit-identical to what md_eval_enqueue writes there for the same handle and positions.
+int md_energy_enqueue(vb_handle* h, cudaStream_t st, const double* x, float* ef) {
+    const int N = h->batch_atoms();
+    float* pos = h->batch_pos();
+    md_place_kernel<<<(N + 255) / 256, 256, 0, st>>>(N, h->d_real, h->d_acc, h->d_rem, h->d_blen, x, pos, h->rs);
+    if (h->caph_ready) caph_relax_kernel<<<1, CAPH_THREADS, 0, st>>>(h->caph, pos);
+    Launcher Lc{h, st, -1, 0, false};
+    enqueue_energy_protein(Lc, eval_io(h, ef));
+    if (Lc.status != cudaSuccess) { h->set_error("kernel launch failed: %s", cudaGetErrorString(Lc.status)); return VB_ERR_CUDA; }
+    if (h->nb_ready && h->nb.hi > h->nb.lo) {
+        nonbonded_kernel<double, false><<<(h->nb.hi - h->nb.lo + 7) / 8, 256, 0, st>>>(h->nb, x, ef, h->d_nb_eatom);
+        nonbonded_energy_kernel<<<1, 256, 0, st>>>(h->nb, h->d_nb_eatom, ef);
+    }
+    CUDA_TRY(h, cudaGetLastError());
     return VB_OK;
 }
 void md_kick1_enqueue(vb_handle* h, cudaStream_t st) {
@@ -2272,7 +2310,9 @@ int vb_set_batch_window(vb_handle* h, int64_t n_batch_atoms, int64_t first_atom)
 }
 
 namespace {
-int fragments_check(vb_handle* h, const char* who) {
+// `forces` = false: the checks of the energy entries, which also take a derivative = 0 handle but not one whose
+// evaluations all-reduce their buffer over connected ranks (their energy would be this rank's part alone)
+int fragments_check(vb_handle* h, const char* who, bool forces = true) {
     if (h->md_unfrag) {
         h->set_error("%s: the MD step is set up un-fragmented (vb_md_setup with real_host = NULL): there are no fragments "
                      "to place; call vb_set_topology again for a fragment batch", who);
@@ -2284,7 +2324,13 @@ int fragments_check(vb_handle* h, const char* who) {
         h->set_error("%s: no placement recipe: call vb_set_fragment_recipe (or vb_md_setup)", who);
         return VB_ERR_STATE;
     }
-    if (int rc = need_derivative(h, who)) return rc;
+    if (forces) {
+        if (int rc = need_derivative(h, who)) return rc;
+    } else if (h->comm_ready && h->comm_auto) {
+        h->set_error("%s: the handle is connected through vb_comm_connect with option comm_auto = 1, and the energy entries "
+                     "do not all-reduce: use vb_forward_fragments", who);
+        return VB_ERR_STATE;
+    }
     return comm_check(h, who);
 }
 // the positions buffer and pinned staging of vb_forward_fragments_host, allocated at its first use and kept with the map
@@ -2341,6 +2387,52 @@ int vb_forward_fragments_host(vb_handle* h, const double* prot_pos_host, float* 
     return VB_OK;
 }
 
+int vb_forward_fragments_energy(vb_handle* h, const double* prot_pos_dev, float* energy_dev, void* stream) {
+    NvtxRange nvtx_("vb_forward_fragments_energy");
+    if (!h) return VB_ERR_ARG;
+    std::lock_guard<std::mutex> lk(h->mu);
+    if (int rc = fragments_check(h, "vb_forward_fragments_energy", false)) return rc;
+    if (!prot_pos_dev || !energy_dev) { h->set_error("vb_forward_fragments_energy: null buffer"); return VB_ERR_ARG; }
+    CUDA_TRY(h, cudaSetDevice(h->device));
+    float* e = h->d_ef + 3 * (size_t)h->n_protein;
+    StepIO io = eval_io(h, h->d_ef);
+    io.x = prot_pos_dev;
+    io.e_out = energy_dev;
+    return run_cached(h, (cudaStream_t)stream, K_FRAG_E, io, [&](cudaStream_t s) -> int {
+        if (int r = md_energy_enqueue(h, s, prot_pos_dev, h->d_ef)) return r;
+        CUDA_TRY(h, cudaMemcpyAsync(energy_dev, e, sizeof(float), cudaMemcpyDeviceToDevice, s));
+        return (int)VB_OK;
+    });
+}
+
+int vb_forward_fragments_energy_host(vb_handle* h, const double* prot_pos_host, float* energy_host) {
+    NvtxRange nvtx_("vb_forward_fragments_energy_host");
+    if (!h) return VB_ERR_ARG;
+    std::lock_guard<std::mutex> lk(h->mu);
+    if (int rc = fragments_check(h, "vb_forward_fragments_energy_host", false)) return rc;
+    if (!prot_pos_host || !energy_host) { h->set_error("vb_forward_fragments_energy_host: null buffer"); return VB_ERR_ARG; }
+    const size_t n3 = 3 * (size_t)h->n_protein;
+    cudaStream_t st = h->own_stream;
+    CUDA_TRY(h, cudaSetDevice(h->device));
+    if (h->md_ready) CUDA_TRY(h, cudaDeviceSynchronize());      // as vb_forward_fragments_host: MD work may still run
+    if (int r = fragments_staging(h)) return r;
+    memcpy(h->h_fx, prot_pos_host, sizeof(double) * n3);
+    // H2D of the positions, every launch of vb_forward_fragments_energy, D2H of the one energy: one graph replay
+    StepIO io = eval_io(h, h->d_ef);
+    io.x = h->d_fx;
+    int rc = run_cached(h, st, K_FRAG_E_HOST, io, [&](cudaStream_t s) -> int {
+        CUDA_TRY(h, cudaMemcpyAsync(h->d_fx, h->h_fx, sizeof(double) * n3, cudaMemcpyHostToDevice, s));
+        if (int r = md_energy_enqueue(h, s, h->d_fx, h->d_ef)) return r;
+        CUDA_TRY(h, cudaMemcpyAsync(h->h_fef + n3, h->d_ef + n3, sizeof(float), cudaMemcpyDeviceToHost, s));
+        return (int)VB_OK;
+    });
+    if (rc != VB_OK) return rc;
+    CUDA_TRY(h, cudaStreamSynchronize(st));
+    if (int r = check_edge_overflow(h, "vb_forward_fragments_energy_host")) return r;
+    *energy_host = h->h_fef[n3];
+    return VB_OK;
+}
+
 // ---- an in-process group of window handles: one FragmentCalculator call over several GPUs of one process ---------------
 // Every member places and refines the whole batch and evaluates its own window into its own partial buffer (its d_ef, on
 // its device), as a rank of the one-process-per-GPU path does; the leader (member 0) then sums the partials in rank order
@@ -2363,6 +2455,7 @@ struct vb_group {
     cudaEvent_t ev_start = nullptr;          // dev[0]: the call's positions are ready
     cudaEvent_t ev_join = nullptr;           // dev[0]: the last join has read the partials
     CommParams join{};                       // comm_allreduce_kernel in gather mode over the partials
+    CommParams join_e{};                     // the same over the partials' energy slots [3n] alone (the energy entries)
     void set_error(const char* fmt, ...) {
         char buf[1024];
         va_list ap;
@@ -2445,7 +2538,7 @@ int group_check_members(vb_handle* const* m, int k, std::string& err) {
 }
 
 // every member as vb_group_create found it, and ready for the call
-int group_check_call(vb_group* g, const char* who) {
+int group_check_call(vb_group* g, const char* who, bool forces = true) {
     for (int r = 0; r < (int)g->m.size(); r++) {
         vb_handle* h = g->m[r];
         if (h->gen != g->gen[r]) {
@@ -2453,7 +2546,7 @@ int group_check_call(vb_group* g, const char* who) {
                          "term, MD or comm setup, or an option); create the group again", who, r);
             return VB_ERR_STATE;
         }
-        if (int rc = fragments_check(h, who)) return member_fail(g, r, rc);
+        if (int rc = fragments_check(h, who, forces)) return member_fail(g, r, rc);
     }
     return VB_OK;
 }
@@ -2472,9 +2565,12 @@ int group_md_sync(vb_group* g, const char* who) {
 // One group call enqueued, members locked: positions to every member (host_x: from pinned host memory; else dev_x on
 // dev[0], read in place by the members there and copied peer-to-peer to the others), each member's evaluation into its
 // partial on its own stream, then, on `leader` (dev[0]), the wait for every member and the rank-order join into ef.
-int group_enqueue(vb_group* g, const double* host_x, const double* dev_x, float* ef, cudaStream_t leader) {
+// With `energy` the members run their energy graphs, which write the partials' energy slots alone, and the join sums
+// those into ef[0].
+int group_enqueue(vb_group* g, const double* host_x, const double* dev_x, float* ef, cudaStream_t leader, bool energy = false) {
     const int k = (int)g->m.size();
     const size_t n3 = 3 * (size_t)g->n_protein;
+    const size_t off = energy ? n3 : 0, len = energy ? 1 : n3 + 1;     // the part of each partial the join reads
     vb_handle* h0 = g->m[0];
     CUDA_TRY(h0, cudaSetDevice(g->dev[0]));
     CUDA_TRY(h0, cudaStreamWaitEvent(leader, g->ev_join, 0));   // the last join, on whichever stream, has read the partials
@@ -2492,8 +2588,10 @@ int group_enqueue(vb_group* g, const double* host_x, const double* dev_x, float*
             else CUDA_TRY(h, cudaMemcpyPeerAsync(h->d_fx, h->device, dev_x, g->dev[0], sizeof(double) * n3, s));
             StepIO io = eval_io(h, h->d_ef);
             io.x = x;
-            if (int r2 = run_cached(h, s, K_FRAG, io, [&](cudaStream_t q) -> int { return md_eval_enqueue(h, q, x, h->d_ef, false); }))
-                return r2;
+            const int r2 = energy
+                ? run_cached(h, s, K_FRAG_E, io, [&](cudaStream_t q) -> int { return md_energy_enqueue(h, q, x, h->d_ef); })
+                : run_cached(h, s, K_FRAG, io, [&](cudaStream_t q) -> int { return md_eval_enqueue(h, q, x, h->d_ef, false); });
+            if (r2) return r2;
             CUDA_TRY(h, cudaEventRecord(g->done[r], s));
             return VB_OK;
         };
@@ -2503,11 +2601,12 @@ int group_enqueue(vb_group* g, const double* host_x, const double* dev_x, float*
     for (int r = 0; r < k; r++) {
         CUDA_TRY(h0, cudaStreamWaitEvent(leader, g->done[r], 0));
         if (!g->peer[r])
-            CUDA_TRY(h0, cudaMemcpyPeerAsync(g->d_stage + r * (n3 + 1), g->dev[0], g->m[r]->d_ef, g->dev[r], sizeof(float) * (n3 + 1), leader));
+            CUDA_TRY(h0, cudaMemcpyPeerAsync(g->d_stage + r * (n3 + 1) + off, g->dev[0], g->m[r]->d_ef + off, g->dev[r],
+                                             sizeof(float) * len, leader));
     }
-    const long long n = (long long)n3 + 1;
+    const long long n = (long long)len;
     const int ctas = (int)std::max<long long>(1, std::min<long long>((n + COMM_THREADS - 1) / COMM_THREADS, COMM_MAX_CTAS));
-    comm_allreduce_kernel<<<ctas, COMM_THREADS, 0, leader>>>(g->join, ef, n);
+    comm_allreduce_kernel<<<ctas, COMM_THREADS, 0, leader>>>(energy ? g->join_e : g->join, ef, n);
     CUDA_TRY(h0, cudaGetLastError());
     CUDA_TRY(h0, cudaEventRecord(g->ev_join, leader));
     return VB_OK;
@@ -2605,6 +2704,8 @@ int vb_group_create(vb_handle* const* members, int n_members, vb_group** out) {
     g->join.world = n_members;
     g->join.gather = 1;
     for (int r = 0; r < n_members; r++) g->join.slots[r] = g->peer[r] ? g->m[r]->d_ef : g->d_stage + r * (n3 + 1);
+    g->join_e = g->join;
+    for (int r = 0; r < n_members; r++) g->join_e.slots[r] = g->join.slots[r] + n3;
     for (int r = 0; r < n_members; r++) g->gen.push_back(members[r]->gen);
     *out = g;
     return VB_OK;
@@ -2651,6 +2752,50 @@ int vb_group_forward_fragments_host(vb_group* g, const double* prot_pos_host, fl
         if (int rc = check_edge_overflow(h, who)) return member_fail(g, r, rc);
     }
     memcpy(ef_prot_host, g->h_ef, sizeof(float) * (n3 + 1));
+    return VB_OK;
+}
+
+
+int vb_group_forward_fragments_energy(vb_group* g, const double* prot_pos_dev, float* energy_dev, void* stream) {
+    NvtxRange nvtx_("vb_group_forward_fragments_energy");
+    if (!g) return VB_ERR_ARG;
+    std::lock_guard<std::mutex> lk(g->mu);
+    if (!prot_pos_dev || !energy_dev) { g->set_error("vb_group_forward_fragments_energy: null buffer"); return VB_ERR_ARG; }
+    DeviceRestore restore;
+    auto locks = lock_members(g->m.data(), (int)g->m.size());
+    const char* who = "vb_group_forward_fragments_energy";
+    if (int rc = group_check_call(g, who, false)) return rc;
+    if (int rc = group_md_sync(g, who)) return rc;
+    return group_enqueue(g, nullptr, prot_pos_dev, energy_dev, (cudaStream_t)stream, true);
+}
+
+int vb_group_forward_fragments_energy_host(vb_group* g, const double* prot_pos_host, float* energy_host) {
+    NvtxRange nvtx_("vb_group_forward_fragments_energy_host");
+    if (!g) return VB_ERR_ARG;
+    std::lock_guard<std::mutex> lk(g->mu);
+    if (!prot_pos_host || !energy_host) { g->set_error("vb_group_forward_fragments_energy_host: null buffer"); return VB_ERR_ARG; }
+    DeviceRestore restore;
+    auto locks = lock_members(g->m.data(), (int)g->m.size());
+    const char* who = "vb_group_forward_fragments_energy_host";
+    if (int rc = group_check_call(g, who, false)) return rc;
+    if (int rc = group_md_sync(g, who)) return rc;
+    const size_t n3 = 3 * (size_t)g->n_protein;
+    memcpy(g->h_x, prot_pos_host, sizeof(double) * n3);
+    if (int rc = group_enqueue(g, g->h_x, nullptr, g->d_ef + n3, g->st, true)) return rc;
+    vb_handle* h0 = g->m[0];
+    auto finish = [&]() -> int {
+        CUDA_TRY(h0, cudaSetDevice(g->dev[0]));
+        CUDA_TRY(h0, cudaMemcpyAsync(g->h_ef + n3, g->d_ef + n3, sizeof(float), cudaMemcpyDeviceToHost, g->st));
+        CUDA_TRY(h0, cudaStreamSynchronize(g->st));
+        return VB_OK;
+    };
+    if (int rc = finish()) return member_fail(g, 0, rc);
+    for (int r = 0; r < (int)g->m.size(); r++) {
+        vb_handle* h = g->m[r];
+        if (cudaSetDevice(h->device) != cudaSuccess) { g->set_error("%s: member %d: cudaSetDevice failed", who, r); return VB_ERR_CUDA; }
+        if (int rc = check_edge_overflow(h, who)) return member_fail(g, r, rc);
+    }
+    *energy_host = g->h_ef[n3];
     return VB_OK;
 }
 

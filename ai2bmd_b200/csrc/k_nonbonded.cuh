@@ -22,7 +22,9 @@ struct NbParams {
     float kj_mol;                 // kJ/mol in eV
 };
 
-template <typename PosT>
+// FORCES = false is the energy-only instantiation: the same per-pair energy arithmetic and lane order, so e_atom is
+// bit-identical to the full kernel's, without the force sums and the ef row stores (and ef is not read).
+template <typename PosT, bool FORCES = true>
 __global__ void __launch_bounds__(256) nonbonded_kernel(NbParams p, const PosT* __restrict__ pos, float* __restrict__ ef,
                                                         double* __restrict__ e_atom) {
     const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
@@ -43,29 +45,36 @@ __global__ void __launch_bounds__(256) nonbonded_kernel(NbParams p, const PosT* 
         if (a < x1 && p.excl_col[a] == j) continue;
         // vec = pos[dst] - pos[src]   (nonbonded.py:41-43)
         const float vx = xi - (float)pos[3 * j], vy = yi - (float)pos[3 * j + 1], vz = zi - (float)pos[3 * j + 2];
-        const float d2 = vx * vx + vy * vy + vz * vz;
+        // d2 and the LJ bracket are spelled out as the compiler contracts them in the force kernel, so that the energy-only
+        // instantiation, where c12 has one use, cannot contract them otherwise (the force kernel's code is unchanged)
+        const float d2 = fmaf(vz, vz, fmaf(vx, vx, vy * vy));
         const float d = sqrtf(d2);
         // LJ (nonbonded.py:46-51)
         const float sij = 0.5f * (p.sigma[j] + si) * 10.0f;
         const float eij = sqrtf(p.eps[j] * ei);
         const float t = sij * sij / d2;
         const float c6 = t * t * t, c12 = c6 * c6;
-        const float e_lj = 4.0f * eij * (c12 - c6);
+        const float e_lj = 4.0f * eij * __fsub_rn(c12, c6);
         const float f_lj = 24.0f * eij * (2.0f * c12 - c6) / d2;
         // Coulomb (nonbonded.py:54-55)
         const float e_c = p.coulomb_k * p.q[j] * qi / d;
         const float f_c = e_c / d2;
-        const float f = f_lj + f_c;
-        fx += f * vx; fy += f * vy; fz += f * vz;
+        if (FORCES) {
+            const float f = f_lj + f_c;
+            fx += f * vx; fy += f * vy; fz += f * vz;
+        }
         e += (double)e_lj + (double)e_c;
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
-        fx += __shfl_xor_sync(0xffffffffu, fx, o); fy += __shfl_xor_sync(0xffffffffu, fy, o);
-        fz += __shfl_xor_sync(0xffffffffu, fz, o); e += __shfl_xor_sync(0xffffffffu, e, o);
+        if (FORCES) {
+            fx += __shfl_xor_sync(0xffffffffu, fx, o); fy += __shfl_xor_sync(0xffffffffu, fy, o);
+            fz += __shfl_xor_sync(0xffffffffu, fz, o);
+        }
+        e += __shfl_xor_sync(0xffffffffu, e, o);
     }
     if (lane == 0) {
-        ef[3 * i] += fx * p.kj_mol; ef[3 * i + 1] += fy * p.kj_mol; ef[3 * i + 2] += fz * p.kj_mol;
+        if (FORCES) { ef[3 * i] += fx * p.kj_mol; ef[3 * i + 1] += fy * p.kj_mol; ef[3 * i + 2] += fz * p.kj_mol; }
         e_atom[i] = e;
     }
 }

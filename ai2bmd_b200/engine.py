@@ -47,7 +47,8 @@ EXPORTED_SYMBOLS = [
     "vb_set_caph", "vb_caph_relax", "vb_chunk_fragments",
     "vb_set_fragment_recipe", "vb_forward_fragments", "vb_forward_fragments_host", "vb_set_batch_window",
     "vb_group_create", "vb_group_destroy", "vb_group_last_error", "vb_group_forward_fragments",
-    "vb_group_forward_fragments_host",
+    "vb_group_forward_fragments_host", "vb_forward_fragments_energy", "vb_forward_fragments_energy_host",
+    "vb_group_forward_fragments_energy", "vb_group_forward_fragments_energy_host",
 ]
 
 
@@ -173,6 +174,12 @@ def load_library(path: Optional[str] = None):
     lib.vb_group_forward_fragments.argtypes = [vp, vp, vp, vp]
     lib.vb_group_forward_fragments_host.restype = C.c_int
     lib.vb_group_forward_fragments_host.argtypes = [vp, vp, vp]
+    for name in ("vb_forward_fragments_energy", "vb_group_forward_fragments_energy"):
+        getattr(lib, name).restype = C.c_int
+        getattr(lib, name).argtypes = [vp, vp, vp, vp]
+    for name in ("vb_forward_fragments_energy_host", "vb_group_forward_fragments_energy_host"):
+        getattr(lib, name).restype = C.c_int
+        getattr(lib, name).argtypes = [vp, vp, vp]
     if path == _build.LIB_PATH:
         _lib = lib
     return lib
@@ -385,6 +392,23 @@ class Engine:
         asynchronous on ``stream_ptr``.  It shares the workspace with the MD step: order it after MD work of this engine
         (the same stream, or a wait on an event of it)."""
         self._check(self.lib.vb_forward_fragments(self.h, prot_pos_ptr, ef_ptr, stream_ptr), "vb_forward_fragments")
+
+    def forward_fragments_energy_host(self, prot_pos: np.ndarray) -> float:
+        """Protein positions [n_protein, 3] (A) in, the energy [eV] of :meth:`forward_fragments_host` out, bit for bit,
+        without forces: the energy plan, in one graph replay, synchronous.  Also on a ``derivative=False`` engine."""
+        x = np.ascontiguousarray(prot_pos, dtype=np.float64)
+        if x.shape != (self.n_protein, 3):
+            raise ValueError(f"prot_pos must be [{self.n_protein},3]")
+        e = np.empty(1, dtype=np.float32)
+        rc = self.lib.vb_forward_fragments_energy_host(self.h, x.__array_interface__["data"][0], e.__array_interface__["data"][0])
+        if rc < 0:
+            self._check(rc, "vb_forward_fragments_energy_host")
+        return float(e[0])
+
+    def forward_fragments_energy_device(self, prot_pos_ptr: int, e_ptr: int, stream_ptr: int = 0):
+        """Raw device pointers: fp64 protein positions [n_protein, 3] -> one float32 energy; asynchronous on
+        ``stream_ptr``, ordered like :meth:`forward_fragments_device`."""
+        self._check(self.lib.vb_forward_fragments_energy(self.h, prot_pos_ptr, e_ptr, stream_ptr), "vb_forward_fragments_energy")
 
     # ---- NVLink peer-memory all-reduce (include/visnet_b200.h: vb_comm_*) ----
     def comm_init(self, rank: int, world: int, max_floats: int) -> bytes:
@@ -667,6 +691,24 @@ class EngineGroup:
         """Raw device pointers on member 0's device: fp64 protein positions [n_protein, 3] -> ef [3 n_protein + 1];
         asynchronous on ``stream_ptr`` (a stream of member 0's device)."""
         self._check(self.lib.vb_group_forward_fragments(self.g, prot_pos_ptr, ef_ptr, stream_ptr), "vb_group_forward_fragments")
+
+    def forward_fragments_energy_host(self, prot_pos: np.ndarray) -> float:
+        """The energy [eV] of :meth:`forward_fragments_host`, bit for bit, without forces: every member runs its energy
+        plan and member 0 sums their energies in rank order; synchronous."""
+        x = np.ascontiguousarray(prot_pos, dtype=np.float64)
+        if x.shape != (self.n_protein, 3):
+            raise ValueError(f"prot_pos must be [{self.n_protein},3]")
+        e = np.empty(1, dtype=np.float32)
+        rc = self.lib.vb_group_forward_fragments_energy_host(self.g, x.__array_interface__["data"][0], e.__array_interface__["data"][0])
+        if rc < 0:
+            self._check(rc, "vb_group_forward_fragments_energy_host")
+        return float(e[0])
+
+    def forward_fragments_energy_device(self, prot_pos_ptr: int, e_ptr: int, stream_ptr: int = 0):
+        """Raw device pointers on member 0's device: fp64 protein positions [n_protein, 3] -> one float32 energy;
+        asynchronous on ``stream_ptr`` (a stream of member 0's device)."""
+        self._check(self.lib.vb_group_forward_fragments_energy(self.g, prot_pos_ptr, e_ptr, stream_ptr),
+                    "vb_group_forward_fragments_energy")
 
 
 def tc_selftest(a: np.ndarray, w_nk: np.ndarray, reps: int = 1, device: int = 0, rows: int = 128):

@@ -328,6 +328,22 @@ int vb_forward_fragments(vb_handle* h, const double* prot_pos_dev, float* ef_pro
  * After vb_md_setup it first synchronises the device, so it may follow MD work enqueued on any stream without a wait. */
 int vb_forward_fragments_host(vb_handle* h, const double* prot_pos_host, float* ef_prot_host);
 
+/* The energy of the same call without forces: the reference's FragmentCalculator on a model loaded with
+ * derivative=False, for conformer ranking, energy scans and Monte-Carlo acceptance tests on a protein.  The placement and
+ * the hydrogen refinement as above, then the energy plan of vb_forward_energy on the placed batch (its window) ending in
+ * the signed fragment-energy sum, then the MM energy without its forces.  The result, bonded + MM energy in eV, is the
+ * number vb_forward_fragments writes to ef_prot_dev[3*n_protein] for the same handle, options and positions, bit for
+ * bit; it is also left in slot 3*n_protein of the internal buffer (vb_debug_read "ef"), whose force rows stay as they
+ * were.  Accepts derivative = 1 and derivative = 0 handles; otherwise the checks and messages of vb_forward_fragments,
+ * and VB_ERR_STATE on a handle connected through vb_comm_connect with option comm_auto = 1 (no all-reduce here).
+ * prot_pos_dev[3*n_protein] (fp64) -> energy_dev[1], device buffers, asynchronous on `stream`: one replay of a CUDA
+ * graph cached per buffer pair, next to the graphs of vb_forward_fragments. */
+int vb_forward_fragments_energy(vb_handle* h, const double* prot_pos_dev, float* energy_dev, void* stream);
+/* The same with HOST buffers, synchronous: one graph replay with the H2D of the positions and the D2H of one float
+ * inside; like vb_forward_fragments_host it waits for the device after vb_md_setup and fails with VB_ERR_STATE when a
+ * step produced more edges than a trimmed max_edges. */
+int vb_forward_fragments_energy_host(vb_handle* h, const double* prot_pos_host, float* energy_host);
+
 /* ---- A window of a fragment batch: one rank's shard that places and refines the whole batch ---------------------------
  * Declares the topology of vb_set_topology, N atoms, to be atoms [first_atom, first_atom + N) of a packed fragment batch of
  * n_batch_atoms atoms.  From then on the placement recipe (vb_md_setup, vb_set_fragment_recipe: arrays of n_batch_atoms
@@ -383,6 +399,13 @@ int vb_group_forward_fragments(vb_group* g, const double* prot_pos_dev, float* e
 /* The same with HOST buffers, synchronous: the positions go from one pinned staging buffer to every member; fails with
  * VB_ERR_STATE, naming the member, when one produced more edges than its trimmed max_edges. */
 int vb_group_forward_fragments_host(vb_group* g, const double* prot_pos_host, float* ef_prot_host);
+/* The energy alone, as vb_forward_fragments_energy on every member: each runs its energy graph into its partial's slot
+ * 3*n_protein, and member 0 sums those slots in rank order from +0.0f into energy_dev[0] (on member 0's device,
+ * asynchronous on `stream`) -- bit-identical to slot 3*n_protein of vb_group_forward_fragments.  The members stay
+ * derivative = 1 handles, so the workspace is not reduced. */
+int vb_group_forward_fragments_energy(vb_group* g, const double* prot_pos_dev, float* energy_dev, void* stream);
+/* The same with HOST buffers, synchronous, with the edge-overflow check of vb_group_forward_fragments_host. */
+int vb_group_forward_fragments_energy_host(vb_group* g, const double* prot_pos_host, float* energy_host);
 
 /* ---- One-shot all-reduce over NVLink peer memory (SURVEY section 8e) ---------------------------------------------
  * One process per GPU.  vb_comm_init allocates this rank's window (2 parities x world slots of max_floats) and returns
