@@ -616,13 +616,15 @@ class Engine:
         vector features by their max and min over the 128 channels, so the gradient of the energy is routed through the
         argmax / argmin channel.  Where the two largest (or two smallest) channel norms agree to fp32 rounding the
         argmax flips with the rounding order and the force on that fragment jumps by up to ~1e-2 eV/A -- in the
-        reference as much as here.  Returns the sorted atom indices whose top-two or bottom-two channel norms in any
-        layer differ by less than ``rel_gap`` relative; callers comparing two evaluation orders (tests,
-        plan-vs-plan checks) exclude the fragments of these atoms.
+        reference as much as here.  Returns the sorted atom indices whose top-two or bottom-two channel norms at any
+        of the seven VecLayerNorm sites differ by less than ``rel_gap`` relative: V[l] entering layer l's
+        ``vec_layernorm`` for l = 1..5 and V[6] entering the head's ``vec_out_norm`` (V[0] is identically zero).
+        Callers comparing two evaluation orders (plan-vs-plan checks) treat the fragments of these atoms apart;
+        oracle/vecln_branch.py names the branch the evaluation took there.
         """
         n = self.n_atoms
         hit = np.zeros(n, dtype=bool)
-        for k in range(1, 6):                     # the vector features entering layer 0 are identically zero
+        for k in range(1, 7):                     # layers 1..5 and the head; V[0] = 0 has no tie
             v = self.debug_read("V", k, (n, 3, 128)).astype(np.float64)
             srt = np.sort(np.sqrt((v * v).sum(1)), axis=1)
             hit |= ((srt[:, -1] - srt[:, -2]) < rel_gap * srt[:, -1]) | ((srt[:, 1] - srt[:, 0]) < rel_gap * srt[:, 1])

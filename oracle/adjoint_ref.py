@@ -45,24 +45,35 @@ def ln_bwd(x, w, gy, eps=1e-5):
     return rstd * (gh - gh.mean(-1, keepdim=True) - xh * (gh * xh).mean(-1, keepdim=True))
 
 
-def vecln_fwd(vec, w, eps=1e-12):
+def _extremes(nc, pin):
+    """(mx, amx, mn, amn) of the clamped channel norms nc [N,D]: the natural max / min, or with ``pin`` = (amx, amn)
+    (long [N]) the norms of the pinned channels.  A pinned evaluation is one smooth branch of the model: the gather
+    below is what the max / min are away from a tie, and its gradient goes to the pinned channels."""
+    if pin is None:
+        mx, amx = nc.max(-1)
+        mn, amn = nc.min(-1)
+        return mx, amx, mn, amn
+    amx, amn = (torch.as_tensor(a, dtype=torch.long, device=nc.device) for a in pin)
+    ar = torch.arange(nc.shape[0], device=nc.device)
+    return nc[ar, amx], amx, nc[ar, amn], amn
+
+
+def vecln_fwd(vec, w, eps=1e-12, pin=None):
     """utils.py:200-228.  The global ``(dist==0).all()`` early-out is value- and gradient-neutral
-    (all-zero rows give 0 either way), so it is not restated."""
+    (all-zero rows give 0 either way), so it is not restated.  pin: optional (amx, amn) per node (see _extremes)."""
     n = torch.sqrt((vec * vec).sum(1))                      # [N,D]
     nc = n.clamp(min=eps)
-    mx = nc.max(-1).values
-    mn = nc.min(-1).values
+    mx, _, mn, _ = _extremes(nc, pin)
     delta = mx - mn
     delta = torch.where(delta == 0, torch.ones_like(delta), delta)
     y = (nc - mn[:, None]) / delta[:, None]
     return torch.relu(y)[:, None, :] * (vec / nc[:, None, :]) * w
 
 
-def vecln_bwd(vec, w, gout, eps=1e-12):
+def vecln_bwd(vec, w, gout, eps=1e-12, pin=None):
     n = torch.sqrt((vec * vec).sum(1))
     nc = n.clamp(min=eps)
-    mx, amx = nc.max(-1)
-    mn, amn = nc.min(-1)
+    mx, amx, mn, amn = _extremes(nc, pin)
     delta_raw = mx - mn
     zero = delta_raw == 0
     delta = torch.where(zero, torch.ones_like(delta_raw), delta_raw)
@@ -79,7 +90,7 @@ def vecln_bwd(vec, w, gout, eps=1e-12):
     g_mx = g_delta
     g_mn = g_mn - g_delta
     g_nc = g_nc.clone()
-    ar = torch.arange(vec.shape[0])
+    ar = torch.arange(vec.shape[0], device=vec.device)
     g_nc[ar, amx] += g_mx
     g_nc[ar, amn] += g_mn
     g_vec = g_dir / nc[:, None, :]
@@ -90,7 +101,13 @@ def vecln_bwd(vec, w, gout, eps=1e-12):
 
 
 class AdjointViSNet:
-    """Explicit forward (saving what the reverse sweep needs) + explicit reverse sweep."""
+    """Explicit forward (saving what the reverse sweep needs) + explicit reverse sweep.
+
+    ``pins`` (forward, backward, energy_and_forces): optional {site: (amx [N], amn [N])} fixing the channels the
+    VecLayerNorm(max_min) max / min take at a site; site l < L is layer l's ``vec_layernorm``, site L is
+    ``vec_out_norm``.  Sites without a pin take the natural argmax / argmin.  Where two channel norms tie to fp32
+    rounding the engine's branch is not the fp64 argmax (DESIGN section 2); pinned to the engine's channels the
+    oracle is the smooth function whose gradient the engine computes (oracle/vecln_branch.py)."""
 
     def __init__(self, oracle: OracleViSNet):
         self.o = oracle
@@ -99,8 +116,9 @@ class AdjointViSNet:
         self.D, self.L, self.H = HP["D"], HP["L"], HP["H"]
 
     # ---------------------------------------------------------------------------------- forward
-    def forward(self, z, pos, batch, edge_index) -> Dict[str, torch.Tensor]:
+    def forward(self, z, pos, batch, edge_index, pins=None) -> Dict[str, torch.Tensor]:
         sd, D, H, L = self.sd, self.D, self.H, self.L
+        pins = pins or {}
         rm = "representation_model."
         S: Dict[str, torch.Tensor] = {}
         src, dst = edge_index[0], edge_index[1]
@@ -134,7 +152,7 @@ class AdjointViSNet:
             S[f"x_in{l}"], S[f"vec_in{l}"], S[f"f_in{l}"] = x, vec, f
             # node stage A
             xn = ln_fwd(x, sd[p + "layernorm.weight"], sd[p + "layernorm.bias"])
-            vn = vecln_fwd(vec, sd[p + "vec_layernorm.weight"])
+            vn = vecln_fwd(vec, sd[p + "vec_layernorm.weight"], pin=pins.get(l))
             q = xn @ sd[p + "q_proj.weight"].T + sd[p + "q_proj.bias"]
             k = xn @ sd[p + "k_proj.weight"].T + sd[p + "k_proj.bias"]
             v = xn @ sd[p + "v_proj.weight"].T + sd[p + "v_proj.bias"]
@@ -179,7 +197,7 @@ class AdjointViSNet:
 
         # head (per atom)
         X = ln_fwd(x, sd[rm + "out_norm.weight"], sd[rm + "out_norm.bias"])
-        V = vecln_fwd(vec, sd[rm + "vec_out_norm.weight"])
+        V = vecln_fwd(vec, sd[rm + "vec_out_norm.weight"], pin=pins.get(L))
         o0, o1_ = "output_model.output_network.0.", "output_model.output_network.1."
         p1 = V @ sd[o0 + "vec1_proj.weight"].T
         n1 = torch.sqrt((p1 * p1).sum(1))
@@ -200,9 +218,11 @@ class AdjointViSNet:
         return S
 
     # --------------------------------------------------------------------------------- backward
-    def backward(self, z, pos, batch, edge_index, S) -> Dict[str, torch.Tensor]:
-        """Reverse sweep for dE_total/dpos; returns forces and every stage's adjoint (for stage checks)."""
+    def backward(self, z, pos, batch, edge_index, S, pins=None) -> Dict[str, torch.Tensor]:
+        """Reverse sweep for dE_total/dpos; returns forces and every stage's adjoint (for stage checks).  ``pins``: as
+        given to the forward that made S."""
         sd, D, H, L = self.sd, self.D, self.H, self.L
+        pins = pins or {}
         rm = "representation_model."
         B: Dict[str, torch.Tensor] = {}
         src, dst = edge_index[0], edge_index[1]
@@ -232,7 +252,7 @@ class AdjointViSNet:
         g_X, g_n1 = g_cat[:, :D], g_cat[:, D:]
         g_p1 = safe_div(g_n1, S["n1"])[:, None, :] * S["p1"]
         g_V = g_p1 @ sd[o0 + "vec1_proj.weight"] + g_p2 @ sd[o0 + "vec2_proj.weight"]
-        gvec = vecln_bwd(S["vec_out"], sd[rm + "vec_out_norm.weight"], g_V)
+        gvec = vecln_bwd(S["vec_out"], sd[rm + "vec_out_norm.weight"], g_V, pin=pins.get(L))
         gx = ln_bwd(S["x_out"], sd[rm + "out_norm.weight"], g_X)
         B["gx_out"], B["gvec_out"] = gx, gvec
 
@@ -318,7 +338,7 @@ class AdjointViSNet:
                 B[f"g_t{l}"], B[f"g_u{l}"] = g_t, g_u
                 g_vn = g_vn + g_t @ sd[p + "w_trg_proj.weight"] + g_u @ sd[p + "w_src_proj.weight"]
             B[f"g_vn{l}"], B[f"g_xn{l}"] = g_vn, g_xn
-            gvec = gvec + vecln_bwd(vec_in, sd[p + "vec_layernorm.weight"], g_vn)
+            gvec = gvec + vecln_bwd(vec_in, sd[p + "vec_layernorm.weight"], g_vn, pin=pins.get(l))
             gx = gx + ln_bwd(x_in, sd[p + "layernorm.weight"], g_xn)
             B[f"gx_in{l}"], B[f"gvec_in{l}"] = gx, gvec
 
@@ -350,11 +370,11 @@ class AdjointViSNet:
         B["forces"] = -dpos
         return B
 
-    def energy_and_forces(self, z, pos, batch, edge_index):
+    def energy_and_forces(self, z, pos, batch, edge_index, pins=None):
         z = torch.as_tensor(z, dtype=torch.long)
         batch = torch.as_tensor(batch, dtype=torch.long)
         pos = torch.as_tensor(pos).to(self.dtype)
         with torch.no_grad():
-            S = self.forward(z, pos, batch, edge_index)
-            B = self.backward(z, pos, batch, edge_index, S)
+            S = self.forward(z, pos, batch, edge_index, pins)
+            B = self.backward(z, pos, batch, edge_index, S, pins)
         return S["E"], B["forces"], S, B

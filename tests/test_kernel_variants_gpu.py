@@ -18,11 +18,14 @@ b. Stage matrix: the evaluation one launch at a time against the fp64 hand-adjoi
        abd-default 1.5e-4 (gvec_in2, 17)       abd-default seed 3 3.3e-4 (g_vn_msg, 13)
    The bars per buffer are at FRAG_BAR below.
 c. End to end per fragment above 4,096 atoms, where the stage oracle is too large for one CPU process: every fragment's
-   energy and forces against the fp64 oracle (run on the GPU in chunks of 64 fragments).  Bars: energy e_tol, forces
-   5e-5 + 2e-5 max|F_fragment|.  Fragments on a VecLayerNorm argmax tie (DESIGN section 2, Engine.vecln_near_ties) are
-   held only to a bounded force jump (5e-2 eV/A) and may be at most 5 % of the batch.  Measured on the same card: |dE|
-   up to 0.30 e_tol (c160) and 0.32 e_tol (c512); |dF| up to 0.40 of its bar (c160, tensor-core node stage), 0.17
-   (c160, SIMT) and 0.59 (c512; largest |dF| 2.1e-4 eV/A, c160); 2 of 160 and 8 of 512 fragments sit on a tie.
+   energy and forces against the fp64 oracle on the VecLayerNorm(max_min) branch the engine took (DESIGN section 2,
+   oracle/vecln_branch.py): the natural oracle (run on the GPU in chunks of 64 fragments) where the engine's channel
+   norms leave one branch and it is the oracle's own, else the CPU hand adjoint pinned to each branch they leave open,
+   the best of them.  Bars, for every fragment: energy e_tol, forces 5e-5 + 2e-5 max|F_fragment|.  Measured on the same
+   card: |dE| up to 0.30 e_tol (c160) and 0.32 e_tol (c512); |dF| up to 0.40 of its bar (c160, tensor-core node stage),
+   0.17 (c160, SIMT) and 0.59 (c512).  No fragment of either batch needed a pinned evaluation: the 2 of 160 and 8 of
+   512 fragments with channel norms within 1e-5 of each other (Engine.vecln_near_ties) leave the engine one branch
+   each, and it is the fp64 oracle's.  That is measured, not assumed: a fragment where it is not is checked pinned.
 d. Every option a case sets changes the dry-run kernel list (or the tile plan / gxa_parts) against the same case
    without it; "krot" and "use_pdl" change kernel arguments and launch attributes only and are exempt.
 """
@@ -235,11 +238,16 @@ def _set_opts(eng, opts):
 
 
 def e2e_errors(real_weights, case):
-    """Engine vs fp64 oracle per fragment for one E2E case: (fd, eng, dE [G], dF [G], F bar [G], tie fragments)."""
+    """Engine vs fp64 oracle per fragment for one E2E case, on the VecLayerNorm branch the engine took: (fd, eng, dE [G],
+    dF [G], F bar [G], pinned, off_natural).  A fragment is checked against the natural oracle (run on the GPU in chunks
+    of 64 fragments) when the engine's branch there is one branch and is the oracle's own; otherwise against the pinned
+    CPU hand adjoint (oracle/vecln_branch.py) on each branch the engine may have taken, keeping the best.  pinned: the
+    fragments that needed that; off_natural: those of them whose best branch is not the natural one."""
     import torch
     from ai2bmd_b200.engine import Engine
     from ai2bmd_b200.synth import synthetic_batch
     from oracle import visnet_ref as O
+    from oracle.vecln_branch import Candidates, best_branch, engine_vectors, natural_branch
     n, seed, opts, _ = E2E_CASES[case]
     fd = synthetic_batch(n, seed=seed)
     eng = Engine(real_weights, 0)
@@ -248,42 +256,62 @@ def e2e_errors(real_weights, case):
     eng.forward_host(fd.pos)
     eng.set_option("calibrate", 1)                   # the plan the host entry points run
     e, f = eng.forward_host(fd.pos)
-    ties = np.unique(fd.batch[eng.vecln_near_ties()])
+    cand = Candidates(engine_vectors(eng))
+    amb = set(np.unique(fd.batch[cand.ambiguous()[:, 1]]).tolist())
     oracle = O.OracleViSNet({k: torch.from_numpy(v) for k, v in real_weights.items()}, torch.float64, device="cuda")
     G = len(fd)
     de, df, fbar = np.zeros(G), np.zeros(G), np.zeros(G)
+    pinned, off_natural = [], []
+
+    def score(g, e_ref, f_ref, lo):
+        s, t = int(fd.start[g]), int(fd.end[g])
+        return (abs(float(e[g]) - e_ref) / e_tol(e_ref), np.abs(f[s:t] - f_ref[s - lo:t - lo]).max(),
+                5e-5 + 2e-5 * np.abs(f_ref[s - lo:t - lo]).max())
+
     for g0 in range(0, G, 64):                       # fragments are independent: bounded oracle memory
         sub = fd[g0:min(G, g0 + 64)]
+        cap = {}
+        with torch.no_grad():
+            oracle.forward(torch.from_numpy(sub.z).cuda(), torch.from_numpy(sub.pos).cuda().double(),
+                           torch.from_numpy(sub.batch).cuda(), cap=cap)
+        nat = natural_branch([cap[f"vec_in{l}"] for l in range(6)] + [cap["vec_out"]])
+        del cap
         e_ref, f_ref = oracle.energy_and_forces(sub.z, sub.pos, sub.batch)
         e_ref, f_ref = e_ref.cpu().numpy()[:, 0], f_ref.cpu().numpy()
-        a0 = fd.start[g0]
+        a0 = int(fd.start[g0])
         for j in range(len(sub)):
-            g, s, t = g0 + j, int(sub.start[j]), int(sub.end[j])
-            de[g] = abs(float(e[g]) - e_ref[j]) / e_tol(e_ref[j])
-            df[g] = np.abs(f[a0 + s:a0 + t] - f_ref[s:t]).max()
-            fbar[g] = 5e-5 + 2e-5 * np.abs(f_ref[s:t]).max()
+            g, s, t = g0 + j, int(fd.start[g0 + j]), int(fd.end[g0 + j])
+            own = cand.contains({k: (mx[s - a0:t - a0], mn[s - a0:t - a0]) for k, (mx, mn) in nat.items()}, s, t)
+            if own and g not in amb:
+                de[g], df[g], fbar[g] = score(g, e_ref[j], f_ref, a0)
+                continue
+            pinned.append(g)
+            er, fr, _ = best_branch(real_weights, cand, fd.z, fd.pos, s, t, f)
+            de[g], df[g], fbar[g] = score(g, er, fr, s)
+            nat_err = score(g, e_ref[j], f_ref, a0)
+            if nat_err[1] > nat_err[2]:
+                off_natural.append(g)
     del oracle
     torch.cuda.empty_cache()
-    return fd, eng, de, df, fbar, ties
+    return fd, eng, de, df, fbar, pinned, off_natural
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", list(E2E_CASES))
 def test_every_fragment_against_the_fp64_oracle(real_weights, case):
-    fd, eng, de, df, fbar, ties = e2e_errors(real_weights, case)
-    G = len(fd)
+    fd, eng, de, df, fbar, pinned, off_natural = e2e_errors(real_weights, case)
     ran = _kernel_set(eng.stage_kernels())
     want = set(_pinned(f"e2e:{case}")) | set(E2E_EXTRA.get(case, []))
     assert want <= ran, f"{case} does not run {sorted(want - ran)}; it runs {sorted(ran)}"
     assert len(fd.z) > 4096
     for k, v in E2E_CASES[case][3].items():
         assert eng.get_option(k) == v, (case, k)
+    print(f"{case}: |dE| / e_tol up to {de.max():.2f}, |dF| / bar up to {(df / fbar).max():.2f}; "
+          f"{len(pinned)} fragments checked on a pinned branch (worst |dF| / bar "
+          f"{max([df[g] / fbar[g] for g in pinned], default=0):.2f}), {len(off_natural)} off the natural one")
     assert (de <= 1).all(), f"energy: fragments {np.flatnonzero(de > 1)[:8]} (|dE| / e_tol up to {de.max():.2f})"
-    assert len(ties) <= G // 20, f"{len(ties)} fragments on a VecLayerNorm tie"
-    keep = ~np.isin(np.arange(G), ties)
-    bad = np.flatnonzero(keep & (df > fbar))
+    bad = np.flatnonzero(df > fbar)
     assert not len(bad), f"forces: fragments {bad[:8]}, |dF| {df[bad[:8]]} over {fbar[bad[:8]]}"
-    assert df.max() <= 5e-2
 
 
 # ---- d. knobs act ---------------------------------------------------------------------------------------------------

@@ -103,13 +103,26 @@ def _geometry_key(z, pos, batch):
     return h.hexdigest()
 
 
-def _oracle(key, sd, z, pos, batch, ei):
-    """fp64 hand-adjoint tensors of one geometry; the last one is kept, so that runs of cases on one geometry (one
-    case under several decoys, options or launch plans) build it once."""
+def _pins_key(pins):
+    """Cache key of VecLayerNorm pins {site: (amx, amn)} (None: the natural branch)."""
+    if pins is None:
+        return None
+    h = hashlib.sha256()
+    for site in sorted(pins):
+        h.update(str(site).encode())
+        for a in pins[site]:
+            h.update(np.ascontiguousarray(np.asarray(a, dtype=np.int64)).tobytes())
+    return h.hexdigest()
+
+
+def _oracle(key, sd, z, pos, batch, ei, pins=None):
+    """fp64 hand-adjoint tensors of one geometry (on the VecLayerNorm branch ``pins``, AdjointViSNet); the last one is
+    kept, so that runs of cases on one geometry (one case under several decoys, options or launch plans) build it
+    once."""
     if key is not None and key in _oracle_cache:
         return _oracle_cache[key]
     adj = AdjointViSNet(O.OracleViSNet(sd, torch.float64))
-    Eo, Fo, S, B = adj.energy_and_forces(z, pos, batch, ei)
+    Eo, Fo, S, B = adj.energy_and_forces(z, pos, batch, ei, pins=pins)
     out = ({k: v.numpy() for k, v in S.items()}, {k: v.numpy() for k, v in B.items()})
     _oracle_cache.clear()
     if key is not None:
@@ -118,7 +131,7 @@ def _oracle(key, sd, z, pos, batch, ei):
 
 
 def stage_report(frags="chig", weights="real", max_frags=0, opts="", calibrate=False, detail=None, decoy=None,
-                 derivative=True, calibrate_pos=None):
+                 derivative=True, calibrate_pos=None, pins=None):
     """Run the evaluation one launch at a time and compare every buffer a stage produces with the fp64 hand-adjoint
     oracle.  Returns (lines, worst) where worst = [(stage, what, rel)] of the comparisons, rel relative to the largest
     reference entry of the buffer.
@@ -132,7 +145,9 @@ def stage_report(frags="chig", weights="real", max_frags=0, opts="", calibrate=F
     fragment_rel), "kernels" = Engine.stage_kernels(), "options" (resolved tile_rows, tc_rows, gxa_parts, node_tc,
     node_nb, edge_tc, npw, and use_pdl / tile_rows / tc_rows again after the last evaluation, as "<key>_after"),
     "n_edges", "n_atoms", "max_degree", and "host" = (energies, forces or None) of the last evaluation through the host
-    entry point."""
+    entry point, and "vectors" = V[0..L] the engine's last evaluation left (oracle/vecln_branch.py reads its VecLayerNorm
+    branch from them).  pins: the VecLayerNorm branch of the oracle ({site: (amx, amn)} over the selected atoms, see
+    AdjointViSNet); None is the natural one."""
     if isinstance(frags, str):
         g = np.load(os.path.join(ROOT, "tests", "golden", f"fragments_{frags}.npz"))
         z, pos, batch = g["z"], g["pos"], g["batch"]
@@ -154,7 +169,7 @@ def stage_report(frags="chig", weights="real", max_frags=0, opts="", calibrate=F
     ei = torch.from_numpy(O.slots_to_edge_index(slots, deg))
     E, N = ei.shape[1], len(z)
     key = frags if isinstance(frags, str) else _geometry_key(z, pos, batch)
-    S, B = _oracle((key, max_frags, str(weights)), sd, z, pos, batch, ei)
+    S, B = _oracle((key, max_frags, str(weights), _pins_key(pins)), sd, z, pos, batch, ei, pins)
 
     eng = Engine({k: v.numpy() for k, v in sd.items()}, 0, derivative=derivative)
     G = int(batch.max()) + 1
@@ -319,6 +334,8 @@ def stage_report(frags="chig", weights="real", max_frags=0, opts="", calibrate=F
         for k in ("use_pdl", "tile_rows", "tc_rows"):
             detail["options"][f"{k}_after"] = eng.get_option(k)
         detail["host"] = (e, f)
+        if derivative:
+            detail["vectors"] = np.stack([eng.debug_read("V", k, (N, 3, D)) for k in range(L + 1)])
     return lines, worst
 
 
