@@ -1,6 +1,7 @@
 #!/usr/bin/env python
-"""Generate ``reference_visnet_mode.npz``: the reference's un-fragmented mode (``--mode visnet``).  Runs ONLY in the
-authoring container (needs the reference tree, like ``make_golden.py``, whose loader and evaluation it reuses).
+"""Generate ``reference_visnet_mode.npz`` and ``reference_visnet_mode_large.npz``: the reference's un-fragmented mode
+(``--mode visnet``).  Runs ONLY in the authoring container (needs the reference tree, like ``make_golden.py``, whose
+loader and evaluation it reuses).
 
     python tests/golden/make_visnet_mode.py
 
@@ -14,11 +15,19 @@ In ``--mode visnet`` the reference feeds the whole input to ViSNet as ONE graph 
                  groups renamed to ACE (CH3, HH31-33, C, O) and NME (N, H, CH3, HH31-33), so that it reads as a capped
                  residue; the protein fields ``c1_names`` / ``c1_resnames`` / ``c1_resnums`` / ``c1_elements`` rebuild it.
 
+and, in ``reference_visnet_mode_large.npz`` (a file of its own, so that the first one stays as it was), the two larger
+example proteins, whose one-graph plans the cases above never select (ABD crosses the 600-atom rule of the tensor-core
+node stage; both run several edge tiles per CTA):
+
+* ``ww``      -- whole WW domain (571 atoms)
+* ``abd``     -- whole ABD (746 atoms)
+
 Per case: ``<key>_z``, ``_pos`` (fp32), ``_batch`` (zeros), ``_slots`` / ``_deg`` (the canonical neighbour slots of
 ``oracle/radius_graph.c``, which the reference's ``radius_graph`` stand-in returns), ``_ref_e`` / ``_ref_f`` (the
 reference's own model source, fp32 CPU, through ``oracle/ref_shims.py``) and ``_e64`` / ``_f64`` (the fp64 oracle).
 In whole proteins most interior atoms have more than 32 atoms within 5 A, so the first-32-by-index cap truncates
-routinely; the script prints the largest candidate count and the number of truncated atoms per case.
+routinely; the script prints the largest candidate count and the number of truncated atoms per case.  Both files are
+byte-identical on every run (the evaluations are deterministic and numpy writes its zip entries without timestamps).
 """
 import os
 import sys
@@ -68,17 +77,8 @@ def c1_input(prot, g=2):
     return CappedProtein(names, resn, np.asarray(resi, dtype=np.int64), elem, pos)
 
 
-def main():
-    sd = O.load_state_dict(CKPT)
-    model = load_reference_model()
-    o64 = O.OracleViSNet(sd, torch.float64)
-    prots = {"chig": read_pdb(f"{REF}/examples/chig.pdb"), "trpcage": read_pdb(f"{REF}/examples/trpcage.pdb")}
-    prots["c1"] = c1_input(prots["trpcage"])
-    try:
-        fragment_protein(prots["c1"])
-        raise AssertionError("the three-residue input was fragmented")
-    except NotImplementedError:
-        pass
+def one_graph_cases(model, o64, prots):
+    """Every field of each case, the whole input as one graph."""
     out = {}
     for key, prot in prots.items():
         fd = whole_input(prot)
@@ -96,10 +96,30 @@ def main():
         print(f"{key}: N={len(fd.z)} E={int(deg.sum())} max candidates within 5 A={int(n_cand.max())} "
               f"truncated atoms={int((n_cand > 32).sum())} maxdeg={int(deg.max())} "
               f"|ref-o64| E {np.abs(e - e64.numpy()).max():.3e} F {np.abs(f - f64.numpy()).max():.3e}")
+    return out
+
+
+def main():
+    sd = O.load_state_dict(CKPT)
+    model = load_reference_model()
+    o64 = O.OracleViSNet(sd, torch.float64)
+    prots = {"chig": read_pdb(f"{REF}/examples/chig.pdb"), "trpcage": read_pdb(f"{REF}/examples/trpcage.pdb")}
+    prots["c1"] = c1_input(prots["trpcage"])
+    try:
+        fragment_protein(prots["c1"])
+        raise AssertionError("the three-residue input was fragmented")
+    except NotImplementedError:
+        pass
+    out = one_graph_cases(model, o64, prots)
     c1 = prots["c1"]
     out.update(c1_names=np.array(c1.names), c1_resnames=np.array(c1.resnames), c1_resnums=c1.resnums,
                c1_elements=np.array(c1.elements))
     np.savez_compressed(os.path.join(HERE, "reference_visnet_mode.npz"), **out)
+    # at these sizes torch's CPU backward splits its scatter-adds over threads, and the reference's fp32 forces then move
+    # by an ulp or two from run to run; one thread keeps the file reproducible
+    torch.set_num_threads(1)
+    large = one_graph_cases(model, o64, {k: read_pdb(f"{REF}/examples/{k}.pdb") for k in ("ww", "abd")})
+    np.savez_compressed(os.path.join(HERE, "reference_visnet_mode_large.npz"), **large)
 
 
 if __name__ == "__main__":

@@ -1,5 +1,6 @@
 """The reference's un-fragmented ``--mode visnet`` input, host side: the golden of tests/golden/make_visnet_mode.py (the
-reference's own model source on whole Chignolin, whole Trp-cage and a three-residue ACE-ALA-NME input, each ONE graph),
+reference's own model source on whole Chignolin, whole Trp-cage, a three-residue ACE-ALA-NME input, whole WW and whole ABD,
+each ONE graph),
 ``pdbfrag.whole_input``, the masses of every element the model accepts, and the hint ``fragment_protein`` gives for
 inputs it cannot fragment."""
 import os
@@ -14,13 +15,19 @@ from ai2bmd_b200.pdbfrag import CappedProtein, fragment_protein, whole_input
 from oracle import visnet_ref as O
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
-CASES = ("chig", "trpcage", "c1")
-N_ATOMS = {"chig": 175, "trpcage": 281, "c1": 22}
+CASES = ("chig", "trpcage", "c1", "ww", "abd")
+PROTEINS = ("chig", "trpcage", "ww", "abd")
+N_ATOMS = {"chig": 175, "trpcage": 281, "c1": 22, "ww": 571, "abd": 746}
 
 
 @pytest.fixture(scope="module")
 def gold():
-    return np.load(os.path.join(GOLDEN, "reference_visnet_mode.npz"))
+    """Both golden files as one mapping: whole WW and ABD are in reference_visnet_mode_large.npz."""
+    out = {}
+    for name in ("reference_visnet_mode.npz", "reference_visnet_mode_large.npz"):
+        with np.load(os.path.join(GOLDEN, name)) as g:
+            out.update({k: g[k] for k in g.files})
+    return out
 
 
 def c1_protein(gold):
@@ -57,7 +64,7 @@ def test_slots_of_the_c_oracle_equal_the_reference(gold, key):
         assert (n_cand > 32).sum() > len(p) // 3
 
 
-@pytest.mark.parametrize("key", ["chig", "trpcage"])
+@pytest.mark.parametrize("key", PROTEINS)
 def test_whole_input_is_one_graph_in_file_order(gold, key):
     prot = load_capped_protein(key)
     fd = whole_input(prot)
@@ -94,9 +101,9 @@ def test_masses_cover_every_element_and_keep_the_old_values():
         elements.atomic_number("Qq")
 
 
-@pytest.mark.parametrize("key", ["c1", "chig"])
+@pytest.mark.parametrize("key", ["c1", "chig", "abd"])
 def test_oracle_matches_the_reference_on_one_graph(real_weights, gold, key):
-    """The fp32 oracle against the reference's own model source, with the neighbour cap truncating (chig)."""
+    """The fp32 oracle against the reference's own model source, with the neighbour cap truncating (chig, abd)."""
     sd = {k: torch.from_numpy(np.asarray(v)) for k, v in real_weights.items()}
     e, f = O.OracleViSNet(sd, torch.float32).energy_and_forces(gold[f"{key}_z"], gold[f"{key}_pos"], gold[f"{key}_batch"])
     ref_e, ref_f = gold[f"{key}_ref_e"], gold[f"{key}_ref_f"]

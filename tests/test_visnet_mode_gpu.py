@@ -383,16 +383,22 @@ def test_loud_refusals(real_weights, gold):
 
 # ---- e. fragment mode did not move -----------------------------------------------------------------------------------
 def _md_step_kernels(dev):
-    """CUDA kernels one direct (uncaptured) MD step launches, counted by torch.profiler."""
+    """CUDA kernels one direct (uncaptured) MD step launches, counted by torch.profiler over two steps: the kernels after
+    the first step's md_kick2_kernel, which ends a step.  Late in a long test process the profiler has lost the first
+    kernels of a session (7 of a whole-WW step's 38, the same count again with 50 ms of idle time before the step; a
+    second session right after counted all 38), so the first step only marks where the counted one begins."""
     from torch.profiler import ProfilerActivity, profile
     dev.engine.set_option("use_graph", 0)
     dev.run(1)
     torch.cuda.synchronize()
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        dev.run(1)
+        dev.run(2)
         torch.cuda.synchronize()
     dev.engine.set_option("use_graph", 1)
-    return sum(1 for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA)
+    ks = sorted((e.time_range.start, e.name) for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA)
+    ends = [i for i, (_, name) in enumerate(ks) if "md_kick2_kernel" in name]
+    assert len(ends) == 2 and ends[1] == len(ks) - 1, [name for _, name in ks]
+    return ends[1] - ends[0]
 
 
 def fragment_plan(real_weights):
