@@ -233,6 +233,10 @@ struct vb_handle {
     unsigned long long* d_stop = nullptr;           // ... and its device address
     std::atomic<unsigned long long> loop_gen{0};    // number of the latest loop launch
     std::atomic<int> comm_world{0};                 // comm.world, readable without the mutex (vb_md_request_stop)
+    // this handle leads a group whose members evaluate its MD step (vb_group_md_run / vb_group_md_eval), until the next
+    // vb_md_setup: its own device loop would integrate its window alone
+    bool md_group = false;
+    int md_group_graph = -1;             // the last group step: 1 one graph over all members, 0 per-member replays
     // Hookean restraints (k_md.cuh MdRestraints): term CSR + rf [3*n_protein + 1] in one allocation
     bool rs_ready = false;
     MdRestraints rs{};
@@ -261,13 +265,18 @@ struct vb_handle {
         err = buf;
     }
     // configuration generation: every call that drops the cached graphs (a topology, window, map, recipe, refinement, MM
-    // term, MD or comm setup, any option) changes what an evaluation computes, so a group (vb_group_*) that checked this
-    // handle at vb_group_create compares it before every call
+    // term, vb_md_setup or comm setup, any option) changes what an evaluation computes, so a group (vb_group_*) that
+    // checked this handle at vb_group_create compares it before every call
     unsigned long long gen = 0;
-    void drop_graph() {
+    // the MD state's own generation: the setters of the noise, normals, restraints and recorder change what the step's
+    // kicks and restraint CTA hold, not what an evaluation computes, so they count here instead; a group that steps this
+    // handle's MD state (vb_group_md_run) captures its step graph again when it changes
+    unsigned long long md_gen = 0;
+    void drop_graph(bool md_state = false) {
         for (auto& g : graphs) cudaGraphExecDestroy(g.exec);
         graphs.clear();
-        gen++;
+        if (md_state) md_gen++;
+        else gen++;
     }
     void free_map() {
         cudaFree(d_map_rowptr); cudaFree(d_map_src); cudaFree(d_map_sign); cudaFree(d_frag_sign); cudaFree(d_ef);
@@ -321,6 +330,8 @@ struct vb_handle {
         cudaFree(d_mx); cudaFree(d_mv); cudaFree(d_mmass); cudaFree(d_ehist); cudaFree(d_step);
         d_mx = d_mv = d_mmass = d_ehist = nullptr; d_step = nullptr;
         md_ready = false;
+        md_group = false;
+        md_group_graph = -1;
         if (md_unfrag) { md_unfrag = false; n_protein = 0; }   // that n_protein came from vb_md_setup, not from a map
     }
     // drop the topology and everything sized by it (the caller has selected the device)
@@ -1047,7 +1058,7 @@ int clean_accumulators(vb_handle* h, cudaStream_t st) {
 }
 
 enum { K_EVAL = 0, K_HOST = 1, K_MD_EVAL = 2, K_MD_STEP = 3, K_ENERGY = 4, K_ENERGY_HOST = 5, K_MD_LOOP = 6, K_FRAG = 7,
-       K_FRAG_HOST = 8, K_FRAG_E = 9, K_FRAG_E_HOST = 10 };
+       K_FRAG_HOST = 8, K_FRAG_E = 9, K_FRAG_E_HOST = 10, K_GROUP_MD = 11 };
 
 // Run `enqueue(stream)` -- a sequence of launches / async copies that depends only on (kind, io) and the handle's
 // configuration -- either directly or as a replay of its cached CUDA graph.  A failed capture always ends the capture
@@ -1811,7 +1822,7 @@ int vb_md_set_normals(vb_handle* h, const double* pool_dev, int64_t pool_steps) 
     }
     h->md.pool = pool_dev;
     h->md.pool_steps = pool_steps;
-    h->drop_graph();              // kernel arguments are baked into the captured step
+    h->drop_graph(true);          // kernel arguments are baked into the captured step
     return VB_OK;
 }
 
@@ -1830,7 +1841,7 @@ int vb_md_set_noise(vb_handle* h, int32_t kind, uint64_t state_hi, uint64_t stat
     }
     CUDA_TRY(h, cudaSetDevice(h->device));
     CUDA_TRY(h, cudaDeviceSynchronize());      // no enqueued step may still use the old buffers
-    h->drop_graph();                           // kick1 holds the noise pointers, both kicks the pool pointer
+    h->drop_graph(true);                       // kick1 holds the noise pointers, both kicks the pool pointer
     if (h->nz.kind == 1) { h->md.pool = nullptr; h->md.pool_steps = 0; }
     h->free_nz();
     if (kind == 0) return VB_OK;
@@ -1919,7 +1930,7 @@ int vb_md_set_recorder(vb_handle* h, int64_t every, int64_t capacity, double run
     }
     CUDA_TRY(h, cudaSetDevice(h->device));
     CUDA_TRY(h, cudaDeviceSynchronize());      // no enqueued step may still write the old ring
-    h->drop_graph();                           // the kicks and the frame copy hold the ring's pointers
+    h->drop_graph(true);                       // the kicks and the frame copy hold the ring's pointers
     h->free_rec();
     if (int rc = md_resync(h)) return rc;
     if (every == 0) return VB_OK;
@@ -2012,7 +2023,7 @@ int vb_md_set_restraints(vb_handle* h, int64_t n_tether, const int32_t* tether_a
     }
     CUDA_TRY(h, cudaSetDevice(h->device));
     CUDA_TRY(h, cudaDeviceSynchronize());
-    h->drop_graph();              // the kick and placement launches hold rf / the term arrays
+    h->drop_graph(true);          // the kick and placement launches hold rf / the term arrays
     h->free_rs();
     if (n_tether == 0 && n_spring == 0) return VB_OK;
     // tethers are anchored where the atoms stand now (the reference re-anchors at the start of every stage)
@@ -2183,6 +2194,11 @@ int vb_md_run_loop(vb_handle* h, int64_t max_steps, void* stream) {
     std::lock_guard<std::mutex> lk(h->mu);
     if (int rc = md_check(h, "vb_md_run_loop")) return rc;
     if (max_steps < 0) { h->set_error("vb_md_run_loop: negative step count"); return VB_ERR_ARG; }
+    if (h->md_group) {
+        h->set_error("vb_md_run_loop: the handle leads a group whose members evaluate its MD step, and the device loop runs one "
+                     "handle's step; use vb_group_md_run");
+        return VB_ERR_STATE;
+    }
     if (h->comm_ready && !h->comm_auto) {
         h->set_error("vb_md_run_loop: the all-reduce of the step is the caller's (option comm_auto = 0), and a host "
                      "all-reduce between the kicks cannot run inside a device loop; use vb_md_kick1 / vb_md_eval / vb_md_kick2");
@@ -2456,6 +2472,9 @@ struct vb_group {
     cudaEvent_t ev_join = nullptr;           // dev[0]: the last join has read the partials
     CommParams join{};                       // comm_allreduce_kernel in gather mode over the partials
     CommParams join_e{};                     // the same over the partials' energy slots [3n] alone (the energy entries)
+    cudaGraphExec_t md_exec = nullptr;       // the group's MD step as one graph over every member's stream (vb_group_md_run)
+    unsigned long long md_exec_gen = 0;      // ... captured at this MD generation of the leader
+    bool md_whole = true;                    // false once that graph failed to capture or instantiate: per-member replays
     void set_error(const char* fmt, ...) {
         char buf[1024];
         va_list ap;
@@ -2562,6 +2581,27 @@ int group_md_sync(vb_group* g, const char* who) {
     return VB_OK;
 }
 
+// On `leader` (dev[0]): the wait for every member's done event, then the rank-order sum of the partials into ef (with
+// `energy`, of their energy slots into ef[0]); copies first the partials dev[0] cannot read in place.
+int group_join(vb_group* g, cudaStream_t leader, float* ef, bool energy) {
+    const int k = (int)g->m.size();
+    const size_t n3 = 3 * (size_t)g->n_protein;
+    const size_t off = energy ? n3 : 0, len = energy ? 1 : n3 + 1;     // the part of each partial the join reads
+    vb_handle* h0 = g->m[0];
+    CUDA_TRY(h0, cudaSetDevice(g->dev[0]));
+    for (int r = 0; r < k; r++) {
+        CUDA_TRY(h0, cudaStreamWaitEvent(leader, g->done[r], 0));
+        if (!g->peer[r])
+            CUDA_TRY(h0, cudaMemcpyPeerAsync(g->d_stage + r * (n3 + 1) + off, g->dev[0], g->m[r]->d_ef + off, g->dev[r],
+                                             sizeof(float) * len, leader));
+    }
+    const long long n = (long long)len;
+    const int ctas = (int)std::max<long long>(1, std::min<long long>((n + COMM_THREADS - 1) / COMM_THREADS, COMM_MAX_CTAS));
+    comm_allreduce_kernel<<<ctas, COMM_THREADS, 0, leader>>>(energy ? g->join_e : g->join, ef, n);
+    CUDA_TRY(h0, cudaGetLastError());
+    return VB_OK;
+}
+
 // One group call enqueued, members locked: positions to every member (host_x: from pinned host memory; else dev_x on
 // dev[0], read in place by the members there and copied peer-to-peer to the others), each member's evaluation into its
 // partial on its own stream, then, on `leader` (dev[0]), the wait for every member and the rank-order join into ef.
@@ -2570,7 +2610,6 @@ int group_md_sync(vb_group* g, const char* who) {
 int group_enqueue(vb_group* g, const double* host_x, const double* dev_x, float* ef, cudaStream_t leader, bool energy = false) {
     const int k = (int)g->m.size();
     const size_t n3 = 3 * (size_t)g->n_protein;
-    const size_t off = energy ? n3 : 0, len = energy ? 1 : n3 + 1;     // the part of each partial the join reads
     vb_handle* h0 = g->m[0];
     CUDA_TRY(h0, cudaSetDevice(g->dev[0]));
     CUDA_TRY(h0, cudaStreamWaitEvent(leader, g->ev_join, 0));   // the last join, on whichever stream, has read the partials
@@ -2597,17 +2636,7 @@ int group_enqueue(vb_group* g, const double* host_x, const double* dev_x, float*
         };
         if ((rc = member())) return member_fail(g, r, rc);
     }
-    CUDA_TRY(h0, cudaSetDevice(g->dev[0]));
-    for (int r = 0; r < k; r++) {
-        CUDA_TRY(h0, cudaStreamWaitEvent(leader, g->done[r], 0));
-        if (!g->peer[r])
-            CUDA_TRY(h0, cudaMemcpyPeerAsync(g->d_stage + r * (n3 + 1) + off, g->dev[0], g->m[r]->d_ef + off, g->dev[r],
-                                             sizeof(float) * len, leader));
-    }
-    const long long n = (long long)len;
-    const int ctas = (int)std::max<long long>(1, std::min<long long>((n + COMM_THREADS - 1) / COMM_THREADS, COMM_MAX_CTAS));
-    comm_allreduce_kernel<<<ctas, COMM_THREADS, 0, leader>>>(energy ? g->join_e : g->join, ef, n);
-    CUDA_TRY(h0, cudaGetLastError());
+    if (int rc = group_join(g, leader, ef, energy)) return member_fail(g, 0, rc);
     CUDA_TRY(h0, cudaEventRecord(g->ev_join, leader));
     return VB_OK;
 }
@@ -2623,6 +2652,7 @@ void vb_group_destroy(vb_group* g) {
         if (!g->dev.empty() && cudaSetDevice(g->dev[0]) == cudaSuccess) {
             if (g->ev_join) cudaEventSynchronize(g->ev_join);     // a device-entry join may still read the staging
             if (g->st) cudaStreamSynchronize(g->st);
+            if (g->md_exec) cudaGraphExecDestroy(g->md_exec);
             cudaFree(g->d_stage); cudaFree(g->d_ef);
             cudaFreeHost(g->h_x); cudaFreeHost(g->h_ef);
             if (g->st) cudaStreamDestroy(g->st);
@@ -2799,6 +2829,210 @@ int vb_group_forward_fragments_energy_host(vb_group* g, const double* prot_pos_h
     return VB_OK;
 }
 
+
+// ---- the device MD step over a group: the members evaluate, the leader integrates --------------------------------------
+// The MD state (vb_md_setup, noise, restraints, recorder) is member 0's.  One step: the leader's kick1; every member reads
+// the leader's fp64 positions (in place on the leader's device, else a peer copy into its d_fx) and runs md_eval_enqueue
+// into its partial on its own stream, the leader with its restraint CTA; the leader's join sums the partials in rank
+// order into the leader's ef; the leader's kick2.  The step is captured once as ONE graph spanning the members' streams
+// (event edges between them, across devices where members sit on several GPUs), so a step costs one host launch where
+// per-member replays cost k + 2 (kick1, k member graphs, the join and kick2 in the leader's order).  When that graph does
+// not capture or instantiate, the group falls back to per-member replays for good; option md_group_graph of the leader
+// says which ran.
+namespace {
+int group_md_check(vb_group* g, const char* who) {
+    vb_handle* h0 = g->m[0];
+    if (h0->md_unfrag) {
+        g->set_error("%s: member 0 leads the step and is set up un-fragmented (vb_md_setup with real_host = NULL): a group "
+                     "steps a fragment batch", who);
+        return VB_ERR_STATE;
+    }
+    if (!h0->md_ready) {
+        g->set_error("%s: member 0 leads the step and has no MD state: call vb_md_setup on it before vb_group_create", who);
+        return VB_ERR_STATE;
+    }
+    for (int r = 0; r < (int)g->m.size(); r++)
+        if (!g->m[r]->derivative) {
+            g->set_error("%s: member %d has option derivative = 0 (no forces)", who, r);
+            return VB_ERR_STATE;
+        }
+    if (int rc = group_check_call(g, who)) return rc;
+    return VB_OK;
+}
+
+// accumulators a truncated vb_debug_run left behind, cleared before a step graph that does not clear them itself
+int group_md_clean(vb_group* g) {
+    for (int r = 0; r < (int)g->m.size(); r++) {
+        vb_handle* h = g->m[r];
+        if (!h->accum_dirty) continue;
+        auto clean = [&]() -> int {
+            CUDA_TRY(h, cudaSetDevice(h->device));
+            if (int rc = clean_accumulators(h, h->own_stream)) return rc;
+            CUDA_TRY(h, cudaStreamSynchronize(h->own_stream));
+            return VB_OK;
+        };
+        if (int rc = clean()) return member_fail(g, r, rc);
+    }
+    return VB_OK;
+}
+
+// One group step (`kicks`) or evaluation enqueued on `leader` (dev[0]) and the members' streams.  `whole`: the members'
+// launches directly (inside the capture of the group's step graph); otherwise each member replays its cached K_GROUP_MD
+// graph.
+int group_md_body(vb_group* g, cudaStream_t leader, bool whole, bool kicks) {
+    const size_t n3 = 3 * (size_t)g->n_protein;
+    vb_handle* h0 = g->m[0];
+    const int d0 = g->dev[0];
+    auto lead = [&]() -> int {
+        CUDA_TRY(h0, cudaSetDevice(d0));
+        if (kicks) {
+            md_kick1_enqueue(h0, leader);
+            CUDA_TRY(h0, cudaGetLastError());
+        }
+        CUDA_TRY(h0, cudaEventRecord(g->ev_start, leader));
+        return VB_OK;
+    };
+    if (int rc = lead()) return member_fail(g, 0, rc);
+    for (int r = 0; r < (int)g->m.size(); r++) {
+        vb_handle* h = g->m[r];
+        const cudaStream_t s = h->own_stream;
+        const bool restrain = r == 0;             // the restraint CTA runs once, with the leader's placement
+        auto member = [&]() -> int {
+            CUDA_TRY(h, cudaSetDevice(h->device));
+            CUDA_TRY(h, cudaStreamWaitEvent(s, g->ev_start, 0));
+            const double* x = h0->d_mx;
+            if (h->device != d0) {
+                CUDA_TRY(h, cudaMemcpyPeerAsync(h->d_fx, h->device, h0->d_mx, d0, sizeof(double) * n3, s));
+                x = h->d_fx;
+            }
+            if (whole) {
+                if (int rc = md_eval_enqueue(h, s, x, h->d_ef, restrain)) return rc;
+            } else {
+                StepIO io = eval_io(h, h->d_ef);
+                io.x = x;
+                if (int rc = run_cached(h, s, K_GROUP_MD, io,
+                                        [&](cudaStream_t q) -> int { return md_eval_enqueue(h, q, x, h->d_ef, restrain); }))
+                    return rc;
+            }
+            CUDA_TRY(h, cudaEventRecord(g->done[r], s));
+            return VB_OK;
+        };
+        if (int rc = member()) return member_fail(g, r, rc);
+    }
+    auto join = [&]() -> int {
+        if (int rc = group_join(g, leader, h0->md_ef, false)) return rc;
+        if (kicks) {
+            md_kick2_enqueue(h0, leader);
+            CUDA_TRY(h0, cudaGetLastError());
+        }
+        return VB_OK;
+    };
+    if (int rc = join()) return member_fail(g, 0, rc);
+    return VB_OK;
+}
+
+// the group's step graph, captured on g->st; on failure the capture is ended and md_whole cleared (the caller replays)
+void group_md_capture(vb_group* g) {
+    vb_handle* h0 = g->m[0];
+    cudaGraph_t graph = nullptr;
+    cudaGraphExec_t exec = nullptr;
+    cudaError_t e_begin = cudaSetDevice(g->dev[0]), e_end = cudaSuccess, e_inst = cudaSuccess;
+    if (e_begin == cudaSuccess) e_begin = cudaStreamBeginCapture(g->st, cudaStreamCaptureModeThreadLocal);
+    int rc = VB_ERR_CUDA;
+    if (e_begin == cudaSuccess) {
+        rc = group_md_body(g, g->st, true, true);
+        cudaSetDevice(g->dev[0]);
+        e_end = cudaStreamEndCapture(g->st, &graph);
+    }
+    if (rc == VB_OK && e_end == cudaSuccess) e_inst = cudaGraphInstantiate(&exec, graph, 0);
+    if (graph) cudaGraphDestroy(graph);
+    if (rc == VB_OK && e_end == cudaSuccess && e_inst == cudaSuccess) {
+        g->md_exec = exec;
+        g->md_exec_gen = h0->md_gen;
+        h0->graph_captures++;
+        return;
+    }
+    (void)cudaGetLastError();
+    g->md_whole = false;
+}
+
+int group_md_step(vb_group* g, cudaStream_t st) {
+    vb_handle* h0 = g->m[0];
+    bool graphs = g->md_whole;
+    for (vb_handle* h : g->m) graphs = graphs && h->use_graph;
+    if (graphs) {
+        if (g->md_exec && g->md_exec_gen != h0->md_gen) { cudaGraphExecDestroy(g->md_exec); g->md_exec = nullptr; }
+        if (!g->md_exec) group_md_capture(g);
+    }
+    if (graphs && g->md_exec) {
+        h0->md_group_graph = 1;
+        auto launch = [&]() -> int {
+            CUDA_TRY(h0, cudaSetDevice(g->dev[0]));
+            CUDA_TRY(h0, cudaGraphLaunch(g->md_exec, st));
+            return VB_OK;
+        };
+        if (int rc = launch()) return member_fail(g, 0, rc);
+        return VB_OK;
+    }
+    h0->md_group_graph = 0;
+    return group_md_body(g, st, false, true);
+}
+
+// the common start of vb_group_md_run / vb_group_md_eval, members locked and checked: the leader's host mirrors, clean
+// accumulators, `st` after the group's last join
+int group_md_begin(vb_group* g, cudaStream_t st) {
+    vb_handle* h0 = g->m[0];
+    auto lead = [&]() -> int {
+        CUDA_TRY(h0, cudaSetDevice(g->dev[0]));
+        if (int rc = md_fresh(h0)) return rc;
+        CUDA_TRY(h0, cudaStreamWaitEvent(st, g->ev_join, 0));
+        return VB_OK;
+    };
+    if (int rc = lead()) return member_fail(g, 0, rc);
+    h0->md_group = true;
+    return group_md_clean(g);
+}
+int group_md_end(vb_group* g, cudaStream_t st) {
+    vb_handle* h0 = g->m[0];
+    auto lead = [&]() -> int {
+        CUDA_TRY(h0, cudaSetDevice(g->dev[0]));
+        CUDA_TRY(h0, cudaEventRecord(g->ev_join, st));
+        return VB_OK;
+    };
+    if (int rc = lead()) return member_fail(g, 0, rc);
+    return VB_OK;
+}
+}  // namespace
+
+int vb_group_md_run(vb_group* g, int64_t n_steps, void* stream) {
+    NvtxRange nvtx_("vb_group_md_run");
+    if (!g) return VB_ERR_ARG;
+    std::lock_guard<std::mutex> lk(g->mu);
+    if (n_steps < 0) { g->set_error("vb_group_md_run: negative step count"); return VB_ERR_ARG; }
+    DeviceRestore restore;
+    auto locks = lock_members(g->m.data(), (int)g->m.size());
+    if (int rc = group_md_check(g, "vb_group_md_run")) return rc;
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (int rc = group_md_begin(g, st)) return rc;
+    for (int64_t s = 0; s < n_steps; s++) {
+        if (int rc = group_md_step(g, st)) return rc;
+        md_count_steps(g->m[0], 1);
+    }
+    return group_md_end(g, st);
+}
+
+int vb_group_md_eval(vb_group* g, void* stream) {
+    NvtxRange nvtx_("vb_group_md_eval");
+    if (!g) return VB_ERR_ARG;
+    std::lock_guard<std::mutex> lk(g->mu);
+    DeviceRestore restore;
+    auto locks = lock_members(g->m.data(), (int)g->m.size());
+    if (int rc = group_md_check(g, "vb_group_md_eval")) return rc;
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (int rc = group_md_begin(g, st)) return rc;
+    if (int rc = group_md_body(g, st, false, false)) return rc;
+    return group_md_end(g, st);
+}
 
 // ---- non-bonded MM term (k_nonbonded.cuh) ----------------------------------------------------------------
 int vb_set_nonbonded(vb_handle* h, int64_t n_protein_atoms, const float* charges_host, const float* sigmas_nm_host,
@@ -3187,6 +3421,7 @@ int64_t vb_get_option(const vb_handle* h, const char* key) {
     if (k == "md_unfragmented") return h->md_unfrag ? 1 : 0;
     if (k == "graph_captures") return h->graph_captures;
     if (k == "md_loop_pdl") return h->loop_pdl;
+    if (k == "md_group_graph") return h->md_group_graph;
     if (k == "batch_atoms") return h->batch_atoms();
     if (k == "batch_first_atom") return h->win_first;
     if (k == "caph_evals") {           // energy evaluations of the last refinement (synchronises)

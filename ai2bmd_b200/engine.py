@@ -48,7 +48,7 @@ EXPORTED_SYMBOLS = [
     "vb_set_fragment_recipe", "vb_forward_fragments", "vb_forward_fragments_host", "vb_set_batch_window",
     "vb_group_create", "vb_group_destroy", "vb_group_last_error", "vb_group_forward_fragments",
     "vb_group_forward_fragments_host", "vb_forward_fragments_energy", "vb_forward_fragments_energy_host",
-    "vb_group_forward_fragments_energy", "vb_group_forward_fragments_energy_host",
+    "vb_group_forward_fragments_energy", "vb_group_forward_fragments_energy_host", "vb_group_md_run", "vb_group_md_eval",
 ]
 
 
@@ -177,6 +177,10 @@ def load_library(path: Optional[str] = None):
     for name in ("vb_forward_fragments_energy", "vb_group_forward_fragments_energy"):
         getattr(lib, name).restype = C.c_int
         getattr(lib, name).argtypes = [vp, vp, vp, vp]
+    lib.vb_group_md_run.restype = C.c_int
+    lib.vb_group_md_run.argtypes = [vp, i64, vp]
+    lib.vb_group_md_eval.restype = C.c_int
+    lib.vb_group_md_eval.argtypes = [vp, vp]
     for name in ("vb_forward_fragments_energy_host", "vb_group_forward_fragments_energy_host"):
         getattr(lib, name).restype = C.c_int
         getattr(lib, name).argtypes = [vp, vp, vp]
@@ -711,6 +715,17 @@ class EngineGroup:
         asynchronous on ``stream_ptr`` (a stream of member 0's device)."""
         self._check(self.lib.vb_group_forward_fragments_energy(self.g, prot_pos_ptr, e_ptr, stream_ptr),
                     "vb_group_forward_fragments_energy")
+
+    # ---- the device MD step over the group: member 0 holds the MD state (its md_* methods), every member evaluates ----
+    def md_run(self, n_steps: int, stream_ptr: int = 0):
+        """``n_steps`` steps of member 0's MD state, each one launch of the group's step graph (vb_group_md_run);
+        asynchronous on ``stream_ptr`` (a stream of member 0's device)."""
+        self._check(self.lib.vb_group_md_run(self.g, int(n_steps), stream_ptr), "vb_group_md_run")
+
+    def md_eval(self, stream_ptr: int = 0):
+        """The step's evaluation at member 0's current positions into member 0's MD buffer, with its restraint forces
+        (vb_group_md_eval); asynchronous on ``stream_ptr``."""
+        self._check(self.lib.vb_group_md_eval(self.g, stream_ptr), "vb_group_md_eval")
 
 
 def tc_selftest(a: np.ndarray, w_nk: np.ndarray, reps: int = 1, device: int = 0, rows: int = 128):

@@ -192,7 +192,10 @@ class DeviceLangevin:
     GPU: ``run(n)`` enqueues n replays of one captured CUDA graph and never touches the host.
 
     With ``group`` (a ``torch.distributed`` process group, one rank per GPU) every rank holds the whole-protein state
-    and its own shard of fragments; the per-step exchange is the one all-reduce of the force/energy buffer."""
+    and its own shard of fragments; the per-step exchange is the one all-reduce of the force/energy buffer.
+    :meth:`grouped` runs the step over several GPUs of ONE process instead (an :class:`ai2bmd_b200.engine.EngineGroup`)."""
+
+    engine_group = None      # grouped(): the EngineGroup whose members evaluate every step of this engine's state
 
     def __init__(self, state_dict, frags: FragmentData, pm: ProteinMap, recipe: FragmentRecipe, positions, numbers,
                  dt_fs=1.0, temperature_K=300.0, friction_per_fs=0.001, seed=0, device: int = 0, velocities=None,
@@ -267,6 +270,57 @@ class DeviceLangevin:
         return self
 
     @classmethod
+    def grouped(cls, state_dict, frags: FragmentData, pm: ProteinMap, recipe: FragmentRecipe, positions, numbers, *,
+                devices, caph=None, nonbonded=None, chunk_atoms: int = 0, dt_fs=1.0, temperature_K=300.0,
+                friction_per_fs=0.001, seed=0, velocities=None, zero_com_momentum=False, step: int = 0,
+                noise: str = "philox", noise_state: int = None):
+        """The step over several GPUs of this process, as the reference's single-process run spreads each step's
+        fragments over its bonded devices (``DLBondedCalculator.calculate``, ``src/Calculators/bonded.py:64-89``).
+        ``devices`` is the list ``FragmentCalculator(devices=...)`` takes (duplicates allowed, e.g. ``["cuda:0"] * 2``),
+        and the window engines are built as it builds them: one per entry on its block of
+        :func:`ai2bmd_b200.parallel.partition_fragments`, each placing and refining the whole batch (``caph``, the whole
+        :class:`ai2bmd_b200.caph.CapHProblem`) and evaluating its block and its rows of the MM term (``nonbonded``).
+        Member 0 (``devices[0]``) holds the MD state and integrates; every step is one launch of the group's step graph
+        (``vb_group_md_run``).  The other keyword arguments are the constructor's.
+
+        ``run``, ``run_observed``, ``preequilibrate``, ``set_restraints``, ``set_normals``, ``state``, ``energy``,
+        ``temperature`` and ``noise_state`` work as on one GPU, on member 0's engine (``self.engine``; the members are
+        ``self.shards``).  ``run_segment`` raises: its device loop runs one engine's step."""
+        from .calculator import _device_index, _device_list
+        from .engine import EngineGroup, check_recipe
+        from .nonbonded import check_parameters
+        from .parallel import DeviceShard, check_shardable
+        if noise not in ("philox", "reference"):
+            raise ValueError(f"noise must be 'philox' or 'reference', not {noise!r}")
+        devs = _device_list(devices)
+        if devs is None:
+            raise ValueError("devices must be a list of devices, e.g. ['cuda:0', 'cuda:1']")
+        check_recipe(recipe.real, recipe.acc, recipe.rem, recipe.blen, len(frags.z))
+        check_shardable(frags, len(devs))
+        if nonbonded is not None:
+            check_parameters(nonbonded, pm.n_protein)
+        import torch
+        self = cls.__new__(cls)
+        self.torch, self.group = torch, None
+        self.n = pm.n_protein
+        self.masses = masses_of(numbers)
+        self.kT = temperature_K * KB
+        self.fr = friction_per_fs / FS
+        self.shards = [DeviceShard(state_dict, frags, pm, r, len(devs), _device_index(d), native_comm=False,
+                                   chunk_atoms=chunk_atoms) for r, d in enumerate(devs)]
+        for sh in self.shards:
+            sh.set_window(frags, pm, recipe, caph=caph, nonbonded=nonbonded)
+        self.engine = self.shards[0].engine
+        dev = torch.device("cuda", self.engine.device)
+        self.ef = torch.zeros(3 * self.n + 1, dtype=torch.float32, device=dev)
+        self.stream = torch.cuda.current_stream(dev)
+        self.engine.md_setup(self.masses, recipe.real, recipe.acc, recipe.rem, recipe.blen, dt_fs * FS, self.kT, self.fr,
+                             seed, self.ef.data_ptr())
+        self.engine_group = EngineGroup([sh.engine for sh in self.shards])     # after md_setup: it replaces the recipe
+        self._start(positions, velocities, seed, step, noise, noise_state, zero_com_momentum)
+        return self
+
+    @classmethod
     def unfragmented(cls, state_dict, numbers, positions, *, dt_fs=1.0, temperature_K=300.0, friction_per_fs=0.001,
                      seed=0, device: int = 0, velocities=None, step: int = 0, noise: str = "philox",
                      noise_state: int = None, chunk_atoms: int = 0, zero_com_momentum=False, group=None):
@@ -334,6 +388,9 @@ class DeviceLangevin:
 
     def _eval(self):
         sp = self.stream.cuda_stream
+        if self.engine_group is not None:
+            self.engine_group.md_eval(sp)
+            return
         self.engine.md_eval(sp)
         if self.group is not None and not self._native_comm:
             self.torch.distributed.all_reduce(self.ef, group=self.group)
@@ -354,6 +411,9 @@ class DeviceLangevin:
 
     def run(self, n_steps: int):
         sp = self.stream.cuda_stream
+        if self.engine_group is not None:                # every member's evaluation inside the group's step graph
+            self.engine_group.md_run(n_steps, sp)
+            return
         if self.group is None or self._native_comm:      # whole step (incl. the all-reduce) = one graph replay
             self.engine.md_run(n_steps, sp)
             return
@@ -375,6 +435,9 @@ class DeviceLangevin:
         n_steps = int(n_steps)
         if n_steps < 0:
             raise ValueError(f"n_steps must be >= 0, not {n_steps}")
+        if self.engine_group is not None:
+            raise ValueError("run_segment's device loop runs one engine's step, and this step spans the members of an "
+                             "EngineGroup; use run_observed (or run)")
         if self.group is not None and not self._native_comm:
             raise ValueError("run_segment needs the engine's own all-reduce inside the step graph: this run all-reduces "
                              "with torch.distributed between the kicks, which cannot run inside a device loop; use run()")

@@ -383,8 +383,8 @@ int vb_set_batch_window(vb_handle* h, int64_t n_batch_atoms, int64_t first_atom)
  * tile the batch contiguously in rank order, MM rows (vb_set_nonbonded's [atom_lo, atom_hi)) set on some members only or
  * not tiling [0, n_protein) in rank order.  VB_ERR_STATE: a member with derivative = 0, un-fragmented, without a topology,
  * protein map or recipe, or connected through vb_comm_connect.  Any later call on a member that drops its cached graphs (a
- * topology, window, map, recipe, refinement, MM term, MD or comm setup, any vb_set_option) makes every later group call
- * fail with VB_ERR_STATE: create the group again.
+ * topology, window, map, recipe, refinement, MM term, vb_md_setup or comm setup, any vb_set_option) makes every later group
+ * call fail with VB_ERR_STATE: create the group again.
  * A group call takes the member mutexes in rank order, may come from any host thread and restores the caller's current
  * device.  It uses each member's workspace: a member with an MD step set up is synchronised first, as
  * vb_forward_fragments_host does; other work of a member must be ordered before the call by its caller. */
@@ -406,6 +406,33 @@ int vb_group_forward_fragments_host(vb_group* g, const double* prot_pos_host, fl
 int vb_group_forward_fragments_energy(vb_group* g, const double* prot_pos_dev, float* energy_dev, void* stream);
 /* The same with HOST buffers, synchronous, with the edge-overflow check of vb_group_forward_fragments_host. */
 int vb_group_forward_fragments_energy_host(vb_group* g, const double* prot_pos_host, float* energy_host);
+
+/* ---- The device MD step over a group: the members evaluate, member 0 integrates ----------------------------------------
+ * The reference's single-process run with its bonded devices, inside the device MD step: one step is member 0's kick1,
+ * every member's evaluation of its block at member 0's positions (what vb_forward_fragments runs, into its partial), the
+ * rank-order join of the partials into member 0's vb_md_setup buffer, and member 0's kick2.  The MD state is member 0's:
+ * positions, velocities, step counter, restraints, frame recorder, runaway guard and noise stream, set up and read with
+ * the vb_md_* entries on member 0 (the whole recipe for vb_md_setup, as vb_set_fragment_recipe takes it on a window).
+ * Members on member 0's device read its positions in place, the others copy them peer to peer first; the restraint CTA
+ * runs with member 0's placement only, so every restraint applies once.  vb_md_setup on member 0 goes BEFORE
+ * vb_group_create (it replaces the recipe, a reconfiguration); vb_md_set_noise, vb_md_set_normals, vb_md_set_restraints,
+ * vb_md_set_recorder and vb_md_set_state change the step, not what a member evaluates, and the group keeps working.
+ * The step is captured once as ONE CUDA graph spanning every member's stream, event edges between them and across
+ * devices, and cached with the group until member 0's MD state is set up anew (vb_get_option "graph_captures" of member 0
+ * counts it): a step is one host launch, where replaying each member's graph would cost k + 2.  If that graph does not
+ * capture or instantiate, the group replays each member's cached evaluation graph between the leader's kicks from then
+ * on; vb_get_option(member 0, "md_group_graph") answers 1 (one graph) or 0 (per-member replays) after a group step, -1
+ * before.  After a runaway halt every later step leaves the state, the counter and the ring as they are, as on one
+ * handle; the members still evaluate at the halted positions, and nothing of it reaches the state.
+ * Refusals (message in vb_group_last_error): VB_ERR_STATE for a member 0 without vb_md_setup or set up un-fragmented, a
+ * member with derivative = 0, a member reconfigured since vb_group_create; VB_ERR_ARG for a negative step count.  Once a
+ * group step or evaluation ran, vb_md_run_loop on member 0 fails with VB_ERR_STATE until its next vb_md_setup: the device
+ * loop runs one handle's step.  Work of the members outside the group is ordered by the caller, as for the group call. */
+/* n_steps whole steps, asynchronous on `stream` (of member 0's device), no host synchronisation. */
+int vb_group_md_run(vb_group* g, int64_t n_steps, void* stream);
+/* The step's evaluation alone at member 0's current positions: every member's partial, the join into member 0's buffer
+ * and the restraint forces; asynchronous on `stream`.  (vb_md_eval of a group.) */
+int vb_group_md_eval(vb_group* g, void* stream);
 
 /* ---- One-shot all-reduce over NVLink peer memory (SURVEY section 8e) ---------------------------------------------
  * One process per GPU.  vb_comm_init allocates this rank's window (2 parities x world slots of max_floats) and returns
@@ -434,7 +461,7 @@ int vb_launches_per_forward(const vb_handle* h);
  * "node_tc" 0/1 node stage on tensor cores (default: from 600 atoms), "node_nb" 0/1/2/3/4/8 nodes per CTA of the SIMT node kernels (0 = the
  * fewest that fit one wave), "krot" 0/1 every CTA of the SIMT node kernels walks the K dimension of its weight chunks from a
  * different row (default 1: the CTAs of a wave otherwise ask the same L2 slices for the same rows at the same time),
- * "embed_batch" -1/0..3 batch variants of the embedding kernels, "comm_auto" 0/1.  vb_get_option also answers "edge_overflow" (1 after a step exceeded a trimmed max_edges),
+ * "embed_batch" -1/0..3 batch variants of the embedding kernels, "comm_auto" 0/1.  vb_get_option also answers "edge_overflow" (1 after a step exceeded a trimmed max_edges), "md_group_graph" (vb_group_md_run),
  * "tile_rows" (planned edges per tile), "gxa_parts" (1: every tensor-core node CTA runs all column chunks of its row tile; 3: one
  * chunk per CTA, dE/dxa arrives as three partials), "comm_ready", "comm_timeouts" (all-reduce flag waits that gave up after
  * their 10 s deadline; once nonzero, vb_comm_allreduce and every vb_md_* call but vb_md_setup and vb_md_get_state fail
